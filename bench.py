@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """Benchmark of the DDPG / TD3 update hot path (BASELINE.json metric:
-"DDPG update-steps/sec @ batch 4096, 1/2/4/8xB200; embed-gather HBM GB/s").
+"DDPG update-steps/sec @ batch 4096, 1/2/4/8xH100; embed-gather HBM GB/s").
 
   python bench.py --gpus N --steps K --warmup W            # this framework (CUDA path), DDPG (BASELINE configs[1])
   python bench.py --algo td3 ...                           # the same line for TD3 (BASELINE configs[2])
   python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on the host cores
-                                                           # (numpy port in oracle/; /root/reference is Python
-                                                           # and does not exist on the GPU box)
+                                                           # (numpy port in oracle/)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as .npy
 
 One "step" = one update (ddpg_update / td3_update) over one synthetic ML-20M-shaped minibatch:
 26,744 items x 128-d table, frame_size 10, 4096 sample rows per GPU, policy step every 10th
@@ -54,7 +54,8 @@ def load_peaks():
         return dict(hbm=float(p["hbm_gbs"]), bf16=float(p["bf16_tflops"]),
                     bf16_sustained=float(p.get("bf16_tflops_sustained", p["bf16_tflops"])), source="measured")
     except Exception:
-        return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, source="fallback")
+        # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+        return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -206,8 +207,7 @@ def cpu_sample(n_rows, algo, seconds_budget, min_steps=10, max_steps=60):
 
 
 def run_reference(args):
-    """`--impl reference`: the reference algorithm on the host CPU (numpy port in oracle/; /root/reference is
-    Python and is not on the GPU box).  Rank 0 only.  Whatever --gpus is, one unit of work is ONE 4096-row
+    """`--impl reference`: the reference algorithm on the host CPU (numpy port in oracle/).  Rank 0 only.  Whatever --gpus is, one unit of work is ONE 4096-row
     minibatch through the update step -- the same unit the CUDA arm's `value` counts -- so the ratio of the two
     arms is like for like at every N."""
     rank = int(os.environ.get("RANK", "0"))
@@ -347,6 +347,21 @@ class Bench:
         return {"ms": rep_ms, "kernels": int(kernels), "loss": loss, "wall_s": wall}
 
 
+def dump_outputs(out_dir, agent, loss):
+    """What a caller of the timed path holds after its last step: the losses update() returned and every parameter of
+    every net (online and target) as the optimizer and the Polyak update left it.  float32 weights, float64 losses;
+    ~7 MB for DDPG at the benchmark's shapes.  The inputs are seeded, so equal arguments give equal inputs."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in loss.items():
+        if isinstance(v, (int, float)):
+            np.save(os.path.join(out_dir, "loss.%s.npy" % k), np.asarray([v], dtype=np.float64))
+    for net_name in sorted(agent.nets):
+        for p_name, p in agent.nets[net_name].named_parameters():
+            arr = p.detach().to("cpu", torch.float32).contiguous().numpy()
+            np.save(os.path.join(out_dir, "%s.%s.npy" % (net_name, p_name)), arr)
+
+
 def summarize(rep_ms, steps, world):
     """steps/s per repeat -> median (whole job: x world 4096-row minibatches), min, max."""
     v = sorted(steps / (m / 1e3) * world for m in rep_ms)
@@ -355,7 +370,7 @@ def summarize(rep_ms, steps, world):
 
 
 def dp_check(dev, rank, world):
-    """N > 1 only (the driver's GPU test box has one GPU): three parity-mode DDPG steps (SGD, replayed dropout
+    """N > 1 only: three parity-mode DDPG steps (SGD, replayed dropout
     masks) on a small canonical-shape case, rows sharded over the ranks with the peer-memory all-reduce, checked
     (1) replicas bit-identical after the steps and (2) equal to the SAME steps run unsharded on one GPU
     (losses 1e-5 relative; every weight within 2e-3 of the largest weight change + 1e-5 relative).  Raises on failure."""
@@ -456,6 +471,8 @@ def run_native(args):
         sampler.start()
     r_dev = main.run(False, steps, warmup, repeats)
     clocks = sampler.stop() if rank == 0 else {}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, main.agent, r_dev["loss"])
     r_e2e = main.run(True, steps, 3, repeats)
     r_warm = main.run(False, steps, 3, 1, flush_l2=False)
     value, spread = summarize(r_dev["ms"], steps, world)
@@ -467,7 +484,7 @@ def run_native(args):
     strong = None
     if STRONG_ROWS % world == 0:
         sb = Bench("ddpg", STRONG_ROWS // world, dev, rank, world, data_parallel=True, flush=main.flush)
-        k = min(steps, 50)
+        k = steps
         r = sb.run(False, k, 3, 3)
         sv, ss = summarize(r["ms"], k, 1)
         strong = {"workload": "DDPG batch %d rows sharded over %d GPU(s) (BASELINE configs[3])" % (STRONG_ROWS, world),
@@ -499,7 +516,7 @@ def run_native(args):
 
         def graph_time(fns, reps=10):
             """Average DEVICE time of one launch: the launches `fns` (each on its own operands, together larger than
-            the 126 MB L2, so no launch finds its streamed operand cached) are captured into one CUDA graph and the
+            the 50 MB L2, so no launch finds its streamed operand cached) are captured into one CUDA graph and the
             graph is replayed `reps` times between two events.  Unlike an event pair around a single host launch this
             contains no host-side launch preparation (tensor-map encoding) and is not limited by the ~2 us event
             resolution; it does contain the inter-kernel gaps, as the step's own graph does."""
@@ -560,7 +577,7 @@ def run_native(args):
         gather_big_gbs = big * GATHER_BYTES_PER_ROW / (gather_big_ms * 1e-3) / 1e9
         del gb_state, gb_next, gb_act, gb_rew, gb_items, gb_ratings
         # (2) the dominant kernel of the step: layer-1 forward GEMM [4096,1290] x [1290,256]
-        #     (same tcgen05 3xTF32 kernel and operand pitches as inside the step; plain-store epilogue).
+        #     (same wgmma 3xTF32 kernel and operand pitches as inside the step; plain-store epilogue).
         #     Eight launches on eight different state images (8 x 21 MB > L2) in one graph: average device time.
         ld_s = (S_DIM + 3) // 4 * 4
         x_imgs = [torch.randn(n_rows, ld_s, device=dev) for _ in range(8)]
@@ -595,7 +612,7 @@ def run_native(args):
         if world == 1 and not args.no_other_algo:
             oa = "td3" if algo == "ddpg" else "ddpg"
             ob = Bench(oa, n_rows, dev, rank, 1, data_parallel=False, flush=flush)
-            k = min(steps, 100)
+            k = steps
             ro = ob.run(False, k, 3, 3)
             ro_e2e = ob.run(True, k, 3, 3)
             ov, osp = summarize(ro["ms"], k, 1)
@@ -626,7 +643,7 @@ def run_native(args):
                        "dropout": "on (device Philox)", "l2": "flushed between timed steps (256 MB write)",
                        "timing": "both graph variants primed before the timed region; %d repeats of %d steps, median" % (repeats, steps),
                        "inputs": "items/ratings/done resident in HBM; frames gathered on device inside the step",
-                       "matmul": "tcgen05 3xTF32 (error-compensated, fp32-grade) with fp32 CUDA-core fallbacks for the 256->1 head"},
+                       "matmul": "wgmma 3xTF32 (error-compensated, fp32-grade) with fp32 CUDA-core fallbacks for the 256->1 head"},
             "spread": spread,
             "optimizer_updates_per_sec": updates_per_sec,
             "rows_per_sec": updates_per_sec * rows_global,
@@ -639,23 +656,21 @@ def run_native(args):
                     "h2d_bytes_per_step": int(n_rows * ((FRAME + 1) * 12 + 4)), "d2h_bytes_per_step": 32,
                     "what": "%s_update(batch of pinned host items/ratings/done) -> dict of python floats" % algo},
             "gpu_launches": int(r_dev["kernels"]),
-            "roofline": {"bound": "tensor", "kernel": "layer-1 forward GEMM [4096x1290]x[1290x256] (tc_gemm_kernel, tcgen05 kind::tf32, 3 MMA passes/product)",
+            "roofline": {"bound": "tensor", "kernel": "layer-1 forward GEMM [4096x1290]x[1290x256] (tc_gemm_kernel, wgmma tf32, 3 MMA passes/product)",
                          "achieved": 3.0 * l1_tflops, "algorithmic_fp32": l1_tflops, "peak": tf32_peak, "unit": "TFLOP/s",
                          "frac": 3.0 * l1_tflops / tf32_peak,
-                         "traffic": 22518784, "traffic_source": "dram__bytes_read+write per launch, profiles/r2k/r2k_tc_gemm_raw.csv (ncu --set full)", "peak_source": "%s bf16 %.0f TF/s / 2 (TF32 kind)" % (peaks["source"], peaks["bf16"]),
+                         "peak_source": "%s bf16 %.0f TF/s / 2 (TF32 kind)" % (peaks["source"], peaks["bf16"]),
                          "ms": l1_ms, "tile_n": best_tile, "per_tile": {str(k): v for k, v in l1.items()},
                          "timing": "8 launches on 8 distinct state images (8 x 21 MB > L2) captured in one CUDA graph, "
                                    "replayed 10x between CUDA events, L2 flushed between replays; median per launch",
                          "ms_single_launch_between_events": l1_single_ms},
             "roofline_gather": {"bound": "hbm", "kernel": "frame_gather_kernel", "achieved": gather_gbs,
                                 "peak": peaks["hbm"], "unit": "GB/s", "frac": gather_gbs / peaks["hbm"],
-                                "traffic": 12184064, "traffic_source": "dram__bytes_read+write per launch, profiles/r2k/r2k_gather_raw.csv: the 44 MB of "
-                                "output is absorbed by the 126 MB L2 inside the kernel, so DRAM traffic << algorithmic bytes", "peak_source": peaks["source"], "ms": gather_ms, "ms_min": gather_ms_min, "ms_max": gather_ms_max,
+                                "peak_source": peaks["source"], "ms": gather_ms, "ms_min": gather_ms_min, "ms_max": gather_ms_max,
                                 "ms_single_launch_between_events": gather_single_ms,
                                 "timing": "4 launches (own ids / outputs, 4 x 44 MB > L2) in one CUDA graph, replayed 10x between events; median per launch",
                                 "bytes_per_launch": n_rows * GATHER_BYTES_PER_ROW,
                                 "at_16x_rows": {"rows": big, "ms": gather_big_ms, "algorithmic_gbs": gather_big_gbs,
-                                                "traffic": 710117376, "traffic_source": "profiles/r2k/r2k_gather_big_raw.csv (58.2 MB read + 651.9 MB written)",
                                                 "dram_gbs_est": (big * 10840 + N_ITEMS * DIM * 4) / (gather_big_ms * 1e-3) / 1e9,
                                                 "dram_frac_est": (big * 10840 + N_ITEMS * DIM * 4) / (gather_big_ms * 1e-3) / 1e9 / peaks["hbm"],
                                                 "note": "same kernel, 16x the rows: the 710 MB of output no longer fits in L2 and goes to HBM, "
@@ -780,7 +795,7 @@ def bench_device_feed(main, time_kernel, steps):
     ids_ms = time_kernel(lambda: feed.windows(w))
     users32 = list(range(0, 32 * 8, 8))                    # 32 users x 128 windows = 4096 rows
     users_ms = time_kernel(lambda: feed.batch(users32))
-    k = min(steps, 100)
+    k = steps
     r = main.run(False, k, 3, 3, batch_fn=lambda: feed.sample(n_rows))   # randint + window gather + fused step + loss read-back
     v, sp = summarize(r["ms"], k, 1)
     return {"what": "update step fed by DeviceFrameFeed.sample(4096): windows cut on the device from resident "
@@ -802,10 +817,12 @@ def main():
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the cpu_baseline legs (A/B runs)")
     ap.add_argument("--no-other-algo", action="store_true", help="skip the sub-object of the other algorithm")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's losses and updated weights as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
-        if args.steps > 40:          # bounded: the CPU port does ~3-10 steps/s
-            args.steps = 40
         args.warmup = min(args.warmup, 3)
         run_reference(args)
     else:

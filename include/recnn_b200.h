@@ -1,5 +1,5 @@
 /*
- * recnn_b200 -- C ABI of the B200-native RecNN DDPG/TD3 update hot path.
+ * recnn_b200 -- C ABI of the H100-native RecNN DDPG/TD3 update hot path.
  *
  * The reference (awarebayes/RecNN) is pure Python on PyTorch and has NO FFI:
  * its seams for this path are Python call sites (SURVEY.md 8b).  Each entry
@@ -160,7 +160,7 @@ RECNN_API int recnn_linear_forward(const float* x, int64_t n_rows, int in_dim, c
 /* Generic contraction C[M,N] (pitch ldc) = A . B^T, the building block of every Linear
  * forward/backward in this path (torch addmm sites: recnn/nn/models.py:66-70, :207-212 and
  * their autograd backward).  a_mn=0: A is [M,K] row-major, a_mn=1: A is stored [K,M];
- * same for B with N.  recnn_gemm_tf32x3 runs on the tcgen05 tensor cores with
+ * same for B with N.  recnn_gemm_tf32x3 runs on the Hopper tensor cores (wgmma) with
  * error-compensated 3xTF32 (fp32-grade accuracy; pitches and bases must be 16-byte
  * multiples; tile_n in {0 (auto), 64, 128}); recnn_gemm_fp32 is the exact-fp32
  * CUDA-core path for arbitrary shapes. */

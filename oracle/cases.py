@@ -32,6 +32,20 @@ CASES = {
 FULL_SPEC = dict(seeds={"ddpg": 11, "td3": 12}, n_items=26744, dim=128, frame=10, hidden=256, n_rows=4096,
                  steps=3, actor_init_w=6e-1, critic_init_w=54e-2)
 
+
+def _unscreened(seed, **kw):
+    base = dict(CASES["tiny"], steps=12)
+    base["seeds"] = {"ddpg": seed, "td3": seed + 1}
+    base.update(kw)
+    return base
+
+
+# Differential cases on seeds that were NOT screened by find_seeds.py (a case with an ambiguous gate is skipped by
+# its test): the reference's results are stored as tests/golden/unscreened_<id>_<algo>_<opt>.npz.
+UNSCREENED = {"tiny-a": _unscreened(1001),
+              "narrow": _unscreened(1002, n_rows=17, dim=8, frame=3, hidden=16, n_items=40),
+              "wide": _unscreened(1003, n_rows=40, hidden=64)}
+
 DDPG_PARAMS = dict(gamma=0.99, min_value=-10, max_value=10, policy_step=10, soft_tau=0.001)  # algo.py:103-109
 TD3_PARAMS = dict(gamma=0.99, noise_std=0.5, noise_clip=3, soft_tau=0.001, policy_update=10)  # algo.py:164-174
 

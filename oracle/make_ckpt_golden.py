@@ -10,10 +10,12 @@ available offline, so the fixture is the same artefact made here: state_dicts of
 reference does, plus eval-mode inputs and the REFERENCE's forward outputs on them.
 tests/test_checkpoint_compat.py loads the file into recnn_b200.nn.Actor / Critic (CUDA forward must reproduce the
 stored outputs) and checks that a state_dict saved by recnn_b200 loads back into the reference classes (same keys,
-shapes, dtypes, contiguous tensors).
+shapes, dtypes, contiguous tensors).  ``ref_state_dict_layout.json`` records, independently of that file, the key order,
+shapes and dtypes of freshly built reference Actor / Critic objects (the fixture's dims and the published 1290/128/256).
 """
 from __future__ import annotations
 
+import json
 import os
 import sys
 
@@ -30,8 +32,27 @@ OUT = os.path.join(ROOT, "tests", "golden", "ref_checkpoint.pt")
 S, A, H, N = 44, 8, 32, 19          # state = frame 4 x dim 10 + 4, hidden 32
 
 
+LAYOUT = os.path.join(ROOT, "tests", "golden", "ref_state_dict_layout.json")
+LAYOUT_DIMS = ((S, A, H), (1290, 128, 256))     # the fixture's dims and the published model's
+
+
+def state_dict_layout(recnn):
+    """Key order, shape and dtype of the state_dict of freshly built reference Actor / Critic objects: what their
+    load_state_dict(strict=True) accepts."""
+    out = {}
+    for s_dim, a_dim, h in LAYOUT_DIMS:
+        for name, cls in (("actor", recnn.nn.models.Actor), ("critic", recnn.nn.models.Critic)):
+            sd = cls(s_dim, a_dim, h).state_dict()
+            out["%s %d %d %d" % (name, s_dim, a_dim, h)] = [[k, list(v.shape), str(v.dtype)] for k, v in sd.items()]
+    return out
+
+
 def main():
     recnn = import_reference()
+    with open(LAYOUT, "w") as fh:
+        json.dump(state_dict_layout(recnn), fh, indent=1)
+        fh.write("\n")
+    print("wrote", LAYOUT)
     torch.manual_seed(20260923)
     actor = recnn.nn.models.Actor(S, A, H, 6e-1).eval()
     critic = recnn.nn.models.Critic(S, A, H, 54e-2).eval()

@@ -217,6 +217,24 @@ def run_gather_case(recnn):
     return out
 
 
+def run_random_users_gather_case(recnn):
+    """prepare_batch_static_size on five random users (frame 7, a 90 x 12 table): inputs and outputs."""
+    rng = np.random.default_rng(31)
+    frame = 7
+    table = rng.standard_normal((90, 12), dtype=np.float32)
+    users = [{"items": rng.integers(0, 90, size=n, dtype=np.int64), "rates": rng.standard_normal(n) * 2,
+              "sizes": n, "users": 5 + i} for i, n in enumerate((8, 30, 9, 8, 21))]
+    got = recnn.data.utils.prepare_batch_static_size(copy.deepcopy(users), torch.from_numpy(table), frame_size=frame)
+    out = {"table": table, "frame_size": np.int64(frame)}
+    for i, u in enumerate(users):
+        out["user%d.items" % i] = u["items"]
+        out["user%d.rates" % i] = u["rates"]
+        out["user%d.id" % i] = np.int64(u["users"])
+    for k in ("state", "next_state", "action", "reward", "done"):
+        out["out." + k] = got[k].numpy()
+    return out
+
+
 COLLATE_LENGTHS = (11, 12, 30, 11, 57, 13, 100, 25, 11, 19, 64, 33, 12, 47)
 COLLATE_MINIBATCH = (9, 0, 13, 4, 3, 6)      # positions in storage order, as a shuffling DataLoader would pick
 
@@ -315,11 +333,25 @@ def main():
     if not only or "collate" in only:
         np.savez_compressed(os.path.join(GOLDEN_DIR, "collate.npz"), **run_collate_case(recnn))
         print("wrote collate.npz")
-    if only and "gather" not in only and "update" not in only:
+    if only and not only & {"gather", "update", "unscreened"}:
         return
     if not only or "gather" in only:
         np.savez_compressed(os.path.join(GOLDEN_DIR, "gather.npz"), **run_gather_case(recnn))
         print("wrote gather.npz")
+    if not only or "unscreened" in only:
+        np.savez_compressed(os.path.join(GOLDEN_DIR, "gather_random_users.npz"), **run_random_users_gather_case(recnn))
+        for cid, spec in C.UNSCREENED.items():
+            for algo in ("ddpg", "td3"):
+                for opt_kind in ("adam", "sgd"):
+                    name = "unscreened_%s_%s_%s.npz" % (cid, algo, opt_kind)
+                    out = run_update_case(recnn, spec, algo, opt_kind)
+                    # what tests._golden.compare_with_golden reads (every snapshot of SNAP_AFTER)
+                    snaps = tuple("after%d." % n for n in SNAP_AFTER)
+                    keep = {k: v for k, v in out.items()
+                            if k in ("input_checksums", "gate_margin") or k.startswith(("loss.", "noise."))
+                            or (k.endswith(".sample") and k.startswith(("init.", "grad_") + snaps))}
+                    np.savez_compressed(os.path.join(GOLDEN_DIR, name), **keep)
+                    print("wrote", name)
     if only and "update" not in only:
         return
     for case in C.CASES:

@@ -1,4 +1,4 @@
-"""recnn_b200: B200-native implementation of RecNN's DDPG/TD3 update hot path
+"""recnn_b200: H100-native implementation of RecNN's DDPG/TD3 update hot path
 (gather -> Actor/Critic forward+backward -> losses -> optimizer -> Polyak), behind
 RecNN's own Python API.  See DESIGN.md for scope and INTEGRATION.md for drop-in use.
 """
@@ -10,7 +10,7 @@ __version__ = "0.1.0"
 def install_as_recnn():
     """Register this package under the reference's import names (``recnn``,
     ``recnn.nn``, ``recnn.nn.update``, ``recnn.data``, ``recnn.utils`` ...) so code
-    written against awarebayes/RecNN resolves to the B200 path for the hot-path
+    written against awarebayes/RecNN resolves to the H100 path for the hot-path
     symbols.  Raises if the real ``recnn`` is already imported."""
     import sys
     existing = sys.modules.get("recnn")

@@ -7,8 +7,7 @@
 // kernel per gradient arena does a TWO-SHOT all-reduce made of remote STORES only, in the style of NCCL's
 // low-latency protocol: every payload float travels as an 8-byte word {value, epoch}, so the receiver polls
 // the payload itself -- there are no flags, no system-scope fences and no arrival counters on the path
-// (r2m8 / r2m2b measured what those cost: a flag-and-fence version of this kernel took 31-47 us for a 16-byte
-// payload and 46-63 us for a 1.7 MB arena at 4-8 ranks; NCCL's own all_reduce 18 / 23-33 us).
+// (a system fence and a flag per peer and step cost more latency than the small payloads take to move).
 //
 //   A  reduce-scatter, push side: rank r owns slice r of the arena.  Every rank sums its split-K partials on the
 //      fly (GradSource) and stores slice s of its gradient into rank s's contribution buffer [my rank], plus its few
@@ -303,7 +302,12 @@ int launch_comm_allreduce(const recnn_comm* comm, float* buf, int64_t n, const C
   if (r.src) gsrc = *r.src;
   const int64_t per = (int64_t)kCommThreads * 8;                   // eight floats per thread
   int64_t blocks = ceil_div(n, per);
-  const int grid = (int)(blocks < 1 ? 1 : (blocks > kNumSMs ? kNumSMs : blocks));
+  // every CTA must be resident at once: at most one per SM of THIS device (and no more than the L1-partials array holds)
+  int dev = 0, sms = 0;
+  RECNN_CHECK_CUDA(cudaGetDevice(&dev));
+  RECNN_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int cap = sms < kNumSMs ? sms : kNumSMs;
+  const int grid = (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
   // partial-sourced gradients are read four at a time: the arena case (n % 4 == 0, 16-byte aligned)
   const bool vec = (n & 1) == 0 && ((reinterpret_cast<uintptr_t>(buf) & 7) == 0) &&
                    (!r.src || ((n & 3) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0));

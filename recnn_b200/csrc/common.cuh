@@ -1,4 +1,4 @@
-// Shared device/host helpers for the recnn_b200 kernels (sm_100a only).
+// Shared device/host helpers for the recnn_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,7 +47,7 @@ void count_launch();   // every kernel launch of this library bumps a process-wi
     if (_s != RECNN_OK) return _s;                                                    \
   } while (0)
 
-constexpr int kNumSMs = 148;   // B200
+constexpr int kNumSMs = 132;   // H100 SXM: grid caps; kernels that need every CTA resident query the device
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }

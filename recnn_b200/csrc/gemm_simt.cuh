@@ -2,7 +2,7 @@
 //
 // Role in the design (DESIGN.md "kernels"): exact-fp32 building block for every
 // contraction of the update step.  It is the arbitrary-shape path (any S/A/H,
-// any row count) and the on-device reference the tcgen05 3xTF32 kernels are
+// any row count) and the on-device reference the wgmma 3xTF32 kernels are
 // unit-tested against.  C[m,n] = sum_k A(m,k) * B(n,k) with both operands given
 // as "views" so the reference's torch.cat([state, action], 1)
 // (recnn/nn/models.py:207) and the bias column of a weight-gradient never have

@@ -316,7 +316,7 @@ int launch_zero_pad_columns(float* b0, float* b1, float* b2, int64_t n_rows, int
   if (n_rows <= 0) return RECNN_OK;
   const int64_t total = n_rows * (ld - cols);
   const int64_t blocks = ceil_div(total, 256);
-  dim3 grid((unsigned)(blocks < 148 ? blocks : 148), 3);
+  dim3 grid((unsigned)(blocks < kNumSMs ? blocks : kNumSMs), 3);
   zero_pad_columns_kernel<<<grid, 256, 0, st>>>(b0, b1, b2, n_rows, ld, lead, cols);
   RECNN_CHECK_LAUNCH("zero_pad_columns_kernel");
   return RECNN_OK;

@@ -119,7 +119,7 @@ struct ValueHeadArgs {
   float* gw3;                        // [H] gradient of the head weights
   float* gb3;                        // [1]
   float* loss;
-  float* block_partials;             // >= 148 * (H + 2) floats
+  float* block_partials;             // >= kNumSMs * (H + 2) floats
   unsigned* ticket;
 };
 bool value_head_fusable(int hidden);

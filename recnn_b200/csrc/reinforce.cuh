@@ -3,7 +3,7 @@
 // Restates, for one GPU, recnn/nn/models.py:76-184 (DiscreteActor: forward, Categorical sampling, log-probs, importance
 // correction, lambda_K) and recnn/nn/update/reinforce.py:10-65 (ChooseREINFORCE: the three policy losses and their
 // backward).  Included at the end of step.cu: it is built from the same four contraction helpers as the DDPG / TD3 step
-// (hidden_layer, linear_out, backprop_hidden, weight_grad -> tcgen05 3xTF32 GEMMs) plus three row kernels.
+// (hidden_layer, linear_out, backprop_hidden, weight_grad -> wgmma 3xTF32 GEMMs) plus three row kernels.
 //
 // What is different from the reference's formulation:
 //   * the reference keeps one autograd graph per env step (saved_log_probs, models.py:110,156,183) and back-propagates

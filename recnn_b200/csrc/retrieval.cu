@@ -3,8 +3,8 @@
 // matrix; recnn/data/db_con.py:45-56: MilvusConnection.search(search_vecs, topk)).
 //
 //   scores[q, j] = <query_q, item_j>            one [Q, D] x [D, n_items] contraction on the tensor cores
-//                                               (tcgen05 3xTF32, the update step's own GEMM kernel), in slabs
-//                                               of query rows so that a slab of scores stays inside the 126 MB L2
+//                                               (wgmma 3xTF32, the update step's own GEMM kernel), in slabs
+//                                               of query rows so that a slab of scores stays inside the 50 MB L2
 //   key[q, j]    = |item_j|^2 - 2 scores        L2   (+ |query_q|^2 at the end: the squared distance faiss/Milvus report)
 //                = -scores                      IP   (larger inner product = better)
 //                = -scores / |item_j|           COS  (/ |query_q| at the end)
@@ -168,9 +168,10 @@ static int topk_splits(int64_t n_queries, int64_t n_items) {
   return (int)(s < 1 ? 1 : s);
 }
 static int64_t slab_rows(int64_t n_items) {
-  // a slab of scores should stay L2-resident between the GEMM that writes it and the top-k pass that reads it
+  // a slab of scores should stay L2-resident between the GEMM that writes it and the top-k pass that reads it:
+  // 32 MB of the H100's 50 MB L2, leaving room for the item table, its norms and the top-k partials
   const int64_t ld = round_up(n_items, 4);
-  int64_t r = (96ll << 20) / (ld * 4);
+  int64_t r = (32ll << 20) / (ld * 4);
   r = r / 128 * 128;
   return r < 128 ? 128 : (r > 4096 ? 4096 : r);
 }

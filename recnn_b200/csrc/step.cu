@@ -7,7 +7,7 @@
 //
 // Every contraction goes through one of four helpers (hidden_layer, linear_out,
 // backprop_hidden, weight_grad).  Each has two back ends with identical
-// semantics: the tcgen05 3xTF32 tensor-core kernel (tc_gemm.cuh; default) and
+// semantics: the wgmma 3xTF32 tensor-core kernel (tc_gemm.cuh; default) and
 // the exact-fp32 CUDA-core kernel (gemm_simt.cuh; arbitrary shapes, and
 // RECNN_B200_MATH=simt forces it for A/B comparisons).
 #include <stdlib.h>
@@ -37,7 +37,7 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 // ---------------------------------------------------------------- intra-step concurrency
 // The three forward chains at the head of a step are independent: (T) target policy -> target critic
 // -> TD target, (V) online critic forward, (P) online policy forward.  Each GEMM fills at most 64-128
-// of the 148 SMs, so they are issued on three streams (fork/join with events; capturable into the
+// of the 132 SMs, so they are issued on three streams (fork/join with events; capturable into the
 // step's CUDA graph).  RECNN_B200_OVERLAP=0 serialises everything on the caller's stream.
 struct AuxStreams {
   cudaStream_t sv, sp, sw;
@@ -91,8 +91,8 @@ struct Workspace {
 // split count of a weight-gradient GEMM dW[C, K] = dZ^T X over n_rows (the contraction dim).
 // Must be a pure function of the shapes: the workspace size depends on it.
 // The tensor-core kernel holds one CTA per SM and has a fixed cost of several microseconds, so more CTAs than SMs
-// means a second wave of the whole fixed cost (measured in round 1: the critic's dW1 as 22+4 tiles x 8 splits = 208
-// CTAs took 48 us = two waves); aim at ONE wave of ~132 CTAs, leaving room for the GEMM that runs beside it.
+// means a second wave of the whole fixed cost; aim at ONE wave of ~132 CTAs, leaving room for the GEMM that runs
+// beside it.
 static int dw_splits(int C, int K, int64_t n_rows, bool tc_path, int bn = 128) {
   if (tc_path) {
     const int64_t tiles = ceil_div(C, 128) * ceil_div(K, bn);
@@ -508,7 +508,7 @@ static int phase_value_grad(Ctx& c) {
     const Seg sc1 = {c1, H, H, 0}, ss = {c.S, S, c.ldS, 0}, sa = {c.ACT, A + c.lead, c.ldA, c.lead};
     // When this call also runs the built-in optimizer, the split-K partials of layers 1-2 are not reduced by
     // kernels of their own: the optimizer (or the data-parallel all-reduce) pass sums them (GradSource).
-    // (r2i A/B against separate reduce kernels: 2708 vs 2711 steps/s -- kept for the three launches it saves)
+    // (no slower than separate reduce kernels, and three launches fewer)
     const bool fuse_opt = (a.phases & RECNN_PH_VALUE_OPT) && a.value_optim.kind != RECNN_OPT_EXTERNAL;
     GradSource gs;
     memset(&gs, 0, sizeof(gs));
@@ -760,7 +760,7 @@ static int run_step(const recnn_step_args* a, int algo, void* stream) {
       c.v1_prefetched = true;
     }
     // chain P is forked later (after the target policy's hidden layers, see phase_value_grad): three
-    // concurrent layer-1 GEMMs are 192 CTAs = two waves on 148 SMs, two are one wave
+    // concurrent layer-1 GEMMs are 192 CTAs = two waves on 132 SMs, two are one wave
     c.p_deferred = (a->phases & RECNN_PH_POLICY_LOSS) != 0;
   }
   if (a->phases & RECNN_PH_VALUE_GRAD) RECNN_PROPAGATE(phase_value_grad(c));
@@ -820,8 +820,7 @@ extern "C" int recnn_net_layout(const recnn_dims* d, int is_critic, int64_t* out
 
 // Inference entry points take densely packed inputs ([n, S] / [n, A]).  A row pitch that is not a 16-byte
 // multiple (S = 1290) cannot be a TMA tensor, so the inputs are first re-pitched into scratch images (one 2-D
-// device copy each, 21 MB at 4096 rows) and every layer runs on the tcgen05 path -- the CUDA-core kernel took
-// 62 us per layer-1 launch at this shape, 30x a tensor-core launch.
+// device copy each, 21 MB at 4096 rows) and every layer runs on the tensor-core path rather than the much slower CUDA-core kernel.
 extern "C" int64_t recnn_forward_scratch_floats(const recnn_dims* d, int64_t n_rows, int is_critic) {
   if (!d || n_rows <= 0) return 0;
   const int64_t ldS = pad4(d->state_dim), ldA = pad4(d->action_dim + d->state_dim % 4);

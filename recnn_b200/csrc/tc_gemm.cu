@@ -1,4 +1,4 @@
-// Host side of the tcgen05 3xTF32 GEMM: tensor-map construction, launch
+// Host side of the wgmma 3xTF32 GEMM: tensor-map construction, launch
 // configuration, and the generic C-ABI entry points recnn_gemm_tf32x3 / recnn_gemm_fp32.
 #include "tc_gemm.cuh"
 
@@ -32,13 +32,12 @@ int make_tmap(CUtensorMap* out, const float* base, int64_t rows, int64_t cols, i
   }
   RECNN_REQUIRE(reinterpret_cast<uintptr_t>(base) % 16 == 0, "TMA base must be 16-byte aligned");
   RECNN_REQUIRE(ld % 4 == 0 && ld >= cols, "TMA row pitch must be a multiple of 4 floats");
-  RECNN_REQUIRE(box_cols * 4 <= (swizzle_bytes == 1032 ? 128 : swizzle_bytes) && box_rows <= 256, "TMA box");
+  RECNN_REQUIRE(box_cols * 4 <= swizzle_bytes && box_rows <= 256, "TMA box");
   const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   const cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
   const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapSwizzle sw = swizzle_bytes == 1032 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-                               : swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+  const CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                                                      : CU_TENSOR_MAP_SWIZZLE_32B;
   const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
@@ -74,16 +73,16 @@ static int launch_cfg(const Operand& A0, const Operand& A1, const Operand& B, co
   CUtensorMap ma0, ma1, mb;
   // K-major operand: tensor [rows = M|N, cols = K], box {BK, tile rows}; MN-major: tensor [rows = K, cols = M|N], box {32, BK}
   if (!C::A_MN) {
-    RECNN_PROPAGATE(make_tmap(&ma0, A0.ptr, p.M, p.K0, A0.ld, C::BK, C::BM, C::K_SWZ));
-    if (p.K1 > 0) RECNN_PROPAGATE(make_tmap(&ma1, A1.ptr, p.M, p.K1, A1.ld, C::BK, C::BM, C::K_SWZ));
+    RECNN_PROPAGATE(make_tmap(&ma0, A0.ptr, p.M, p.K0, A0.ld, C::BK, C::BM, 128));
+    if (p.K1 > 0) RECNN_PROPAGATE(make_tmap(&ma1, A1.ptr, p.M, p.K1, A1.ld, C::BK, C::BM, 128));
     else ma1 = ma0;
   } else {
     RECNN_REQUIRE(p.K1 == 0, "MN-major A cannot be a K-concat");
-    RECNN_PROPAGATE(make_tmap(&ma0, A0.ptr, p.K0, p.M, A0.ld, 32, C::BK, 1032));
+    RECNN_PROPAGATE(make_tmap(&ma0, A0.ptr, p.K0, p.M, A0.ld, 32, C::BK, 128));
     ma1 = ma0;
   }
-  if (!C::B_MN) RECNN_PROPAGATE(make_tmap(&mb, B.ptr, B.rows, B.cols, B.ld, C::BK, C::BN, C::K_SWZ));
-  else RECNN_PROPAGATE(make_tmap(&mb, B.ptr, B.rows, B.cols, B.ld, 32, C::BK, 1032));
+  if (!C::B_MN) RECNN_PROPAGATE(make_tmap(&mb, B.ptr, B.rows, B.cols, B.ld, C::BK, C::BN, 128));
+  else RECNN_PROPAGATE(make_tmap(&mb, B.ptr, B.rows, B.cols, B.ld, 32, C::BK, 128));
   dim3 grid((unsigned)ceil_div(p.N, C::BN), (unsigned)ceil_div(p.M, C::BM), (unsigned)splits);
   static const bool debug = getenv("RECNN_B200_DEBUG") != nullptr;
   if (debug)
@@ -121,9 +120,10 @@ static int launch_cfg(const Operand& A0, const Operand& A1, const Operand& B, co
 template <bool A_MN, bool B_MN, int EPI>
 int launch(const Operand& A0, const Operand& A1, const Operand& B, const Problem& p, int splits, int bn,
            const Epilogue& epi, cudaStream_t st) {
-  // stages chosen to fill ~190 KB of shared memory: stage = 16 KB (raw A) + 2 * BN/8 KB (B hi | B lo)
-  if (bn >= 128) return launch_cfg<Cfg<128, 4, A_MN, B_MN>, EPI>(A0, A1, B, p, splits, epi, st);
-  return launch_cfg<Cfg<64, 6, A_MN, B_MN>, EPI>(A0, A1, B, p, splits, epi, st);
+  // raw stages chosen to fill the 227 KB of shared memory left beside the two split buffers
+  // (raw stage = 16 KB A + BN/8 KB B; split buffer = twice that)
+  if (bn >= 128) return launch_cfg<Cfg<128, 3, A_MN, B_MN>, EPI>(A0, A1, B, p, splits, epi, st);
+  return launch_cfg<Cfg<64, 5, A_MN, B_MN>, EPI>(A0, A1, B, p, splits, epi, st);
 }
 
 // explicit instantiations used by step.cu / the generic entry points

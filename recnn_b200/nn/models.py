@@ -1,5 +1,5 @@
 """Actor / Critic / DiscreteActor with the reference's constructor, attributes and state_dict
-layout (recnn/nn/models.py:41-73, :76-184, :187-213), evaluated by the sm_100a kernels.
+layout (recnn/nn/models.py:41-73, :76-184, :187-213), evaluated by the sm_90a kernels.
 
 ``forward`` is the inference / evaluation entry (no autograd graph): training
 goes through recnn_b200.nn.update.*, which runs forward+backward+optimizer as

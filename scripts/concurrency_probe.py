@@ -1,4 +1,4 @@
-"""How much do tcgen05 GEMMs slow each other down when they run side by side?  (diagnostic for DESIGN.md section 5)
+"""How much do the 3xTF32 GEMMs slow each other down when they run side by side?  (diagnostic for the intra-step stream overlap)
 
 K concurrent layer-1 GEMMs [4096x1292]x[1292x256] on K streams inside one CUDA graph, per configuration:
     tile 128 (64 CTAs each) / tile 64 (128 CTAs each);  distinct A operands / the SAME A operand;

@@ -1,4 +1,4 @@
-"""One tcgen05 GEMM at the layer-1 shape, a few launches (for ncu)."""
+"""One wgmma 3xTF32 GEMM at the layer-1 shape, a few launches (for ncu)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

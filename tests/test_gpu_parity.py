@@ -1,4 +1,4 @@
-"""GPU parity: the CUDA path (public API -> C ABI -> sm_100a kernels) against
+"""GPU parity: the CUDA path (public API -> C ABI -> sm_90a kernels) against
 (a) the golden vectors generated from the unmodified reference and (b) the numpy
 oracle run live on the same seeded inputs."""
 import ctypes

@@ -1,4 +1,4 @@
-"""tcgen05 3xTF32 GEMM (recnn_gemm_tf32x3) against float64 numpy and against the exact-fp32
+"""wgmma 3xTF32 GEMM (recnn_gemm_tf32x3) against float64 numpy and against the exact-fp32
 CUDA-core GEMM (recnn_gemm_fp32), all four operand-major combinations, ragged shapes."""
 import numpy as np
 import pytest

@@ -1,52 +1,39 @@
-"""Live differential test: the numpy oracle against the UNMODIFIED reference imported from /root/reference, on
-seeds that are NOT in the golden fixtures.  Only runs where the reference tree exists (the build container); on
-the GPU box it is skipped -- the committed golden vectors carry the pinning there."""
+"""Differential test: the numpy oracle against results of the UNMODIFIED reference on seeds that were NOT screened
+for unambiguous ReLU gates (oracle/cases.py UNSCREENED).  The reference's results are stored vectors
+(tests/golden/unscreened_*.npz, gather_random_users.npz; oracle/make_golden.py writes them)."""
 import numpy as np
 import pytest
 
 from oracle import cases as C
 from oracle import recnn_oracle as O
-from oracle.ref_import import reference_available
-from tests._golden import compare_with_golden, run_oracle_case
-
-pytestmark = pytest.mark.skipif(not reference_available(), reason="reference tree not present (GPU box)")
-
-
-def _spec(seed, **kw):
-    base = dict(C.CASES["tiny"], steps=12)
-    base["seeds"] = {"ddpg": seed, "td3": seed + 1}
-    base.update(kw)
-    return base
+from tests._golden import compare_with_golden, load_golden, run_oracle_case
 
 
 @pytest.mark.parametrize("opt", ["adam", "sgd"])
 @pytest.mark.parametrize("algo", ["ddpg", "td3"])
-@pytest.mark.parametrize("spec", [_spec(1001), _spec(1002, n_rows=17, dim=8, frame=3, hidden=16, n_items=40),
-                                  _spec(1003, n_rows=40, hidden=64)], ids=["tiny-a", "narrow", "wide"])
+@pytest.mark.parametrize("spec", list(C.UNSCREENED.values()), ids=list(C.UNSCREENED))
 def test_oracle_tracks_the_live_reference(spec, algo, opt):
-    from oracle.make_golden import run_update_case
-    from oracle.ref_import import import_reference
-    recnn = import_reference()
-    live = run_update_case(recnn, spec, algo, opt)
-    if float(live["gate_margin"]) <= C.GATE_GUARD:
+    cid = next(k for k, v in C.UNSCREENED.items() if v is spec)
+    ref = load_golden("unscreened_%s_%s_%s.npz" % (cid, algo, opt))
+    if float(ref["gate_margin"]) <= C.GATE_GUARD:
         pytest.skip("unscreened seed with an ambiguous ReLU gate (margin %.2g): torch/MKL and numpy may gate "
-                    "differently; the screened golden seeds cover this algorithm" % float(live["gate_margin"]))
-    got = run_oracle_case(spec, algo, opt, golden=live if algo == "td3" else None)
-    compare_with_golden(got, live, check_grads=(algo == "ddpg"))
+                    "differently; the screened golden seeds cover this algorithm" % float(ref["gate_margin"]))
+    got = run_oracle_case(spec, algo, opt, golden=ref if algo == "td3" else None)
+    compare_with_golden(got, ref, check_grads=(algo == "ddpg"))
 
 
 def test_reference_gather_equals_oracle_on_random_users():
-    import copy
-    import torch
-    from oracle.ref_import import import_reference
-    recnn = import_reference()
-    rng = np.random.default_rng(31)
-    frame = 7
-    table = rng.standard_normal((90, 12), dtype=np.float32)
-    users = [{"items": rng.integers(0, 90, size=n, dtype=np.int64), "rates": rng.standard_normal(n) * 2,
-              "sizes": n, "users": 5 + i} for i, n in enumerate((8, 30, 9, 8, 21))]
-    ref = recnn.data.utils.prepare_batch_static_size(copy.deepcopy(users), torch.from_numpy(table), frame_size=frame)
+    ref = load_golden("gather_random_users.npz")
+    frame = int(ref["frame_size"])
+    users = []
+    i = 0
+    while "user%d.items" % i in ref:
+        items = ref["user%d.items" % i]
+        users.append({"items": items, "rates": ref["user%d.rates" % i], "sizes": len(items),
+                      "users": int(ref["user%d.id" % i])})
+        i += 1
+    assert len(users) == 5
     col = O.collate_users(users, frame)
-    out = O.frame_gather(table, col["items"], col["ratings"], col["sizes"], frame)
+    out = O.frame_gather(ref["table"], col["items"], col["ratings"], col["sizes"], frame)
     for k in ("state", "next_state", "action", "reward", "done"):
-        assert np.array_equal(out[k].view(np.uint32), ref[k].numpy().view(np.uint32)), k
+        assert np.array_equal(out[k].view(np.uint32), ref["out." + k].view(np.uint32)), k
