@@ -356,6 +356,17 @@ RECNN_API int recnn_reinforce_policy_grad(const recnn_discrete_dims* d, const fl
                                           const float* state, const int64_t* action, const float* beta_log_prob,
                                           const float* returns, int64_t n_rows, int32_t method, int32_t top_k,
                                           float* out, float* scratch, void* stream);
+/* The same gradient without the [n_rows, num_items] logits: the items are visited in chunks of chunk_items (num_items,
+ * or a positive multiple of 128 below it; the last chunk may be narrower), twice -- per-row softmax statistics, then
+ * the chunk's logits recomputed and back-propagated.  Scratch (recnn_reinforce_scratch_floats) holds one
+ * [n_rows, chunk_items] chunk and does not grow with num_items.  recnn_reinforce_policy_grad is this call with
+ * chunk_items = num_items.  Deterministic: fixed chunk order, no atomics. */
+RECNN_API int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d, const float* params, float* grads,
+                                                  const float* state, const int64_t* action, const float* beta_log_prob,
+                                                  const float* returns, int64_t n_rows, int32_t method, int32_t top_k,
+                                                  int32_t chunk_items, float* out, float* scratch, void* stream);
+/* floats of scratch for recnn_reinforce_policy_grad_chunked; 0 when chunk_items is not accepted */
+RECNN_API int64_t recnn_reinforce_scratch_floats(const recnn_discrete_dims* d, int64_t n_rows, int32_t chunk_items);
 
 /* ---- data parallel: all-reduce over NVLink peer memory ------------------------------------------
  * BASELINE north_star: "partition the embedding gather + update across the 8 GPUs of one box with

@@ -41,7 +41,8 @@ enum EpiKind {
   EPI_LINEAR = 1,   // out = acc + bias[n] (+tanh) (+clamp(noise))       (models.py:70-72, td3.py:74-78)
   EPI_GATE = 2,     // out = acc * (h[m,n] > 0 ? gate_scale : 0)          (relu'/dropout backward)
   EPI_STORE = 3,    // out = acc
-  EPI_PARTIAL = 4   // split-K partial: part[z][m][n] = acc
+  EPI_PARTIAL = 4,  // split-K partial: part[z][m][n] = acc
+  EPI_ACCUM = 5     // out += acc, then (h != null) * (h[m,n] > 0 ? gate_scale : 0)   (one output block of a chunked sum)
 };
 
 struct Epilogue {
@@ -100,6 +101,9 @@ __device__ __forceinline__ void epi_store(const Epilogue& e, int M, int N, int m
     }
   } else if (EPI == EPI_GATE) {
     v = e.h[(long long)m * e.ldh + n] > 0.f ? v * e.gate_scale : 0.f;
+  } else if (EPI == EPI_ACCUM) {
+    v = e.out[(long long)m * e.ldo + n] + v;
+    if (e.h) v = e.h[(long long)m * e.ldh + n] > 0.f ? v * e.gate_scale : 0.f;
   }
   e.out[(long long)m * e.ldo + n] = v;
 }

@@ -135,6 +135,7 @@ RECNN_TC_INST(false, false, EPI_LINEAR)
 RECNN_TC_INST(false, false, EPI_STORE)
 RECNN_TC_INST(false, true, EPI_STORE)
 RECNN_TC_INST(false, true, EPI_GATE)
+RECNN_TC_INST(false, true, EPI_ACCUM)
 RECNN_TC_INST(true, true, EPI_STORE)
 RECNN_TC_INST(true, true, EPI_PARTIAL)
 RECNN_TC_INST(false, false, EPI_PARTIAL)

@@ -276,6 +276,9 @@ __device__ __forceinline__ void epilogue_row(const Epilogue& e, const Problem& p
                 }
               } else if (EPI == EPI_GATE) {
                 x = e.h[(long long)m * e.ldh + nn] > 0.f ? x * e.gate_scale : 0.f;
+              } else if (EPI == EPI_ACCUM) {
+                x = out_row[nn] + x;
+                if (e.h) x = e.h[(long long)m * e.ldh + nn] > 0.f ? x * e.gate_scale : 0.f;
               }
             }
             v[u] = x;

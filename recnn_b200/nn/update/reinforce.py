@@ -1,7 +1,8 @@
 """Drop-in for recnn.nn.update.reinforce (recnn/nn/update/reinforce.py:10-129): ChooseREINFORCE and reinforce_update.
 
-The policy loss and its gradient are ONE device call (recnn_reinforce_policy_grad: recomputed forward, closed-form
-d loss / d logits, three tensor-core GEMMs) over the rows ``DiscreteActor`` saved since the last policy update; the
+The policy loss and its gradient are ONE device call (recnn_reinforce_policy_grad_chunked: recomputed forward,
+closed-form d loss / d logits, three tensor-core GEMMs; over item chunks when the [rows, num_items] logits would exceed
+_LOGITS_BUDGET_BYTES) over the rows ``DiscreteActor`` saved since the last policy update; the
 optimizer step is the fused arena kernel (recnn_b200.optim) or any torch optimizer stepping the aliased ``.grad``
 views.  The critic half is the DDPG critic step (value_update) fed with the target policy's probabilities.
 """
@@ -16,6 +17,19 @@ from ... import utils
 from ...utils.misc import DummyWriter
 from ..arena import param_arena, grad_arena
 from .misc import value_update
+
+# Largest logits buffer ([rows, chunk] fp32) one policy update may hold.  Below it the whole [rows, num_items] matrix
+# is kept (one pass); above it the items are visited in chunks and the logits are computed twice.
+_LOGITS_BUDGET_BYTES = 1 << 30
+
+
+def _chunk_items(rows, num_items):
+    """Item chunk width of the policy gradient over ``rows`` saved rows: every item at once when their logits fit in
+    _LOGITS_BUDGET_BYTES, otherwise the widest multiple of 128 that fits (at least 128)."""
+    if rows * num_items * 4 <= _LOGITS_BUDGET_BYTES:
+        return num_items
+    chunk = max(128, _LOGITS_BUDGET_BYTES // (rows * 4) // 128 * 128)
+    return min(chunk, num_items)
 
 
 def _policy_loss(policy, returns, method):
@@ -44,16 +58,17 @@ def _policy_loss(policy, returns, method):
     n = state.shape[0]
     d = policy.dims
     L = _lib.lib()
-    scratch = torch.empty(L.recnn_discrete_scratch_floats(d, n, 1), device=dev, dtype=torch.float32)
+    chunk = _chunk_items(n, d.num_items)
+    scratch = torch.empty(L.recnn_reinforce_scratch_floats(d, n, chunk), device=dev, dtype=torch.float32)
     out = torch.zeros(2, device=dev, dtype=torch.float32)
     ks = {r.get("K") for r in saved if r.get("K") is not None}
     if len(ks) > 1:
         raise ValueError("select_action was called with different K since the last policy update: %s" % sorted(ks))
     K = ks.pop() if ks else 1
     with torch.cuda.device(dev):
-        _lib.check(L.recnn_reinforce_policy_grad(d, flat.data_ptr(), grads.data_ptr(), state.data_ptr(), action.data_ptr(),
-                                                 _lib.ptr(beta_lp), ret_rows.data_ptr(), n, method, K, out.data_ptr(),
-                                                 scratch.data_ptr(), _lib.stream_ptr(dev)))
+        _lib.check(L.recnn_reinforce_policy_grad_chunked(
+            d, flat.data_ptr(), grads.data_ptr(), state.data_ptr(), action.data_ptr(), _lib.ptr(beta_lp),
+            ret_rows.data_ptr(), n, method, K, chunk, out.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
     if int(out.view(torch.int32)[1].item()) != 0:
         raise IndexError("saved action index out of range for the policy's output layer")
     return out[0].clone()
