@@ -368,6 +368,63 @@ RECNN_API int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d, 
 /* floats of scratch for recnn_reinforce_policy_grad_chunked; 0 when chunk_items is not accepted */
 RECNN_API int64_t recnn_reinforce_scratch_floats(const recnn_discrete_dims* d, int64_t n_rows, int32_t chunk_items);
 
+/* ---- REINFORCE: the critic side with item-id actions ---------------------------------------------
+ * The REINFORCE critic is a Critic(S, num_items, H) (recnn/nn/update/reinforce.py:92-102): layer 1 is W1 [H, S + num_items]
+ * on [state | action], the action being a one-hot row (the batch) or a probability row (the target policy's output).
+ * These calls never form a [n_rows, num_items] matrix: the action block W1a = W1[:, S:] enters layer 1 as an [n_rows, H]
+ * "action term" added in its epilogue -- W1[:, S + a] for an item id a, or probs W1a^T streamed over item chunks.
+ * d: the critic's dims (action_dim = num_items); pd: the DiscreteActor's (equal state_dim and num_items).
+ * chunk_items: num_items, or a positive multiple of 128 below it; scratch does not grow with num_items below it. */
+/* out [n_rows, H] = probs W1a^T, with probs = DiscreteActor(policy_params)(state) (softmax folded over the chunks with a
+ * running max and sum, one pass) or the dense probs [n_rows, probs_ld] (policy_params NULL).  W1a is critic_params' */
+RECNN_API int64_t recnn_critic_action_term_scratch_floats(const recnn_dims* d, const recnn_discrete_dims* pd,
+                                                          int64_t n_rows, int32_t chunk_items);
+RECNN_API int recnn_critic_action_term_chunked(const recnn_dims* d, const float* critic_params,
+                                               const recnn_discrete_dims* pd, const float* policy_params,
+                                               const float* state, const float* probs, int64_t probs_ld,
+                                               int64_t n_rows, int32_t chunk_items, float* out, float* scratch,
+                                               void* stream);
+/* Critic.forward (models.py:205-213) with the action block given as its action term [n_rows, H] (from the call above);
+ * scratch: fp32[recnn_forward_scratch_floats(d, n_rows, 0)] */
+RECNN_API int recnn_critic_forward_action_term(const recnn_dims* d, const float* params, const float* state,
+                                               const float* action_term, int64_t n_rows, const uint8_t* mask1,
+                                               const uint8_t* mask2, float* value_out, float* scratch, void* stream);
+
+typedef struct recnn_discrete_value_args {
+  recnn_dims dims;                  /* the critic: state_dim, action_dim = num_items, hidden */
+  recnn_discrete_dims policy_dims;  /* the target DiscreteActor */
+  int32_t learn;                    /* 0: loss only */
+  int32_t dropout;                  /* 1: the online critic is in train() mode */
+  int32_t chunk_items;
+  int32_t reserved;
+  int64_t n_rows;
+  const float* state;               /* [n_rows, state_dim] */
+  const float* next_state;          /* [n_rows, state_dim] */
+  const int64_t* action;            /* [n_rows] item ids (the batch's one-hot action, as indices) */
+  const float* reward;              /* [n_rows] */
+  const float* done;                /* [n_rows] */
+  recnn_net value, target_value;
+  const float* target_policy;       /* DiscreteActor arena (recnn_discrete_layout) */
+  recnn_optim value_optim;          /* RECNN_OPT_EXTERNAL: the gradient is left in value.grads */
+  float gamma, min_value, max_value;
+  int32_t reserved2;
+  const uint8_t* masks[2];          /* the online critic's two dropout masks uint8 [n_rows, H], or NULL (Philox) */
+  uint64_t seed;
+  int64_t* rng_step;                /* device int64, read by the dropout and incremented at the end of the call */
+  float* losses;                    /* device, 8 words: [0] value loss, [4] int32 error bits (1: an action id was outside
+                                     * [0, num_items) -- its row used a zero action column and added no gradient) */
+  float* losses_host;               /* optional pinned host copy of `losses` */
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_discrete_value_args;
+RECNN_API int64_t recnn_sizeof_discrete_value_args(void);
+RECNN_API int64_t recnn_discrete_value_workspace_bytes(const recnn_dims* d, const recnn_discrete_dims* pd,
+                                                       int64_t n_rows, int32_t chunk_items);
+/* misc.py:10-55 with a DiscreteActor target policy and item-id actions: TD target through the chunked action term of
+ * the target critic, online critic with the gathered action columns, MSE, backward (the action block of dW1 is zero
+ * except in the selected columns, each the ascending-row sum of its rows' dz1: deterministic), optimizer. */
+RECNN_API int recnn_discrete_value_step(const recnn_discrete_value_args* args, void* stream);
+
 /* ---- data parallel: all-reduce over NVLink peer memory ------------------------------------------
  * BASELINE north_star: "partition the embedding gather + update across the 8 GPUs of one box with
  * an allreduce of the Actor/Critic gradients over NVLink".  The reference itself is single-process

@@ -63,7 +63,23 @@ class StepArgs(C.Structure):
     ]
 
 
-_PROBE_FIELDS = ["dims", "n_rows", "table", "policy", "policy_optim", "gamma", "soft_tau", "masks", "seed",
+class DiscreteValueArgs(C.Structure):
+    _fields_ = [
+        ("dims", Dims), ("policy_dims", DiscreteDims),
+        ("learn", C.c_int32), ("dropout", C.c_int32), ("chunk_items", C.c_int32), ("reserved", C.c_int32),
+        ("n_rows", C.c_int64),
+        ("state", C.c_void_p), ("next_state", C.c_void_p), ("action", C.c_void_p), ("reward", C.c_void_p),
+        ("done", C.c_void_p),
+        ("value", Net), ("target_value", Net), ("target_policy", C.c_void_p),
+        ("value_optim", Optim),
+        ("gamma", C.c_float), ("min_value", C.c_float), ("max_value", C.c_float), ("reserved2", C.c_int32),
+        ("masks", C.c_void_p * 2), ("seed", C.c_uint64), ("rng_step", C.c_void_p),
+        ("losses", C.c_void_p), ("losses_host", C.c_void_p),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
+_PROBE_FIELDS =["dims", "n_rows", "table", "policy", "policy_optim", "gamma", "soft_tau", "masks", "seed",
                  "losses", "workspace_bytes", "comm"]
 
 # name -> (restype, argtypes); every symbol include/recnn_b200.h declares
@@ -120,6 +136,17 @@ SIGNATURES = {
                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
                                                       C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_reinforce_scratch_floats": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32]),
+    "recnn_critic_action_term_scratch_floats": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
+                                                            C.c_int32]),
+    "recnn_critic_action_term_chunked": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.POINTER(DiscreteDims), C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]),
+    "recnn_critic_forward_action_term": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_sizeof_discrete_value_args": (C.c_int64, []),
+    "recnn_discrete_value_workspace_bytes": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
+                                                         C.c_int32]),
+    "recnn_discrete_value_step": (C.c_int, [C.POINTER(DiscreteValueArgs), C.c_void_p]),
     "recnn_comm_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]),
     "recnn_comm_handle_bytes": (C.c_int32, []),
     "recnn_comm_local_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -161,6 +188,9 @@ def lib():
     if handle.recnn_sizeof_step_args() != C.sizeof(StepArgs):
         raise RecnnError("recnn_step_args layout mismatch: C %d bytes, ctypes %d bytes"
                          % (handle.recnn_sizeof_step_args(), C.sizeof(StepArgs)))
+    if handle.recnn_sizeof_discrete_value_args() != C.sizeof(DiscreteValueArgs):
+        raise RecnnError("recnn_discrete_value_args layout mismatch: C %d bytes, ctypes %d bytes"
+                         % (handle.recnn_sizeof_discrete_value_args(), C.sizeof(DiscreteValueArgs)))
     for i, f in enumerate(_PROBE_FIELDS):
         if handle.recnn_offsetof_step_args(i) != getattr(StepArgs, f).offset:
             raise RecnnError("recnn_step_args.%s offset mismatch" % f)

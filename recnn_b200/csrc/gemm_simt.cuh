@@ -37,7 +37,7 @@ __device__ __forceinline__ float view_at(const MatView& v, long long r, int c) {
 }
 
 enum EpiKind {
-  EPI_HIDDEN = 0,   // out = relu(acc + bias[n]) * keep(m,n)*2          (models.py:66-69)
+  EPI_HIDDEN = 0,   // out = relu(acc + bias[n] (+ add[m,n])) * keep(m,n)*2   (models.py:66-69)
   EPI_LINEAR = 1,   // out = acc + bias[n] (+tanh) (+clamp(noise))       (models.py:70-72, td3.py:74-78)
   EPI_GATE = 2,     // out = acc * (h[m,n] > 0 ? gate_scale : 0)          (relu'/dropout backward)
   EPI_STORE = 3,    // out = acc
@@ -62,6 +62,8 @@ struct Epilogue {
   float noise_clip;
   float noise_std;       // perf mode: philox normal * std (noise == null && add_noise)
   int add_noise;
+  const float* add;      // EPI_HIDDEN: optional per-row addend [M, ldadd] (a layer-1 input block contracted elsewhere)
+  long long ldadd;
 };
 
 template <int EPI>
@@ -72,7 +74,9 @@ __device__ __forceinline__ void epi_store(const Epilogue& e, int M, int N, int m
   }
   float v = acc;
   if (EPI == EPI_HIDDEN) {
-    v = fmaxf(v + e.bias[n], 0.f);
+    v = v + e.bias[n];
+    if (e.add) v += e.add[(long long)m * e.ldadd + n];
+    v = fmaxf(v, 0.f);
     if (e.train) {
       bool keep;
       if (e.mask) keep = e.mask[(long long)m * N + n] != 0;

@@ -224,12 +224,12 @@ static int gemm_nt(const Seg& x0, const Seg& x1, const float* W, long long ldw, 
   return launch_gemm_simt<true, true, EPI>(X, mat(W, ldw), (int)n, N, K, 1, e, st);
 }
 
-// h = dropout(relu([x0|x1] W^T + b))
+// h = dropout(relu([x0|x1] W^T + b (+ add)))      add: optional [n, H] term of an input block contracted elsewhere
 static int hidden_layer(const Seg& x0, const Seg& x1, const float* W, long long ldw, const float* b, int H,
                         int64_t n, bool train, const uint8_t* mask, const Rng& rng, unsigned stream_id, float* out,
-                        cudaStream_t st) {
+                        cudaStream_t st, const float* add = nullptr) {
   Epilogue e = base_epi();
-  e.out = out; e.ldo = H; e.bias = b;
+  e.out = out; e.ldo = H; e.bias = b; e.add = add; e.ldadd = H;
   e.train = train ? 1 : 0; e.mask = mask; e.seed = rng.seed; e.rng_step = rng.step; e.stream_id = stream_id;
   return gemm_nt<EPI_HIDDEN>(x0, x1, W, ldw, H, n, e, st);
 }
@@ -921,3 +921,5 @@ extern "C" int recnn_linear_forward(const float* x, int64_t n_rows, int in_dim, 
 
 // ---------------------------------------------------------------- REINFORCE (policy side)
 #include "reinforce.cuh"
+// ---------------------------------------------------------------- REINFORCE (critic side, item-id actions)
+#include "critic_ids.cuh"

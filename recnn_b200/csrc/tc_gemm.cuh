@@ -256,7 +256,9 @@ __device__ __forceinline__ void epilogue_row(const Epilogue& e, const Problem& p
             const int nn = n + u;
             if (nn < N) {
               if (EPI == EPI_HIDDEN) {
-                x = fmaxf(x + __ldg(e.bias + nn), 0.f);
+                x = x + __ldg(e.bias + nn);
+                if (e.add) x += e.add[(long long)m * e.ldadd + nn];
+                x = fmaxf(x, 0.f);
                 if (e.train) x = ((keep_bits >> (j4 + u)) & 1u) ? x * 2.0f : 0.f;
               } else if (EPI == EPI_LINEAR) {
                 x = x + __ldg(e.bias + nn);

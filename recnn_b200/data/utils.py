@@ -59,20 +59,24 @@ def batch_tensor_embeddings(batch, item_embeddings_tensor, frame_size, *args, **
             "meta": {"users": users_t, "sizes": sizes_t}}
 
 
-def batch_contstate_discaction(batch, item_embeddings_tensor, frame_size, num_items, *args, **kwargs):
+def batch_contstate_discaction(batch, item_embeddings_tensor, frame_size, num_items, *args, one_hot=True, **kwargs):
     """Embed batch: continuous state, discrete action (utils.py:84-120), on the device.
 
     Same gather kernel as ``batch_tensor_embeddings`` for state / next_state / reward / done; the action is the item id
     of the last frame position -- returned as the reference's dense one-hot ``action`` [N, num_items] (what its
-    ``Critic(1290, num_items, ...)`` consumes) and as ``action_index`` int64 [N]."""
+    ``Critic(1290, num_items, ...)`` consumes) and as ``action_index`` int64 [N].  ``one_hot=False`` returns the ids as
+    ``action`` too: value_update / reinforce_update then run the critic without any [N, num_items] matrix."""
     out = batch_tensor_embeddings(batch, item_embeddings_tensor, frame_size, *args, **kwargs)
     dev = out["state"].device
     index = batch["items"][:, -1].to(device=dev, dtype=torch.int64)
     if int(index.max().item()) >= num_items or int(index.min().item()) < 0:
         raise RuntimeError("index out of range for a one-hot action of %d items" % num_items)   # scatter_ raises too
-    one_hot = torch.zeros(index.shape[0], num_items, device=dev)
-    one_hot.scatter_(1, index.view(-1, 1), 1)
-    out["action"] = one_hot
+    if one_hot:
+        dense = torch.zeros(index.shape[0], num_items, device=dev)
+        dense.scatter_(1, index.view(-1, 1), 1)
+        out["action"] = dense
+    else:
+        out["action"] = index
     out["action_index"] = index
     return out
 

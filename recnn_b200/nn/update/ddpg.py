@@ -6,6 +6,7 @@ import torch
 from ... import _lib
 from ... import utils
 from ._engine import get_engine
+from ._ids import reject_ids
 
 
 def ddpg_update(batch, params, nets, optimizer, device=torch.device("cpu"), debug=None,
@@ -28,6 +29,7 @@ def ddpg_update(batch, params, nets, optimizer, device=torch.device("cpu"), debu
     if not learn and debug is None:
         # the reference fails the same way: debug["next_action"] = ... on None (misc.py:47)
         raise TypeError("'NoneType' object does not support item assignment")
+    reject_ids(batch, "ddpg_update")
     eng = get_engine(_lib.ALGO_DDPG, nets, device)
     vals = eng.step(batch, params, nets, optimizer, learn, step, debug, "policy_step")
     losses = {"value": vals[0], "policy": vals[2], "step": step}

@@ -6,6 +6,7 @@ import torch
 from ... import _lib
 from ... import utils
 from ._engine import get_engine
+from . import _ids
 
 
 def temporal_difference(reward, done, gamma, target):
@@ -17,7 +18,15 @@ def temporal_difference(reward, done, gamma, target):
 def value_update(batch, params, nets, optimizer, device=torch.device("cpu"), debug=None,
                  writer=utils.DummyWriter(), learn=False, step=-1):
     """DDPG critic step on its own (misc.py:10-55).  Returns the value loss as a 0-dim tensor
-    (the reference returns the loss tensor, not a float)."""
+    (the reference returns the loss tensor, not a float).
+
+    With a DiscreteActor target policy, ``batch["action"]`` may be an integer tensor of item ids [N] instead of the
+    dense one-hot [N, num_items]: the same update then runs without any [N, num_items] buffer (recnn_b200/nn/update/
+    _ids.py), which is what makes a million-item critic fit on one GPU."""
+    if _ids.is_item_ids(batch["action"]):
+        if not _ids._is_discrete(nets["target_policy_net"]):
+            raise ValueError("item-id actions need a DiscreteActor target policy (nets['target_policy_net'])")
+        return torch.tensor(_ids.get_ids_step(nets, device).run(batch, params, nets, optimizer, learn, debug))
     eng = get_engine(_lib.ALGO_DDPG, nets, device)
     vals = eng.value_only(batch, params, nets, optimizer, learn, debug)
     return torch.tensor(vals[0])

@@ -4,7 +4,9 @@ The policy loss and its gradient are ONE device call (recnn_reinforce_policy_gra
 closed-form d loss / d logits, three tensor-core GEMMs; over item chunks when the [rows, num_items] logits would exceed
 _LOGITS_BUDGET_BYTES) over the rows ``DiscreteActor`` saved since the last policy update; the
 optimizer step is the fused arena kernel (recnn_b200.optim) or any torch optimizer stepping the aliased ``.grad``
-views.  The critic half is the DDPG critic step (value_update) fed with the target policy's probabilities.
+views.  The critic half is the DDPG critic step (value_update) fed with the target policy's probabilities, or -- when
+``batch["action"]`` holds integer item ids -- the item-id critic step of _ids.py, which never forms a [N, num_items]
+matrix.
 """
 from __future__ import annotations
 
@@ -17,6 +19,7 @@ from ... import utils
 from ...utils.misc import DummyWriter
 from ..arena import param_arena, grad_arena
 from .misc import value_update
+from . import _ids
 
 # Largest logits buffer ([rows, chunk] fp32) one policy update may hold.  Below it the whole [rows, num_items] matrix
 # is kept (one pass); above it the items are visited in chunks and the logits are computed twice.
@@ -136,6 +139,10 @@ def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"),
     dev = policy.linear1.weight.device
     if dev.type != "cuda":
         raise _lib.RecnnError("recnn_b200 update functions run on CUDA only (policy net is on %s); there is no CPU path" % dev)
+    # item-id batch actions (an integer [N] tensor): the critic never sees a [N, num_items] matrix (_ids.py)
+    ids = _ids.is_item_ids(batch["action"])
+    if ids and not _ids._is_discrete(nets["target_policy_net"]):
+        raise ValueError("item-id actions need a DiscreteActor target policy (nets['target_policy_net'])")
     state = batch["state"].to(dev)
     action = batch["action"].to(dev)
 
@@ -146,7 +153,10 @@ def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"),
         mx = predicted_probs.max(dim=1).values
         writer.add_histogram("predicted_probs_max_mean", mx.mean(), step)
         writer.add_histogram("predicted_probs_max_std", mx.std(), step)
-    reward = nets["value_net"](state, predicted_probs).detach()
+    if ids:
+        reward = _ids.critic_value_of_probs(nets["value_net"], state, predicted_probs).detach()
+    else:
+        reward = nets["value_net"](state, predicted_probs).detach()
     policy.rewards.append(reward.mean())
 
     value_loss = value_update(batch, params, nets, optimizer, writer=writer, device=dev, debug=debug, learn=True, step=step)

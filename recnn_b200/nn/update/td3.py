@@ -6,6 +6,7 @@ import torch
 from ... import _lib
 from ... import utils
 from ._engine import get_engine
+from ._ids import reject_ids
 
 
 def td3_update(batch, params, nets, optimizer, device=torch.device("cpu"), debug=None,
@@ -19,6 +20,7 @@ def td3_update(batch, params, nets, optimizer, device=torch.device("cpu"), debug
     reference draws the noise on the CPU generator, td3.py:74)."""
     if debug is None:
         debug = dict()           # td3.py:66-67
+    reject_ids(batch, "td3_update")
     eng = get_engine(_lib.ALGO_TD3, nets, device)
     vals = eng.step(batch, params, nets, optimizer, learn, step, debug, "policy_update")
     losses = {"value1": vals[0], "value2": vals[1], "policy": vals[2], "step": step}
