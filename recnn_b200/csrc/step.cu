@@ -108,6 +108,9 @@ static int dw_splits(int C, int K, int64_t n_rows, bool tc_path, int bn = 128) {
   return (int)(s < 1 ? 1 : s);
 }
 
+// rows per split of the unfused value head's gradient (launch_head_grad_partials)
+constexpr int64_t kHeadGradRowsPerSplit = 256;
+
 static int64_t partial_floats(const recnn_dims& d, int64_t n_rows) {
   const int in_c = d.state_dim + d.action_dim;
   int64_t best = 0;
@@ -119,7 +122,11 @@ static int64_t partial_floats(const recnn_dims& d, int64_t n_rows) {
       if (f > best) best = f;
     }
   const int64_t head = (int64_t)kNumSMs * (d.hidden + 2);     // block partials of the fused value-head kernel
-  return best > head ? best : head;
+  // partials [splits][1][H+1] of the unfused value head's dW3 / db3: one split per 256 rows, which is not bounded by
+  // any dw_splits() above (n = 1000, H = 512: 4 splits vs dw_splits(1, 512, 1000, false) = 3)
+  const int64_t head_grad = ceil_div(n_rows, kHeadGradRowsPerSplit) * (d.hidden + 1);
+  if (head > best) best = head;
+  return head_grad > best ? head_grad : best;
 }
 
 static Workspace carve(const recnn_dims& d, int64_t n, void* base) {
@@ -503,9 +510,8 @@ static int phase_value_grad(Ctx& c) {
       RECNN_PROPAGATE(launch_critic_head(h, c.st));
       if (!a.learn) continue;
       // layer 3: dW3 = dq^T h2, db3 = sum dq ; dz2 = (dq w3) * gate(h2)
-      const int64_t rows_per = 256;
-      const int splits = (int)ceil_div(c.n, rows_per);       // <= dw_splits(1, H, n, false): fits ws.partial
-      RECNN_PROPAGATE(launch_head_grad_partials(c.ws.dq, c2, c.n, H, rows_per, splits, c.ws.partial, c.st));
+      const int splits = (int)ceil_div(c.n, kHeadGradRowsPerSplit);      // partial_floats() reserves splits * (H+1)
+      RECNN_PROPAGATE(launch_head_grad_partials(c.ws.dq, c2, c.n, H, kHeadGradRowsPerSplit, splits, c.ws.partial, c.st));
       RECNN_PROPAGATE(launch_reduce_partials(c.ws.partial, splits, 1, H + 1, G + c.lc.w3, c.lc.ld3, G + c.lc.b3, c.st));
       RECNN_PROPAGATE(launch_critic_head_bwd(c.ws.dq, 0.f, P + c.lc.w3, c2, c.gate, dz2, c.n, H, c.st));
     }

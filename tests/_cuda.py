@@ -120,4 +120,5 @@ def run_cuda_case(case, algo, opt_kind, golden=None, form="dense", external=Fals
         for k, v in dump_net(m).items():
             out["final.%s.%s" % (name, k)] = v
     out["_nets"] = nets
+    out["_opts"] = opts
     return out

@@ -98,6 +98,51 @@ def neutralise_ambiguous_gates(spec, algo, opt_kind, thresh=2e-5, max_iter=8):
     raise AssertionError("ambiguous gates remain after %d rounds" % max_iter)
 
 
+def assert_tight_parity(got, want, init_nets, loss_rtol=1e-5, rtol=1e-5, floor_frac=1e-2, delta_rtol=2e-3,
+                        outliers=0, outlier_abs=0.0):
+    """The golden bar on EVERY element of every final weight (a run with no ambiguous ReLU gate, see
+    neutralise_ambiguous_gates).  ``got`` / ``want``: run_cuda_case / run_oracle_case outputs; ``init_nets``: the
+    nets the run started from (C.make_inputs(...)["nets"]).
+
+    Losses: |got-want| <= loss_rtol*(|want| + 0.1).  Weights: |got-want| <= rtol*(|want| + floor_frac*max|tensor|).
+    Weight changes since init: within delta_rtol of the tensor's largest change, beyond 2 ulp of its largest weight
+    (differences below that are rounding of the stored weight, not signal).  A tensor that does not move must stay
+    bit-identical.
+
+    ``outliers``: elements per tensor that may miss the weight / change bars, each by at most ``outlier_abs``.  Only
+    for Adam, whose g / (|g| + eps) turns the fp32 rounding of a gradient that nearly cancels into an lr-sized
+    difference of that one element.  Returns the largest error found on each bar (outliers excluded), the largest
+    outlier count of a tensor and the number of tensors whose change was checked."""
+    rep = {"loss": 0.0, "weight": 0.0, "delta": 0.0, "outliers": 0, "checked": 0}
+    for k in (k for k in want if k.startswith("loss.")):
+        err = float(np.max(np.abs(got[k] - want[k]) / (np.abs(want[k]) + 0.1)))
+        rep["loss"] = max(rep["loss"], err)
+        assert err <= loss_rtol, (k, err, got[k], want[k])
+    for k in (k for k in want if k.startswith("final.")):
+        _, name, tensor = k.split(".")
+        init = init_nets[name][tensor].astype(np.float64)
+        w_want, w_got = want[k].astype(np.float64), got[k].astype(np.float64)
+        wmax = np.max(np.abs(w_want))
+        rel = np.abs(w_got - w_want) / (np.abs(w_want) + floor_frac * wmax)
+        d_want, d_got = w_want - init, w_got - init
+        scale = np.max(np.abs(d_want))
+        if scale == 0.0:                       # e.g. TD3's target policy is never updated (td3.py:136-141)
+            assert np.array_equal(got[k], want[k]), k
+            continue
+        ulp2 = 2.0 * 1.1920929e-07 * wmax
+        excess = np.maximum(np.abs(d_got - d_want) - ulp2, 0.0) / scale
+        bad = (rel > rtol) | (excess > delta_rtol)
+        n_bad = int(bad.sum())
+        assert n_bad <= outliers, (k, n_bad, float(rel.max()), float(excess.max()))
+        if n_bad:
+            assert np.max(np.abs(w_got - w_want)[bad]) <= outlier_abs, (k, np.max(np.abs(w_got - w_want)[bad]))
+        rep["weight"] = max(rep["weight"], float(np.max(rel[~bad])))
+        rep["delta"] = max(rep["delta"], float(np.max(excess[~bad])))
+        rep["outliers"] = max(rep["outliers"], n_bad)
+        rep["checked"] += 1
+    return rep
+
+
 def rel_err(got, want, floor):
     got = np.asarray(got, dtype=np.float64)
     want = np.asarray(want, dtype=np.float64)
