@@ -189,7 +189,10 @@ typedef struct recnn_net {
  * (requirements.txt:7, unpinned) and absent from this environment: the restatement follows the published algorithm
  * (Liu et al. 2019 rectified Adam with the N_sma_threshhold switch; Zhang et al. 2019 Lookahead every k steps) and
  * its parity with the package is UNPINNED (DESIGN.md section 2). */
-enum { RECNN_OPT_EXTERNAL = 0, RECNN_OPT_SGD = 1, RECNN_OPT_ADAM = 2, RECNN_OPT_RANGER = 3 };
+/* RADAM = Ranger's RAdam half alone (torch_optimizer.RAdam: rectified from N_sma >= 5, decoupled weight decay, no
+ * Lookahead and no slow arena), the optimizer of the Top-K notebook's behaviour policy (recnn_beta_step).  Pinned
+ * against torch.optim.RAdam(decoupled_weight_decay=True); parity with the package is UNPINNED as for Ranger. */
+enum { RECNN_OPT_EXTERNAL = 0, RECNN_OPT_SGD = 1, RECNN_OPT_ADAM = 2, RECNN_OPT_RANGER = 3, RECNN_OPT_RADAM = 4 };
 
 typedef struct recnn_optim {   /* torch.optim.SGD / torch.optim.Adam / torch_optimizer.Ranger semantics */
   int32_t kind;
@@ -424,6 +427,47 @@ RECNN_API int64_t recnn_discrete_value_workspace_bytes(const recnn_dims* d, cons
  * the target critic, online critic with the gathered action columns, MSE, backward (the action block of dW1 is zero
  * except in the selected columns, each the ascending-row sum of its rows' dz1: deterministic), optimizer. */
 RECNN_API int recnn_discrete_value_step(const recnn_discrete_value_args* args, void* stream);
+
+/* ---- REINFORCE with Top-K correction: the behaviour policy beta ------------------------------------
+ * The reference ships beta in its Top-K notebook, not in the library (examples/2. REINFORCE TopK Off Policy
+ * Correction/3. TopK Reinforce Off Policy Correction.ipynb, cell 3: class Beta), and DiscreteActor.pi_beta_sample
+ * (recnn/nn/models.py:113-145) calls its forward once per env step.  Beta is nn.Sequential(nn.Linear(S, num_items),
+ * nn.Softmax()) trained by every forward(state, action): p = softmax(W s + b) (dim 1);
+ * loss = CrossEntropyLoss(p, action.argmax(1)) -- applied to the PROBABILITIES, a softmax of a softmax, reproduced on
+ * purpose; zero_grad, backward, optim.step() (torch_optimizer.RAdam(lr=1e-5, weight_decay=1e-5)); the pre-step p is
+ * returned.  Parameter arena: net.0.weight [num_items, S] with row pitch pad4(S), then net.0.bias [num_items]. */
+typedef struct recnn_beta_dims {
+  int32_t state_dim, num_items, reserved[2];
+} recnn_beta_dims;
+/* out[4]: offsets of the weight and the bias, the weight's row pitch, total float count (cell 3: the Linear's layout) */
+RECNN_API int recnn_beta_layout(const recnn_beta_dims* d, int64_t* out);
+/* bytes of workspace of recnn_beta_step; chunk_items: num_items, or a positive multiple of 128 below it (0 when not
+ * accepted).  Holds one [n_rows, chunk_items] chunk and does not grow with num_items below it. */
+RECNN_API int64_t recnn_beta_workspace_bytes(const recnn_beta_dims* d, int64_t n_rows, int32_t chunk_items);
+
+typedef struct recnn_beta_args {
+  recnn_beta_dims dims;
+  int64_t n_rows;
+  int32_t chunk_items;
+  int32_t reserved;
+  recnn_net net;              /* params, grads (required), opt_m / opt_v / opt_t for the built-in optimizer */
+  recnn_optim optim;          /* RECNN_OPT_EXTERNAL: stop after the gradient (left in net.grads) */
+  const float* state;         /* [n_rows, state_ld] */
+  int64_t state_ld;           /* >= state_dim */
+  const int64_t* action;      /* [n_rows] target item ids (the notebook's action.argmax(1)) */
+  float* probs_out;           /* [n_rows, num_items]: p with the weights from before the step */
+  float* loss;                /* device fp32: mean cross-entropy of the call */
+  int32_t* error;             /* device int32: 1 when an id was outside [0, num_items) -- then no row of that id added
+                               * loss or gradient and the built-in optimizer step was skipped (t included) */
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_beta_args;
+RECNN_API int64_t recnn_sizeof_beta_args(void);
+RECNN_API int64_t recnn_offsetof_beta_args(int field);
+/* One Beta.forward(state, action) of the notebook's cell 3 (forward, loss, backward, optimizer step) on `stream`, no
+ * allocation, no synchronisation.  The items are visited in chunks of chunk_items, twice: logits into probs_out with a
+ * running max / sum, then dZ of each chunk from probs_out and that chunk's rows of dW / db.  Deterministic. */
+RECNN_API int recnn_beta_step(const recnn_beta_args* args, void* stream);
 
 /* ---- data parallel: all-reduce over NVLink peer memory ------------------------------------------
  * BASELINE north_star: "partition the embedding gather + update across the 8 GPUs of one box with

@@ -18,7 +18,7 @@ def install_as_recnn():
         raise ImportError("a different 'recnn' package is already imported")
     alias = {
         "recnn": sys.modules[__name__],
-        "recnn.nn": nn, "recnn.nn.models": nn.models, "recnn.nn.algo": nn.algo, "recnn.nn.update": nn.update,
+        "recnn.nn": nn, "recnn.nn.models": nn.models, "recnn.nn.algo": nn.algo, "recnn.nn.beta": nn.beta, "recnn.nn.update": nn.update,
         "recnn.nn.update.ddpg": nn.update.ddpg, "recnn.nn.update.td3": nn.update.td3,
         "recnn.nn.update.misc": nn.update.misc, "recnn.nn.update.reinforce": nn.update.reinforce,
         "recnn.data": data, "recnn.data.utils": data.utils, "recnn.data.env": data.env, "recnn.data.db_con": data.db_con,

@@ -17,7 +17,7 @@ PH_VALUE_GRAD, PH_VALUE_OPT, PH_POLICY_LOSS, PH_POLICY_GRAD, PH_POLICY_OPT, PH_S
 PH_FINISH = 128
 PH_ALL = 255
 ALGO_DDPG, ALGO_TD3 = 0, 1
-OPT_EXTERNAL, OPT_SGD, OPT_ADAM, OPT_RANGER = 0, 1, 2, 3
+OPT_EXTERNAL, OPT_SGD, OPT_ADAM, OPT_RANGER, OPT_RADAM = 0, 1, 2, 3, 4
 METRIC_L2, METRIC_IP, METRIC_COS = 0, 1, 2
 REINFORCE_BASIC, REINFORCE_CORRECTED, REINFORCE_TOPK = 0, 1, 2
 
@@ -78,6 +78,23 @@ class DiscreteValueArgs(C.Structure):
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
     ]
 
+
+class BetaDims(C.Structure):
+    _fields_ = [("state_dim", C.c_int32), ("num_items", C.c_int32), ("reserved", C.c_int32 * 2)]
+
+
+class BetaArgs(C.Structure):
+    _fields_ = [
+        ("dims", BetaDims), ("n_rows", C.c_int64), ("chunk_items", C.c_int32), ("reserved", C.c_int32),
+        ("net", Net), ("optim", Optim),
+        ("state", C.c_void_p), ("state_ld", C.c_int64), ("action", C.c_void_p), ("probs_out", C.c_void_p),
+        ("loss", C.c_void_p), ("error", C.c_void_p),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
+_BETA_PROBE_FIELDS = ["dims", "n_rows", "net", "optim", "state", "action", "probs_out", "loss", "error",
+                      "workspace_bytes"]
 
 _PROBE_FIELDS =["dims", "n_rows", "table", "policy", "policy_optim", "gamma", "soft_tau", "masks", "seed",
                  "losses", "workspace_bytes", "comm"]
@@ -147,6 +164,11 @@ SIGNATURES = {
     "recnn_discrete_value_workspace_bytes": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                          C.c_int32]),
     "recnn_discrete_value_step": (C.c_int, [C.POINTER(DiscreteValueArgs), C.c_void_p]),
+    "recnn_beta_layout": (C.c_int, [C.POINTER(BetaDims), C.POINTER(C.c_int64)]),
+    "recnn_beta_workspace_bytes": (C.c_int64, [C.POINTER(BetaDims), C.c_int64, C.c_int32]),
+    "recnn_sizeof_beta_args": (C.c_int64, []),
+    "recnn_offsetof_beta_args": (C.c_int64, [C.c_int]),
+    "recnn_beta_step": (C.c_int, [C.POINTER(BetaArgs), C.c_void_p]),
     "recnn_comm_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]),
     "recnn_comm_handle_bytes": (C.c_int32, []),
     "recnn_comm_local_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -194,6 +216,12 @@ def lib():
     for i, f in enumerate(_PROBE_FIELDS):
         if handle.recnn_offsetof_step_args(i) != getattr(StepArgs, f).offset:
             raise RecnnError("recnn_step_args.%s offset mismatch" % f)
+    if handle.recnn_sizeof_beta_args() != C.sizeof(BetaArgs):
+        raise RecnnError("recnn_beta_args layout mismatch: C %d bytes, ctypes %d bytes"
+                         % (handle.recnn_sizeof_beta_args(), C.sizeof(BetaArgs)))
+    for i, f in enumerate(_BETA_PROBE_FIELDS):
+        if handle.recnn_offsetof_beta_args(i) != getattr(BetaArgs, f).offset:
+            raise RecnnError("recnn_beta_args.%s offset mismatch" % f)
     _LIB = handle
     return handle
 

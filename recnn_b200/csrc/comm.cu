@@ -286,9 +286,11 @@ int launch_comm_allreduce(const recnn_comm* comm, float* buf, int64_t n, const C
   opt.kind = RECNN_OPT_EXTERNAL;
   if (r.optim && r.optim->kind != RECNN_OPT_EXTERNAL) {
     RECNN_REQUIRE(r.net && r.net->params && r.net->opt_t, "fused optimizer needs params and the step counter");
-    RECNN_REQUIRE(r.optim->kind == RECNN_OPT_SGD || r.optim->kind == RECNN_OPT_ADAM || r.optim->kind == RECNN_OPT_RANGER,
-                  "built-in optimizer kind must be SGD, ADAM or RANGER");
-    if (r.optim->kind == RECNN_OPT_ADAM) RECNN_REQUIRE(r.net->opt_m && r.net->opt_v, "Adam needs exp_avg / exp_avg_sq arenas");
+    RECNN_REQUIRE(r.optim->kind == RECNN_OPT_SGD || r.optim->kind == RECNN_OPT_ADAM || r.optim->kind == RECNN_OPT_RANGER ||
+                      r.optim->kind == RECNN_OPT_RADAM,
+                  "built-in optimizer kind must be SGD, ADAM, RANGER or RADAM");
+    if (r.optim->kind == RECNN_OPT_ADAM || r.optim->kind == RECNN_OPT_RADAM)
+      RECNN_REQUIRE(r.net->opt_m && r.net->opt_v, "Adam / RAdam need exp_avg / exp_avg_sq arenas");
     if (r.optim->kind == RECNN_OPT_RANGER) RECNN_REQUIRE(r.net->opt_m && r.net->opt_v && r.net->opt_slow, "Ranger needs exp_avg / exp_avg_sq / slow arenas");
     if (r.optim->kind == RECNN_OPT_SGD && r.optim->momentum != 0.f) RECNN_REQUIRE(r.net->opt_m, "SGD momentum needs a buffer arena");
     opt.kind = r.optim->kind;

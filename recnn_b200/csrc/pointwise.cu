@@ -377,7 +377,9 @@ __global__ void __launch_bounds__(256)
 optimizer_kernel(int kind, OptConsts k, double beta1, double beta2, double lr, double wd, double n_sma_threshold,
                  int k_look, float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                  float* __restrict__ v, float* __restrict__ slow, int* __restrict__ t_ptr,
-                 const float* __restrict__ grad_scale, long long count, unsigned* ticket, GradSource src) {
+                 const float* __restrict__ grad_scale, long long count, unsigned* ticket, GradSource src,
+                 const unsigned* __restrict__ skip) {
+  if (skip && *skip) return;         // the caller's error word is set: parameters, moments and t stay as they are
   __shared__ OptStep s_st;
   const int t = *t_ptr + 1;
   if (threadIdx.x == 0) s_st = opt_step_scalars(kind, beta1, beta2, lr, wd, n_sma_threshold, k_look, t);
@@ -439,11 +441,14 @@ int launch_bump64(long long* t, cudaStream_t st) {
 }
 
 int launch_optimizer(const recnn_optim& o, const recnn_net& net, int64_t count, const float* grad_scale,
-                     cudaStream_t st, unsigned* ticket, const GradSource* src) {
-  RECNN_REQUIRE(o.kind == RECNN_OPT_SGD || o.kind == RECNN_OPT_ADAM || o.kind == RECNN_OPT_RANGER,
-                "built-in optimizer kind must be SGD, ADAM or RANGER");
+                     cudaStream_t st, unsigned* ticket, const GradSource* src, const unsigned* skip) {
+  RECNN_REQUIRE(o.kind == RECNN_OPT_SGD || o.kind == RECNN_OPT_ADAM || o.kind == RECNN_OPT_RANGER ||
+                    o.kind == RECNN_OPT_RADAM,
+                "built-in optimizer kind must be SGD, ADAM, RANGER or RADAM");
+  RECNN_REQUIRE(!skip || ticket, "a gated optimizer step counts its steps itself (ticket)");
   RECNN_REQUIRE(net.params && net.grads && net.opt_t, "optimizer needs params, grads and the step counter");
-  if (o.kind == RECNN_OPT_ADAM) RECNN_REQUIRE(net.opt_m && net.opt_v, "Adam needs exp_avg / exp_avg_sq arenas");
+  if (o.kind == RECNN_OPT_ADAM || o.kind == RECNN_OPT_RADAM)
+    RECNN_REQUIRE(net.opt_m && net.opt_v, "Adam / RAdam need exp_avg / exp_avg_sq arenas");
   if (o.kind == RECNN_OPT_RANGER) RECNN_REQUIRE(net.opt_m && net.opt_v && net.opt_slow, "Ranger needs exp_avg / exp_avg_sq / slow arenas");
   if (o.kind == RECNN_OPT_SGD && o.momentum != 0.f) RECNN_REQUIRE(net.opt_m, "SGD momentum needs a buffer arena");
   const OptConsts k = opt_consts(o);
@@ -457,7 +462,7 @@ int launch_optimizer(const recnn_optim& o, const recnn_net& net, int64_t count, 
   const int grid = (int)(blocks < 4 * kNumSMs ? (blocks > 0 ? blocks : 1) : 4 * kNumSMs);
   optimizer_kernel<<<grid, 256, 0, st>>>(o.kind, k, o.beta1, o.beta2, o.lr, o.weight_decay, o.n_sma_threshold, o.k,
                                          net.params, net.grads, net.opt_m, net.opt_v, net.opt_slow, net.opt_t,
-                                         grad_scale, count, ticket, gs);
+                                         grad_scale, count, ticket, gs, skip);
   RECNN_CHECK_LAUNCH("optimizer_kernel");
   if (!ticket) {
     bump_counter_kernel<<<1, 1, 0, st>>>(net.opt_t);

@@ -189,7 +189,7 @@ struct OptStep {
   float step_size;     // Adam: lr / (1 - beta1^t); Ranger: -(rectified step size) * lr as torch_optimizer forms it
   float bc2_sqrt;      // Adam: sqrt(1 - beta2^t)
   float wd_lr;         // Ranger: -weight_decay * lr
-  int adaptive;        // Ranger: N_sma > threshold (use the variance term)
+  int adaptive;        // Ranger / RAdam: N_sma past the threshold (use the variance term)
   int lookahead;       // Ranger: t % k == 0 (interpolate towards / reset to the slow weights)
   int first;           // Ranger: first step (slow weights start as a copy of the parameters)
 };
@@ -203,12 +203,14 @@ __device__ __forceinline__ OptStep opt_step_scalars(int kind, double beta1, doub
     const double bc2 = 1.0 - pow(beta2, (double)t);
     s.step_size = (float)(lr / bc1);
     s.bc2_sqrt = (float)sqrt(bc2);
-  } else if (kind == RECNN_OPT_RANGER) {
+  } else if (kind == RECNN_OPT_RANGER || kind == RECNN_OPT_RADAM) {
     const double beta2_t = pow(beta2, (double)t);
     const double n_sma_max = 2.0 / (1.0 - beta2) - 1.0;
     const double n_sma = n_sma_max - 2.0 * t * beta2_t / (1.0 - beta2_t);
+    // torch_optimizer.RAdam rectifies from N_sma >= 5 on; Ranger past its N_sma_threshhold
+    const bool rectify = kind == RECNN_OPT_RADAM ? n_sma >= 5.0 : n_sma > n_sma_threshold;
     double step_size;
-    if (n_sma > n_sma_threshold) {
+    if (rectify) {
       step_size = sqrt((1.0 - beta2_t) * (n_sma - 4.0) / (n_sma_max - 4.0) * (n_sma - 2.0) / n_sma * n_sma_max /
                        (n_sma_max - 2.0)) / (1.0 - pow(beta1, (double)t));
       s.adaptive = 1;
@@ -217,17 +219,17 @@ __device__ __forceinline__ OptStep opt_step_scalars(int kind, double beta1, doub
     }
     s.step_size = (float)(-step_size * lr);
     s.wd_lr = (float)(-wd * lr);
-    s.lookahead = (k_look > 0 && t % k_look == 0) ? 1 : 0;
+    s.lookahead = (kind == RECNN_OPT_RANGER && k_look > 0 && t % k_look == 0) ? 1 : 0;
   }
   return s;
 }
-// one element of torch.optim.SGD / Adam (torch 2.11 single-tensor op order) or torch_optimizer.Ranger;
-// `grad` already carries any clip scale
+// one element of torch.optim.SGD / Adam (torch 2.11 single-tensor op order), torch_optimizer.Ranger or its RAdam half
+// alone (RECNN_OPT_RADAM: no Lookahead, no slow arena); `grad` already carries any clip scale
 __device__ __forceinline__ void opt_apply(int kind, const OptConsts& k, const OptStep& st, int t,
                                           float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
                                           float* __restrict__ slow, long long i, float grad) {
   const float w = p[i];
-  if (kind == RECNN_OPT_RANGER) {
+  if (kind == RECNN_OPT_RANGER || kind == RECNN_OPT_RADAM) {
     // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1-beta2); exp_avg.mul_(beta1).add_(grad, alpha=1-beta1)
     float vi = __fmul_rn(v[i], k.b2);
     vi = __fadd_rn(vi, __fmul_rn(__fmul_rn(k.one_minus_b2, grad), grad));
@@ -235,7 +237,6 @@ __device__ __forceinline__ void opt_apply(int kind, const OptConsts& k, const Op
     mi = __fadd_rn(mi, __fmul_rn(k.one_minus_b1, grad));
     v[i] = vi;
     m[i] = mi;
-    float sl = st.first ? w : slow[i];                 // slow_buffer starts as a copy of the (un-stepped) weights
     float x = w;
     if (k.wd != 0.f) x = __fadd_rn(x, __fmul_rn(st.wd_lr, x));             // p.add_(p, alpha=-wd*lr)
     if (st.adaptive) {
@@ -244,11 +245,14 @@ __device__ __forceinline__ void opt_apply(int kind, const OptConsts& k, const Op
     } else {
       x = __fadd_rn(x, __fmul_rn(st.step_size, mi));                         // p.add_(exp_avg, alpha=-step_size*lr)
     }
-    if (st.lookahead) {
-      sl = __fadd_rn(sl, __fmul_rn(k.alpha, __fsub_rn(x, sl)));              // slow.add_(p - slow, alpha=alpha); p = slow
-      x = sl;
+    if (kind == RECNN_OPT_RANGER) {
+      float sl = st.first ? w : slow[i];               // slow_buffer starts as a copy of the (un-stepped) weights
+      if (st.lookahead) {
+        sl = __fadd_rn(sl, __fmul_rn(k.alpha, __fsub_rn(x, sl)));            // slow.add_(p - slow, alpha=alpha); p = slow
+        x = sl;
+      }
+      if (st.lookahead || st.first) slow[i] = sl;
     }
-    if (st.lookahead || st.first) slow[i] = sl;
     p[i] = x;
     return;
   }
@@ -272,9 +276,11 @@ __device__ __forceinline__ void opt_apply(int kind, const OptConsts& k, const Op
 }
 #endif
 
-// ticket: zero-initialised self-resetting counter; when given, the kernel itself increments *net.opt_t
+// ticket: zero-initialised self-resetting counter; when given, the kernel itself increments *net.opt_t.
+// skip: optional device word; when it is non-zero at run time the step does nothing (t included; needs a ticket)
 int launch_optimizer(const recnn_optim& o, const recnn_net& net, int64_t count, const float* grad_scale,
-                     cudaStream_t st, unsigned* ticket = nullptr, const GradSource* src = nullptr);
+                     cudaStream_t st, unsigned* ticket = nullptr, const GradSource* src = nullptr,
+                     const unsigned* skip = nullptr);
 
 int launch_bump64(long long* t, cudaStream_t st);
 int launch_finish(long long* rng_step, const unsigned* oob, const unsigned* dp_mismatch, float* flags_out,

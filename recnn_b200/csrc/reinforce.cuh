@@ -188,13 +188,15 @@ __global__ void categorical_log_prob_kernel(const float* __restrict__ probs, lon
 // each chunk's logits and turns them into d loss / d logits.  With one chunk this is the plain softmax backward.
 
 // Pass 1: (run_max, run_sum) <- the online max / sum of exp over the logits seen so far (chunk c0 == 0 starts them);
-// za[r] <- z[r, a_r] when the row's action lies in this chunk.  One CTA per row.
+// za[r] <- z[r, a_r] when the row's action lies in this chunk.  z: the chunk's [n, w] logits with row pitch ld.
+// One CTA per row.
 __global__ void __launch_bounds__(kRowThreads)
-logit_stats_kernel(const float* __restrict__ z, long long n, int w, int c0, const long long* __restrict__ action,
-                   float* __restrict__ run_max, float* __restrict__ run_sum, float* __restrict__ za) {
+logit_stats_kernel(const float* __restrict__ z, long long ld, long long n, int w, int c0,
+                   const long long* __restrict__ action, float* __restrict__ run_max, float* __restrict__ run_sum,
+                   float* __restrict__ za) {
   __shared__ float red[32];
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
-    const float* row = z + r * w;
+    const float* row = z + r * ld;
     float m = -INFINITY, s = 0.f;
     for (int j = threadIdx.x; j < w; j += blockDim.x) {     // the same reduction as softmax_rows_kernel
       const float x = row[j];
@@ -283,13 +285,14 @@ reinforce_dlogits_kernel(float* __restrict__ z, long long n, int w, int c0, cons
   }
 }
 
-// out[0] = sum of v[0..n) in a fixed order (one CTA)
-__global__ void __launch_bounds__(1024) sum_rows_kernel(const float* __restrict__ v, long long n, float* __restrict__ out) {
+// out[0] = scale * (sum of v[0..n) in a fixed order)  (one CTA)
+__global__ void __launch_bounds__(1024) sum_rows_kernel(const float* __restrict__ v, long long n, float scale,
+                                                        float* __restrict__ out) {
   __shared__ float red[32];
   float t = 0.f;
   for (long long i = threadIdx.x; i < n; i += blockDim.x) t += v[i];
   t = block_sum(t, red);
-  if (threadIdx.x == 0) out[0] = t;
+  if (threadIdx.x == 0) out[0] = t * scale;
 }
 
 static int row_grid(int64_t n) { return (int)(n < (int64_t)kNumSMs * 8 ? n : (int64_t)kNumSMs * 8); }
@@ -298,31 +301,42 @@ static bool chunk_ok(const recnn_discrete_dims& d, int64_t chunk) {
   return chunk == d.num_items || (chunk > 0 && chunk % 128 == 0 && chunk < d.num_items);
 }
 
-// split-K partial space of the two weight gradients of the policy (either back end) when dW2 is computed in row blocks
-// of `chunk` items, the last one possibly narrower.  dw_splits sees a block's width only through ceil(width / 128) and
-// the partials grow with the width at a fixed split count, so the widest width of every 128-band bounds that band; once
-// both back ends use one split, the partials only grow with the width.  Independent of num_items when chunk < num_items.
-static int64_t reinforce_partial_floats(const recnn_discrete_dims& d, int64_t rows, int chunk) {
+// split-K partial space of a weight gradient dW[C, K] over `rows` (either back end); *one_split: both use one split
+static int64_t dw_partial_floats(int C, int K, int64_t rows, bool* one_split) {
   int64_t best = 0;
-  auto consider = [&](int C, int K) {
-    bool one = true;
-    for (int tcp = 0; tcp < 2; ++tcp) {
-      const int s = dw_splits(C, K, rows, tcp != 0);
-      const int64_t f = (int64_t)s * C * (K + 1);
-      if (f > best) best = f;
-      one = one && s == 1;
-    }
-    return one;
-  };
-  consider(d.hidden, d.state_dim);
-  if (chunk == d.num_items) {
-    consider(chunk, d.hidden);
-  } else {
-    for (int64_t c = 128; c < chunk; c += 128)
-      if (consider((int)c, d.hidden)) break;
-    consider(chunk, d.hidden);
+  bool one = true;
+  for (int tcp = 0; tcp < 2; ++tcp) {
+    const int s = dw_splits(C, K, rows, tcp != 0);
+    const int64_t f = (int64_t)s * C * (K + 1);
+    if (f > best) best = f;
+    one = one && s == 1;
   }
+  if (one_split) *one_split = one;
   return best;
+}
+
+// ... of a weight gradient [num_items, K] computed in row blocks of `chunk` items, the last one possibly narrower.
+// dw_splits sees a block's width only through ceil(width / 128) and the partials grow with the width at a fixed split
+// count, so the widest width of every 128-band bounds that band; once both back ends use one split, the partials only
+// grow with the width.  Independent of num_items when chunk < num_items.
+static int64_t chunked_partial_floats(int chunk, int num_items, int K, int64_t rows) {
+  int64_t best = 0;
+  if (chunk != num_items) {
+    bool one = false;
+    for (int64_t c = 128; c < chunk && !one; c += 128) {
+      const int64_t f = dw_partial_floats((int)c, K, rows, &one);
+      if (f > best) best = f;
+    }
+  }
+  const int64_t f = dw_partial_floats(chunk, K, rows, nullptr);
+  return f > best ? f : best;
+}
+
+// the two weight gradients of the policy, dW2 in row blocks of `chunk` items
+static int64_t reinforce_partial_floats(const recnn_discrete_dims& d, int64_t rows, int chunk) {
+  const int64_t f1 = dw_partial_floats(d.hidden, d.state_dim, rows, nullptr);
+  const int64_t f2 = chunked_partial_floats(chunk, d.num_items, d.hidden, rows);
+  return f1 > f2 ? f1 : f2;
 }
 
 struct DiscreteScratch {
@@ -471,13 +485,14 @@ extern "C" int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d,
   for (int c = 0; c < n_chunks; ++c) {
     const int c0 = c * W, w = I - c0 < W ? I - c0 : W;
     RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, c0, w, s.z, st));
-    logit_stats_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(s.z, n_rows, w, c0, act, s.run_max, s.run_sum, s.za);
+    logit_stats_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(s.z, w, n_rows, w, c0, act, s.run_max, s.run_sum,
+                                                                  s.za);
     RECNN_CHECK_LAUNCH("logit_stats_kernel");
   }
   reinforce_row_weights_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
       n_rows, I, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss, s.flags);
   RECNN_CHECK_LAUNCH("reinforce_row_weights_kernel");
-  sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n_rows, out);
+  sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n_rows, 1.f, out);
   RECNN_CHECK_LAUNCH("sum_rows_kernel");
   // pass 2, last chunk first (its logits are still in the buffer): dz = d loss / d logits of the chunk;
   // dW2[c0:c0+w] = dz^T h, db2[c0:c0+w] = colsum dz; dh (+)= dz W2[c0:c0+w], gated by [h > 0] after the last term

@@ -10,6 +10,7 @@
 // semantics: the wgmma 3xTF32 tensor-core kernel (tc_gemm.cuh; default) and
 // the exact-fp32 CUDA-core kernel (gemm_simt.cuh; arbitrary shapes, and
 // RECNN_B200_MATH=simt forces it for A/B comparisons).
+#include <stddef.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -837,15 +838,17 @@ extern "C" int64_t recnn_forward_scratch_floats(const recnn_dims* d, int64_t n_r
   return 2 * n_rows * d->hidden + n_rows * ldS + (is_critic ? n_rows * ldA : 0) + 64;
 }
 
-// state [n, S] (pitch S) -> a pitch-ldS image when needed; returns the Seg to read
-static int repitch_state(const recnn_dims& d, const float* state, int64_t n, float* img, Seg* out, cudaStream_t st) {
+// state [n, S] (row pitch ld; 0: S) -> a pitch-ldS image when needed; returns the Seg to read
+static int repitch_state(const recnn_dims& d, const float* state, int64_t n, float* img, Seg* out, cudaStream_t st,
+                         long long ld = 0) {
   const int S = d.state_dim;
-  if (S % 4 == 0 && aligned16(state)) {
-    *out = Seg{state, S, S, 0};
+  if (ld == 0) ld = S;
+  if (S % 4 == 0 && ld % 4 == 0 && aligned16(state)) {
+    *out = Seg{state, S, ld, 0};
     return RECNN_OK;
   }
   const int ldS = pad4(S);
-  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(img, (size_t)ldS * 4, state, (size_t)S * 4, (size_t)S * 4, n,
+  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(img, (size_t)ldS * 4, state, (size_t)ld * 4, (size_t)S * 4, n,
                                      cudaMemcpyDeviceToDevice, st));
   *out = Seg{img, S, ldS, 0};
   return RECNN_OK;
@@ -929,3 +932,5 @@ extern "C" int recnn_linear_forward(const float* x, int64_t n_rows, int in_dim, 
 #include "reinforce.cuh"
 // ---------------------------------------------------------------- REINFORCE (critic side, item-id actions)
 #include "critic_ids.cuh"
+// ---------------------------------------------------------------- REINFORCE Top-K: the behaviour policy beta
+#include "beta.cuh"

@@ -25,7 +25,14 @@ def _is_discrete(module):
     return not hasattr(module, "linear3")
 
 
+def _is_beta(module):
+    """The Top-K notebook's behaviour policy (nn.Beta): one nn.Linear in ``module.net[0]``."""
+    return getattr(module, "_recnn_beta", False)
+
+
 def _params(module):
+    if _is_beta(module):
+        return [module.net[0].weight, module.net[0].bias]
     ps = [module.linear1.weight, module.linear1.bias, module.linear2.weight, module.linear2.bias]
     if not _is_discrete(module):
         ps += [module.linear3.weight, module.linear3.bias]
@@ -38,7 +45,12 @@ def discrete_dims(module):
 
 def net_layout(module):
     """(offsets[6], pitches[3], count) of this module's arena, from the C library (4 offsets / 2 pitches for the
-    two-layer DiscreteActor)."""
+    two-layer DiscreteActor, 2 offsets / 1 pitch for nn.Beta)."""
+    if _is_beta(module):
+        buf = (ctypes.c_int64 * 4)()
+        _lib.check(_lib.lib().recnn_beta_layout(module.dims, buf))
+        v = list(buf)
+        return v[0:2], v[2:3], v[3]
     if _is_discrete(module):
         buf = (ctypes.c_int64 * 7)()
         _lib.check(_lib.lib().recnn_discrete_layout(discrete_dims(module), buf))

@@ -45,7 +45,8 @@ class _ArenaOptimizer(torch.optim.Optimizer):
         if self._t is None:
             self._t = torch.zeros(1, dtype=torch.int32, device=flat.device)
             self._m = torch.zeros_like(flat)
-            self._v = torch.zeros_like(flat) if self._recnn_kind in (_lib.OPT_ADAM, _lib.OPT_RANGER) else None
+            self._v = (torch.zeros_like(flat) if self._recnn_kind in (_lib.OPT_ADAM, _lib.OPT_RANGER, _lib.OPT_RADAM)
+                       else None)
             self._slow = torch.zeros_like(flat) if self._recnn_kind == _lib.OPT_RANGER else None
         elif self._t.device != flat.device or self._m.numel() != flat.numel():
             if self._m.numel() != flat.numel():
@@ -159,3 +160,20 @@ class Ranger(_ArenaOptimizer):
         return _lib.Optim(_lib.OPT_RANGER, int(g["k"]), float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]),
                           float(g["eps"]), float(g["weight_decay"]), 0.0, float(g["alpha"]),
                           float(g["N_sma_threshhold"]))
+
+
+class RAdam(_ArenaOptimizer):
+    """torch_optimizer.RAdam, the optimizer of the Top-K notebook's behaviour policy (``optim.RAdam(lr=1e-5,
+    weight_decay=1e-5)``), with the package's signature and defaults: rectified Adam switched on from N_sma >= 5 and
+    decoupled weight decay -- Ranger's RAdam half without Lookahead.  Pinned against
+    ``torch.optim.RAdam(decoupled_weight_decay=True)``; parity with the package itself is UNPINNED, as for Ranger
+    (DESIGN.md section 2)."""
+    _recnn_kind = _lib.OPT_RADAM
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0):
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+
+    def c_optim(self):
+        g = self.param_groups[0]
+        return _lib.Optim(_lib.OPT_RADAM, 0, float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]),
+                          float(g["eps"]), float(g["weight_decay"]), 0.0, 0.0, 5.0)
