@@ -53,6 +53,8 @@ def build_optimizers(kind, nets, algo, external=False):
                 torch.optim.SGD(net.parameters(), lr=1e-3)
         if kind == "ranger":
             return recnn_b200.optim.Ranger(net.parameters(), lr=1e-4, weight_decay=1e-2)
+        if kind == "sgd_momentum":
+            return recnn_b200.optim.SGD(net.parameters(), lr=1e-3, momentum=0.9, weight_decay=1e-3)
         return recnn_b200.optim.Adam(net.parameters(), lr=1e-5) if kind == "adam" else \
             recnn_b200.optim.SGD(net.parameters(), lr=1e-3)
     names = {"policy_optimizer": "policy_net"}
@@ -65,9 +67,12 @@ def build_optimizers(kind, nets, algo, external=False):
 
 
 def run_cuda_case(case, algo, opt_kind, golden=None, form="dense", external=False, device="cuda:0",
-                  shard=None, inp=None):
+                  shard=None, inp=None, comm=None, on_step=None):
     """shard=(rank, world): this process handles rows [lo, hi) of every minibatch (data parallel).
-    ``inp``: pre-made inputs (C.make_inputs, possibly with edited masks) instead of regenerating them."""
+    ``inp``: pre-made inputs (C.make_inputs, possibly with edited masks) instead of regenerating them.
+    ``comm``: callable nets -> peer communicator (an object with ``.ptr``), attached before the first update so the
+    step runs its gradient all-reduce kernels through it.  ``on_step(step, nets, opts, loss)``: called after each
+    update."""
     spec = C.CASES[case] if isinstance(case, str) else case      # a name or a spec dict
     if inp is None:
         inp = C.make_inputs(spec, algo)
@@ -78,6 +83,8 @@ def run_cuda_case(case, algo, opt_kind, golden=None, form="dense", external=Fals
     opts = build_optimizers(opt_kind, nets, algo, external)
     if shard is not None:
         recnn_b200.dist.enable_data_parallel(nets)
+    if comm is not None:           # read by get_engine when it creates the engine, i.e. on the first update
+        nets["policy_net"].__dict__["_recnn_dp"] = (None, 1, comm(nets))
     params = dict(C.DDPG_PARAMS if algo == "ddpg" else C.TD3_PARAMS)
     table = torch.from_numpy(inp["table"]).to(dev)
     ref = O.frame_gather(inp["table"], inp["items"], inp["ratings"], inp["sizes"], spec["frame"])
@@ -100,6 +107,8 @@ def run_cuda_case(case, algo, opt_kind, golden=None, form="dense", external=Fals
             batch["noise"] = torch.from_numpy(np.ascontiguousarray(nz[lo:hi]))
         loss = update(batch, params, nets, opts, dev, {}, recnn_b200.utils.DummyWriter(), learn=True, step=step)
         assert loss["step"] == step
+        if on_step is not None:
+            on_step(step, nets, opts, loss)
         for k in loss_keys:
             losses[k].append(loss[k])
         done_steps = step + 1

@@ -21,6 +21,7 @@ def load_golden(name):
 def oracle_optimizers(kind, algo):
     mk = (lambda: O.make_optimizer("adam", lr=1e-5)) if kind == "adam" else \
          (lambda: O.make_optimizer("ranger", lr=1e-4, weight_decay=1e-2)) if kind == "ranger" else \
+         (lambda: O.make_optimizer("sgd", lr=1e-3, momentum=0.9, weight_decay=1e-3)) if kind == "sgd_momentum" else \
          (lambda: O.make_optimizer("sgd", lr=1e-3))
     names = ("policy_optimizer", "value_optimizer") if algo == "ddpg" else \
             ("policy_optimizer", "value_optimizer1", "value_optimizer2")
@@ -140,6 +141,35 @@ def assert_tight_parity(got, want, init_nets, loss_rtol=1e-5, rtol=1e-5, floor_f
         rep["delta"] = max(rep["delta"], float(np.max(excess[~bad])))
         rep["outliers"] = max(rep["outliers"], n_bad)
         rep["checked"] += 1
+    return rep
+
+
+def assert_oracle_bar(got, want, init_nets, rtol=1e-5):
+    """The bar of the optimizers without golden fixtures (Ranger, SGD with momentum) against run_oracle_case: losses
+    within 1e-5 of |want| + 0.1; every final weight within ``rtol`` relative (floor: 1e-2 of the tensor's largest weight);
+    every weight change within 2e-3 of the tensor's largest change, beyond 2 ulp of its largest weight.  A tensor that
+    does not move must stay bit-identical.  Returns the largest error found on each bar."""
+    rep = {"loss": 0.0, "weight": 0.0, "delta": 0.0}
+    for k in (k for k in want if k.startswith("loss.")):
+        err = float(np.max(np.abs(got[k] - want[k]) / (np.abs(want[k]) + 0.1)))
+        rep["loss"] = max(rep["loss"], err)
+        assert err <= 1e-5, (k, err)
+    for k in (k for k in want if k.startswith("final.")):
+        _, name, tensor = k.split(".")
+        w = want[k].astype(np.float64)
+        wmax = np.max(np.abs(w))
+        err = float(np.max(np.abs(got[k] - w) / (np.abs(w) + 1e-2 * wmax)))
+        rep["weight"] = max(rep["weight"], err)
+        assert err <= rtol, (k, err)
+        d_want = w - init_nets[name][tensor]
+        scale = np.max(np.abs(d_want))
+        if scale == 0:
+            assert np.array_equal(got[k], want[k]), k
+            continue
+        ulp2 = 2.0 * 1.1920929e-07 * wmax
+        excess = float(np.max(np.maximum(np.abs((got[k] - init_nets[name][tensor]) - d_want) - ulp2, 0)) / scale)
+        rep["delta"] = max(rep["delta"], excess)
+        assert excess <= 2e-3, (k, excess)
     return rep
 
 

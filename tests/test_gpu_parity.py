@@ -11,7 +11,7 @@ import recnn_b200
 from recnn_b200 import _lib
 from oracle import cases as C
 from oracle import recnn_oracle as O
-from tests._golden import load_golden, compare_with_golden, run_oracle_case
+from tests._golden import assert_oracle_bar, load_golden, compare_with_golden, run_oracle_case
 from tests._cuda import run_cuda_case
 
 pytestmark = pytest.mark.gpu
@@ -625,22 +625,7 @@ def test_ranger_step_vs_oracle(case, algo):
     want = run_oracle_case(case, algo, "ranger")
     got = run_cuda_case(case, algo, "ranger", form="frames")
     inp = C.make_inputs(C.CASES[case], algo)
-    for k in (k for k in want if k.startswith("loss.")):
-        err = np.max(np.abs(got[k] - want[k]) / (np.abs(want[k]) + 0.1))
-        assert err <= 1e-5, (k, err)
-    for k in (k for k in want if k.startswith("final.")):
-        _, name, tensor = k.split(".")
-        w = want[k].astype(np.float64)
-        wmax = np.max(np.abs(w))
-        assert np.max(np.abs(got[k] - w) / (np.abs(w) + 1e-2 * wmax)) <= 1e-5, k
-        d_want = w - inp["nets"][name][tensor]
-        scale = np.max(np.abs(d_want))
-        if scale == 0:
-            assert np.array_equal(got[k], want[k]), k
-            continue
-        ulp2 = 2.0 * 1.1920929e-07 * wmax
-        excess = np.maximum(np.abs((got[k] - inp["nets"][name][tensor]) - d_want) - ulp2, 0)
-        assert np.max(excess) <= 2e-3 * scale, (k, float(np.max(excess) / scale))
+    assert_oracle_bar(got, want, inp["nets"])
 
 
 def test_default_optimizers_are_ranger_like_the_reference():

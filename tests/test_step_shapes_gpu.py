@@ -137,14 +137,16 @@ def sweep_worker(in_path, out_path):
         pickle.dump(out, f)
 
 
-def run_sweep(tmp_path, keys, **env):
-    """Run the CUDA side of ``keys`` in a fresh process with ``env`` set; returns (results, stderr)."""
+def run_sweep(tmp_path, keys, worker="tests.test_step_shapes_gpu:sweep_worker", **env):
+    """Run the CUDA side of ``keys`` in a fresh process with ``env`` set; returns (results, stderr).  ``worker``:
+    "module:function" taking (inputs pickle, results pickle), sweep_worker's contract."""
     cases = {k: prepared(*k[:3])[:2] for k in keys}
     in_path, out_path = str(tmp_path / "cases.pkl"), str(tmp_path / "results.pkl")
     with open(in_path, "wb") as f:
         pickle.dump(cases, f)
-    code = ("import sys; sys.path.insert(0, %r); from tests import test_step_shapes_gpu as T; T.sweep_worker(%r, %r)"
-            % (ROOT, in_path, out_path))
+    mod, fn = worker.split(":")
+    code = ("import sys, importlib; sys.path.insert(0, %r); importlib.import_module(%r).%s(%r, %r)"
+            % (ROOT, mod, fn, in_path, out_path))
     e = dict(os.environ)
     for k in ("RECNN_B200_MATH", "RECNN_B200_OVERLAP", "RECNN_B200_FUSE_HEAD", "RECNN_B200_DEBUG", "RECNN_B200_GRAPHS"):
         e.pop(k, None)
