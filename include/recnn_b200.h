@@ -371,6 +371,67 @@ RECNN_API int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d, 
 /* floats of scratch for recnn_reinforce_policy_grad_chunked; 0 when chunk_items is not accepted */
 RECNN_API int64_t recnn_reinforce_scratch_floats(const recnn_discrete_dims* d, int64_t n_rows, int32_t chunk_items);
 
+/* ---- REINFORCE: the policy sharded over the item vocabulary across the GPUs of one node -----------
+ * Rank `rank` of `world` holds rows [item_offset, item_offset + d->num_items) of linear2 (weight and bias) in its
+ * arena: d is the LOCAL dims, so recnn_discrete_layout applies unchanged; linear1 is replicated.  Action ids stay
+ * global.  The host issues the phases on one stream with two exchanges between them (recnn_comm_allgather of the
+ * records below, and recnn_comm_allreduce of the layer-1 gradient), so a sharded update stays graph-capturable.
+ * A record (recnn_vocab_record_floats(n_rows) floats) is a header of four int32 words {lo, hi, num_items, n_rows}
+ * followed by three planes of n_rows floats: the local max of the logits, the local sum of exp(z - max) and the logit
+ * of the row's action (from the rank that owns it, 0 on the others).  "gathered" is the W records in rank order.
+ * Every rank merges them in rank order, so all ranks compute the same bits; at world 1 every phase computes exactly
+ * what the unsharded call does. */
+typedef struct recnn_vocab_shard {
+  int32_t item_offset;   /* the global id of the rank's first item */
+  int32_t num_items;     /* the whole vocabulary */
+  int32_t rank, world;
+} recnn_vocab_shard;
+RECNN_API int64_t recnn_vocab_record_floats(int64_t n_rows);
+/* Policy gradient, phase 1: the hidden layer, then pass 1 over the local items in chunks of chunk_items -> record.
+ * scratch: fp32[recnn_reinforce_scratch_floats(d, n_rows, chunk_items)] (local dims; it does not grow with the
+ * vocabulary once chunk_items < d->num_items); phase 2 must get the same scratch, untouched in between. */
+RECNN_API int recnn_reinforce_shard_stats(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                          const float* state, const int64_t* action, int64_t n_rows,
+                                          int32_t chunk_items, float* record, float* scratch, void* stream);
+/* Phase 2, after the all-gather: merge the gathered records, row weights and loss, pass 2 over the local chunks
+ * (dW2 / db2 of the local rows), then this rank's share of the layer-1 gradient into grads[0 : w2 offset) -- the
+ * caller all-reduces that block (recnn_comm_allreduce) to get dW1 / db1.  out[0] = loss (same bits on every rank);
+ * out[1] = int32 flag: an action id was outside [0, num_items) (that row contributed nothing); out[2] = int32 flag:
+ * the gathered headers do not tile the vocabulary in rank order with this rank's rows (the ranks disagree on the
+ * shard plan or on n_rows; the gradient is then meaningless). */
+RECNN_API int recnn_reinforce_shard_grad(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                         float* grads, const float* state, const int64_t* action,
+                                         const float* beta_log_prob, const float* returns, int64_t n_rows,
+                                         int32_t method, int32_t top_k, int32_t chunk_items, const float* gathered,
+                                         float* out, float* scratch, void* stream);
+/* Forward: the local logits into probs_out [n_rows, d->num_items] and the record (action-logit plane 0).
+ * scratch: fp32[recnn_discrete_scratch_floats(d, n_rows, 0)] */
+RECNN_API int recnn_discrete_shard_forward(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                           const float* params, const float* state, int64_t n_rows, float* probs_out,
+                                           float* record, float* scratch, void* stream);
+/* ... after the all-gather: probs <- exp(z - M) / S, the rank's column block of the softmax over the whole vocabulary.
+ * *error_flag <- 1 when the headers disagree (as out[2] above). */
+RECNN_API int recnn_discrete_shard_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                          const float* gathered, int64_t n_rows, float* probs, int32_t* error_flag,
+                                          void* stream);
+/* One draw per row over the whole vocabulary (u as recnn_categorical_sample: uniforms, or Philox(seed, draw, row) --
+ * the same u on every rank).  From the gathered records every rank finds the rank whose share of the cumulative mass
+ * holds u; that rank draws inside its block at the conditional uniform.  draw_record [2, n_rows]: the global id as
+ * int32 bits (-1 on every rank but the owner), then its log-prob.  Exchange it with recnn_comm_allgather and read it
+ * with recnn_discrete_shard_pick. */
+RECNN_API int recnn_discrete_shard_sample(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                          const float* gathered, const float* probs, int64_t n_rows,
+                                          const float* uniforms, uint64_t seed, int64_t draw, float* draw_record,
+                                          void* stream);
+/* The log-prob of given global ids (probs: the finished block), as a draw record; *oob_flag when an id is out of range */
+RECNN_API int recnn_discrete_shard_log_prob(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                            const float* probs, int64_t n_rows, const int64_t* action,
+                                            float* draw_record, int32_t* oob_flag, void* stream);
+/* gathered draw records [world][2][n_rows] -> action_out int64 [n_rows], log_prob_out [n_rows]; *error_flag <- 1 when
+ * a row was claimed by no rank or by several (the ranks used different uniforms, or an id was out of range) */
+RECNN_API int recnn_discrete_shard_pick(int32_t world, const float* gathered_draws, int64_t n_rows,
+                                        int64_t* action_out, float* log_prob_out, int32_t* error_flag, void* stream);
+
 /* ---- REINFORCE: the critic side with item-id actions ---------------------------------------------
  * The REINFORCE critic is a Critic(S, num_items, H) (recnn/nn/update/reinforce.py:92-102): layer 1 is W1 [H, S + num_items]
  * on [state | action], the action being a one-hot row (the batch) or a probability row (the target policy's output).
@@ -486,6 +547,10 @@ RECNN_API int recnn_comm_connect(recnn_comm* comm, const void* all_handles);
 /* buf[i] <- sum over ranks of buf[i], in place, identical bits on every rank (n <= capacity_floats);
  * every rank must issue the same sequence of collectives on ONE stream. */
 RECNN_API int recnn_comm_allreduce(const recnn_comm* comm, float* buf, int64_t n, void* stream);
+/* gathered[q * n + i] <- rank q's local[i], rank-major, the same on every rank; words move as bit patterns (integer
+ * payloads survive).  n * world <= capacity_floats, else refused before any launch.  Shares the epoch sequence of
+ * recnn_comm_allreduce: the two may interleave on one communicator, in the same order on every rank. */
+RECNN_API int recnn_comm_allgather(const recnn_comm* comm, const float* local, int64_t n, float* gathered, void* stream);
 RECNN_API int recnn_comm_destroy(recnn_comm* comm);
 
 #ifdef __cplusplus

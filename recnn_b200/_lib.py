@@ -31,6 +31,10 @@ class DiscreteDims(C.Structure):
     _fields_ = [("state_dim", C.c_int32), ("hidden", C.c_int32), ("num_items", C.c_int32), ("reserved", C.c_int32)]
 
 
+class VocabShard(C.Structure):
+    _fields_ = [("item_offset", C.c_int32), ("num_items", C.c_int32), ("rank", C.c_int32), ("world", C.c_int32)]
+
+
 class Net(C.Structure):
     _fields_ = [("params", C.c_void_p), ("grads", C.c_void_p), ("opt_m", C.c_void_p),
                 ("opt_v", C.c_void_p), ("opt_t", C.c_void_p), ("opt_slow", C.c_void_p)]
@@ -153,6 +157,22 @@ SIGNATURES = {
                                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
                                                       C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_reinforce_scratch_floats": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32]),
+    "recnn_vocab_record_floats": (C.c_int64, [C.c_int64]),
+    "recnn_reinforce_shard_stats": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_reinforce_shard_grad": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                             C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_shard_forward": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                               C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_shard_finish": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_int64,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_shard_sample": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                              C.c_int64, C.c_void_p, C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_shard_log_prob": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_int64,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_shard_pick": (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]),
     "recnn_critic_action_term_scratch_floats": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                             C.c_int32]),
     "recnn_critic_action_term_chunked": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.POINTER(DiscreteDims), C.c_void_p,
@@ -174,6 +194,7 @@ SIGNATURES = {
     "recnn_comm_local_handle": (C.c_int, [C.c_void_p, C.c_void_p]),
     "recnn_comm_connect": (C.c_int, [C.c_void_p, C.c_void_p]),
     "recnn_comm_allreduce": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_comm_allgather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "recnn_comm_destroy": (C.c_int, [C.c_void_p]),
 }
 

@@ -194,7 +194,7 @@ extern "C" int recnn_beta_step(const recnn_beta_args* a, void* stream) {
     const int c0 = c * W, wc = I - c0 < W ? I - c0 : W;
     RECNN_PROPAGATE(linear_out(xs, P + l.w + (int64_t)c0 * l.ldw, l.ldw, P + l.b + c0, wc, n, 0, nullptr, probs + c0, I,
                                st));
-    logit_stats_kernel<<<row_grid(n), kRowThreads, 0, st>>>(probs + c0, I, n, wc, c0, act, w.run_max, w.run_sum, w.za);
+    logit_stats_kernel<<<row_grid(n), kRowThreads, 0, st>>>(probs + c0, I, n, wc, c0, act, 0, w.run_max, w.run_sum, w.za);
     RECNN_CHECK_LAUNCH("logit_stats_kernel");
   }
   beta_rows_kernel<<<row_grid(n), kRowThreads, 0, st>>>(probs, I, n, I, act, w.run_max, w.run_sum, w.za, w.T, w.pe,

@@ -103,17 +103,20 @@ __device__ __forceinline__ void comm_timeout(int rank, unsigned e, const char* w
   printf("recnn_b200 allreduce: rank %d timed out waiting for %s (epoch %u)\n", rank, what, e);
   __trap();
 }
-// spin until the word carries epoch e; returns its value
-__device__ __forceinline__ float wait_ll(const ll_word* p, unsigned e, int rank, const char* what) {
+// spin until the word carries epoch e; returns its payload bits
+__device__ __forceinline__ unsigned wait_ll_bits(const ll_word* p, unsigned e, int rank, const char* what) {
   ll_word w = ld_ll(p);
-  if ((unsigned)(w >> 32) == e) return __uint_as_float((unsigned)w);
+  if ((unsigned)(w >> 32) == e) return (unsigned)w;
   const unsigned long long t0 = comm_gtimer();
   unsigned spins = 0;
   for (;;) {
     w = ld_ll(p);
-    if ((unsigned)(w >> 32) == e) return __uint_as_float((unsigned)w);
+    if ((unsigned)(w >> 32) == e) return (unsigned)w;
     if ((++spins & 1023u) == 0 && comm_gtimer() - t0 > 20000000000ull) comm_timeout(rank, e, what);
   }
+}
+__device__ __forceinline__ float wait_ll(const ll_word* p, unsigned e, int rank, const char* what) {
+  return __uint_as_float(wait_ll_bits(p, e, rank, what));
 }
 __device__ __forceinline__ void wait_ll2(const ll_word* p, unsigned e, int rank, const char* what, float& v0, float& v1) {
   const unsigned long long t0 = comm_gtimer();
@@ -276,6 +279,62 @@ allreduce_kernel(CommPeers c, float* __restrict__ buf, long long n, float max_no
   }
 }
 
+// All-gather in the same word protocol: every rank stores its n words, as raw bits, into slot [my rank] of the
+// contribution buffer of every peer (epoch e, buffer e & 1), then waits for the W slots of its own buffer and writes
+// them out rank-major.  It takes an epoch from the same counter as allreduce_kernel, so the two interleave freely.
+// grid <= number of SMs (all CTAs of all ranks resident at once), n <= slice_cap.
+__global__ void __launch_bounds__(kCommThreads, 1)
+allgather_kernel(CommPeers c, const unsigned* __restrict__ local, long long n, unsigned* __restrict__ gathered) {
+  __shared__ unsigned s_epoch;
+  __shared__ bool s_last;
+  CommDev* me = c.ctrl[c.rank];
+  if (threadIdx.x == 0) s_epoch = *((volatile unsigned*)&me->epoch) + 1;
+  __syncthreads();
+  const unsigned e = s_epoch;
+  const int par = (int)(e & 1u);
+  const int W = c.world;
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nth = (long long)gridDim.x * blockDim.x;
+  for (long long i = tid; i < n; i += nth) {
+    const ll_word w = ((ll_word)e << 32) | (ll_word)local[i];
+    for (int p = 0; p < W; ++p) {
+      ll_word* dst = c.contrib[p] + ((long long)par * W + c.rank) * c.slice_cap + i;
+      asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(dst), "l"(w) : "memory");
+    }
+  }
+  const ll_word* mine = c.contrib[c.rank] + (long long)par * W * c.slice_cap;
+  for (long long i = tid; i < n; i += nth)
+    for (int q = 0; q < W; ++q) gathered[q * n + i] = wait_ll_bits(mine + (long long)q * c.slice_cap + i, e, c.rank, "a peer's slot");
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicInc(&me->done, gridDim.x - 1) == gridDim.x - 1;
+  __syncthreads();
+  if (s_last && threadIdx.x == 0) *((volatile unsigned*)&me->epoch) = e;
+}
+
+// every CTA must be resident at once: at most one per SM of THIS device (and no more than the L1-partials array holds)
+static int comm_grid(int64_t n, int* grid) {
+  int dev = 0, sms = 0;
+  RECNN_CHECK_CUDA(cudaGetDevice(&dev));
+  RECNN_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int cap = sms < kNumSMs ? sms : kNumSMs;
+  const int64_t blocks = ceil_div(n, (int64_t)kCommThreads * 8);   // eight words per thread
+  *grid = (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
+  return RECNN_OK;
+}
+
+int launch_comm_allgather(const recnn_comm* comm, const float* local, int64_t n, float* gathered, cudaStream_t st) {
+  RECNN_REQUIRE(comm != nullptr && comm->connected, "communicator is not connected");
+  RECNN_REQUIRE(n >= 0 && n * comm->peers.world <= comm->peers.capacity,
+                "all-gather larger than the communicator's staging capacity (n * world > capacity)");
+  RECNN_REQUIRE(n == 0 || (local != nullptr && gathered != nullptr), "local / gathered");
+  int grid = 1;
+  RECNN_PROPAGATE(comm_grid(n, &grid));
+  allgather_kernel<<<grid, kCommThreads, 0, st>>>(comm->peers, reinterpret_cast<const unsigned*>(local), n,
+                                                   reinterpret_cast<unsigned*>(gathered));
+  RECNN_CHECK_LAUNCH("allgather_kernel");
+  return RECNN_OK;
+}
+
 int launch_comm_allreduce(const recnn_comm* comm, float* buf, int64_t n, const CommReduce& r, cudaStream_t st) {
   RECNN_REQUIRE(comm != nullptr && comm->connected, "communicator is not connected");
   RECNN_REQUIRE(n >= 0 && n <= comm->peers.capacity, "all-reduce larger than the communicator's staging capacity");
@@ -302,14 +361,8 @@ int launch_comm_allreduce(const recnn_comm* comm, float* buf, int64_t n, const C
   GradSource gsrc;
   memset(&gsrc, 0, sizeof(gsrc));
   if (r.src) gsrc = *r.src;
-  const int64_t per = (int64_t)kCommThreads * 8;                   // eight floats per thread
-  int64_t blocks = ceil_div(n, per);
-  // every CTA must be resident at once: at most one per SM of THIS device (and no more than the L1-partials array holds)
-  int dev = 0, sms = 0;
-  RECNN_CHECK_CUDA(cudaGetDevice(&dev));
-  RECNN_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int cap = sms < kNumSMs ? sms : kNumSMs;
-  const int grid = (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
+  int grid = 1;
+  RECNN_PROPAGATE(comm_grid(n, &grid));
   // partial-sourced gradients are read four at a time: the arena case (n % 4 == 0, 16-byte aligned)
   const bool vec = (n & 1) == 0 && ((reinterpret_cast<uintptr_t>(buf) & 7) == 0) &&
                    (!r.src || ((n & 3) == 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0));
@@ -408,6 +461,10 @@ extern "C" int recnn_comm_connect(recnn_comm* c, const void* all_handles) {
 
 extern "C" int recnn_comm_allreduce(const recnn_comm* c, float* buf, int64_t n, void* stream) {
   return launch_comm_allreduce(c, buf, n, CommReduce(), static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int recnn_comm_allgather(const recnn_comm* c, const float* local, int64_t n, float* gathered, void* stream) {
+  return launch_comm_allgather(c, local, n, gathered, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int recnn_comm_destroy(recnn_comm* c) {

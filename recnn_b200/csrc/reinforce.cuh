@@ -96,64 +96,73 @@ __device__ __forceinline__ float clamped_log_prob(float p) {
   return logf(fminf(fmaxf(p, kProbEps), 1.f - kProbEps));
 }
 
+// The uniform of row r's draw: uniforms[r] (replayable) or Philox keyed by (seed, draw, row), in [0, 1).
+__device__ __forceinline__ float draw_uniform(const float* uniforms, unsigned long long seed, long long draw, long long r) {
+  if (uniforms) return uniforms[r];
+  Philox ph(seed);
+  const uint4 q = ph((unsigned long long)r, ((unsigned long long)draw << 8) | 0x5au);
+  return (float)(q.x >> 8) * (1.0f / 16777216.0f);
+}
+
+struct CdfShared {
+  float warp_tot[kRowThreads / 32];
+  int found;
+  float run;
+};
+// Inverse CDF inside one row, by the whole CTA: the first j with cumsum(row)[j] > target and row[j] > 0; when target
+// rounded past the last partial sum, the last positive entry.  The result is valid in thread 0.
+__device__ int inverse_cdf_row(const float* row, int items, float target, CdfShared& sh) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    sh.found = items;
+    sh.run = 0.f;
+  }
+  __syncthreads();
+  for (int base = 0; base < items; base += blockDim.x) {
+    const int j = base + threadIdx.x;
+    const float p = j < items ? row[j] : 0.f;
+    float incl = p;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    if (lane == 31) sh.warp_tot[warp] = incl;
+    __syncthreads();
+    float before = sh.run;
+    for (int w = 0; w < warp; ++w) before += sh.warp_tot[w];
+    const float c = before + incl;
+    if (j < items && p > 0.f && c > target) atomicMin(&sh.found, j);
+    __syncthreads();
+    if (sh.found < items) break;
+    if (threadIdx.x == blockDim.x - 1) sh.run = c;
+    __syncthreads();
+  }
+  int a = sh.found;
+  if (threadIdx.x == 0 && a >= items) {
+    a = items - 1;
+    while (a > 0 && !(row[a] > 0.f)) --a;
+  }
+  return a;
+}
+
 // Categorical(probs).sample() and .log_prob(sample)   (models.py:107-110, 127-143).  torch normalises the probabilities
 // by their row sum and clamps them to [eps, 1-eps] before the log (torch/distributions/categorical.py, utils.py).
-// Sampling is by inverse CDF: the first j with cumsum(probs)[j] > u * sum(probs); u from `uniforms` (replayable) or from
-// Philox keyed by (seed, draw, row).  One CTA per row.
+// Sampling is by inverse CDF: the first j with cumsum(probs)[j] > u * sum(probs); u from draw_uniform.  One CTA per row.
 __global__ void __launch_bounds__(kRowThreads)
 categorical_sample_kernel(const float* __restrict__ probs, long long ld, long long n, int items,
                           const float* __restrict__ uniforms, unsigned long long seed, long long draw,
                           long long* __restrict__ action, float* __restrict__ logp) {
   __shared__ float red[32];
-  __shared__ float warp_tot[kRowThreads / 32];
-  __shared__ int found;
-  __shared__ float run;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __shared__ CdfShared sh;
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
     const float* row = probs + r * ld;
     float t = 0.f;
     for (int j = threadIdx.x; j < items; j += blockDim.x) t += row[j];
     const float total = block_sum(t, red);
-    float u;
-    if (uniforms) {
-      u = uniforms[r];
-    } else {
-      Philox ph(seed);
-      const uint4 q = ph((unsigned long long)r, ((unsigned long long)draw << 8) | 0x5au);
-      u = (float)(q.x >> 8) * (1.0f / 16777216.0f);          // [0, 1)
-    }
-    const float target = u * total;
+    const float u = draw_uniform(uniforms, seed, draw, r);
+    const int a = inverse_cdf_row(row, items, u * total, sh);
     if (threadIdx.x == 0) {
-      found = items;
-      run = 0.f;
-    }
-    __syncthreads();
-    for (int base = 0; base < items; base += blockDim.x) {
-      const int j = base + threadIdx.x;
-      const float p = j < items ? row[j] : 0.f;
-      float incl = p;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const float v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += v;
-      }
-      if (lane == 31) warp_tot[warp] = incl;
-      __syncthreads();
-      float before = run;
-      for (int w = 0; w < warp; ++w) before += warp_tot[w];
-      const float c = before + incl;
-      if (j < items && p > 0.f && c > target) atomicMin(&found, j);
-      __syncthreads();
-      if (found < items) break;
-      if (threadIdx.x == blockDim.x - 1) run = c;
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-      int a = found;
-      if (a >= items) {                 // u * total rounded past the last partial sum: the last possible outcome
-        a = items - 1;
-        while (a > 0 && !(row[a] > 0.f)) --a;
-      }
       action[r] = a;
       logp[r] = clamped_log_prob(row[a] / total);
     }
@@ -188,12 +197,13 @@ __global__ void categorical_log_prob_kernel(const float* __restrict__ probs, lon
 // each chunk's logits and turns them into d loss / d logits.  With one chunk this is the plain softmax backward.
 
 // Pass 1: (run_max, run_sum) <- the online max / sum of exp over the logits seen so far (chunk c0 == 0 starts them);
-// za[r] <- z[r, a_r] when the row's action lies in this chunk.  z: the chunk's [n, w] logits with row pitch ld.
+// za[r] <- z[r, a_r - a_off] when that column lies in this chunk (a_off: the first item id of the arena's linear2 rows,
+// 0 unless the vocabulary is sharded; action may be NULL).  z: the chunk's [n, w] logits with row pitch ld.
 // One CTA per row.
 __global__ void __launch_bounds__(kRowThreads)
 logit_stats_kernel(const float* __restrict__ z, long long ld, long long n, int w, int c0,
-                   const long long* __restrict__ action, float* __restrict__ run_max, float* __restrict__ run_sum,
-                   float* __restrict__ za) {
+                   const long long* __restrict__ action, long long a_off, float* __restrict__ run_max,
+                   float* __restrict__ run_sum, float* __restrict__ za) {
   __shared__ float red[32];
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
     const float* row = z + r * ld;
@@ -219,8 +229,10 @@ logit_stats_kernel(const float* __restrict__ z, long long ld, long long n, int w
         run_sum[r] = run_sum[r] * expf(M0 - Mn) + S * expf(M - Mn);
         run_max[r] = Mn;
       }
-      const long long a = action[r];
-      if (a >= c0 && a < (long long)c0 + w) za[r] = row[a - c0];
+      if (action) {
+        const long long a = action[r] - a_off;
+        if (a >= c0 && a < (long long)c0 + w) za[r] = row[a - c0];
+      }
     }
     __syncthreads();
   }
@@ -293,6 +305,170 @@ __global__ void __launch_bounds__(1024) sum_rows_kernel(const float* __restrict_
   for (long long i = threadIdx.x; i < n; i += blockDim.x) t += v[i];
   t = block_sum(t, red);
   if (threadIdx.x == 0) out[0] = t * scale;
+}
+
+// ---- Vocabulary-sharded policy: rank q of W holds the linear2 rows of items [lo_q, hi_q), linear1 is replicated.
+// A rank's record of one forward, exchanged by all-gather: a header of kShardHeader int32 words {lo, hi, num_items,
+// n_rows}, then three planes of n_rows floats -- the local max m_q, the local sum s_q = sum exp(z - m_q) and the logit
+// of the row's action (from its owner; 0 on every other rank).  Every rank merges the W records in rank order, so all
+// of them get the same bits; at W = 1 the merge is exact (M = m_0, S = s_0 exp(0) = s_0), so the sharded path computes
+// what the unsharded one does.
+constexpr int kShardHeader = 4;
+__host__ __device__ __forceinline__ int64_t shard_record_floats(int64_t n) { return kShardHeader + 3 * n; }
+
+// header, and a zero action-logit plane (the owners overwrite their rows in pass 1)
+__global__ void shard_record_init_kernel(float* __restrict__ rec, long long n, int lo, int hi, int items) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) rec[kShardHeader + 2 * n + i] = 0.f;
+  if (i == 0) {
+    int* h = reinterpret_cast<int*>(rec);
+    h[0] = lo; h[1] = hi; h[2] = items; h[3] = (int)n;
+  }
+}
+
+// the rank-order merge of row r: M = max m_q, S = sum s_q exp(m_q - M), za = sum za_q
+__device__ __forceinline__ void shard_merge_row(const float* __restrict__ g, int W, long long n, long long r, float& M,
+                                                float& S, float& za) {
+  const long long stride = shard_record_floats(n);
+  M = -INFINITY;
+  for (int q = 0; q < W; ++q) M = fmaxf(M, g[q * stride + kShardHeader + r]);
+  S = 0.f;
+  za = 0.f;
+  for (int q = 0; q < W; ++q) {
+    const float* rec = g + q * stride + kShardHeader;
+    S += rec[n + r] * expf(rec[r] - M);
+    za += rec[2 * n + r];
+  }
+}
+
+// true unless the W headers tile [0, items) in rank order, every rank saw n rows and this rank's entry is [lo, hi)
+__device__ bool shard_plan_bad(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items) {
+  const long long stride = shard_record_floats(n);
+  int expect = 0;
+  bool bad = false;
+  for (int q = 0; q < W; ++q) {
+    const int* h = reinterpret_cast<const int*>(g + q * stride);
+    bad = bad || h[0] != expect || h[1] <= h[0] || h[2] != items || h[3] != (int)n;
+    expect = h[1];
+    if (q == rank) bad = bad || h[0] != lo || h[1] != hi;
+  }
+  return bad || expect != items;
+}
+
+// gathered records -> the merged statistics of every row (into the scratch the unsharded path uses); *plan_bad
+__global__ void shard_merge_kernel(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items,
+                                   float* __restrict__ run_max, float* __restrict__ run_sum, float* __restrict__ za,
+                                   int* plan_bad) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0 && shard_plan_bad(g, W, n, rank, lo, hi, items)) *plan_bad = 1;
+  if (r >= n) return;
+  float M, S, z;
+  shard_merge_row(g, W, n, r, M, S, z);
+  run_max[r] = M;
+  run_sum[r] = S;
+  za[r] = z;
+}
+
+// the rank's logits block [n, w] -> its block of the softmax, exp(z - M) / S (the last loop of softmax_rows_kernel)
+__global__ void __launch_bounds__(kRowThreads)
+shard_softmax_finish_kernel(float* __restrict__ z, long long n, int w, const float* __restrict__ g, int W, int rank,
+                            int lo, int items, int* plan_bad) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, W, n, rank, lo, lo + w, items)) *plan_bad = 1;
+  for (long long r = blockIdx.x; r < n; r += gridDim.x) {
+    float M, S, za;
+    shard_merge_row(g, W, n, r, M, S, za);
+    float* row = z + r * w;
+    for (int j = threadIdx.x; j < w; j += blockDim.x) row[j] = expf(row[j] - M) / S;
+  }
+}
+
+// A draw's record: two planes of n -- the global item id (int32 bits; -1 on every rank but the owner) and its log-prob.
+
+// One draw per row over the whole vocabulary from the rank's block of the softmax.  Every rank finds the owner of u
+// from the shard masses P_q = s_q exp(m_q - M) / S (the first rank whose cumulative mass exceeds u); the owner draws
+// inside its block at u' = (u - C_{owner-1}) / P_owner with the inverse CDF of categorical_sample_kernel.  At W = 1,
+// P_0 = 1 and u' = u exactly.  One CTA per row.
+__global__ void __launch_bounds__(kRowThreads)
+shard_sample_kernel(const float* __restrict__ probs, long long n, int w, const float* __restrict__ g, int W, int rank,
+                    int lo, const float* __restrict__ uniforms, unsigned long long seed, long long draw,
+                    float* __restrict__ draw_rec) {
+  __shared__ float red[32];
+  __shared__ CdfShared sh;
+  const long long stride = shard_record_floats(n);
+  for (long long r = blockIdx.x; r < n; r += gridDim.x) {
+    float M, S, za;
+    shard_merge_row(g, W, n, r, M, S, za);
+    const float u = draw_uniform(uniforms, seed, draw, r);
+    int owner = -1, last = -1;
+    float C = 0.f, before = 0.f, P = 0.f, last_before = 0.f, last_P = 0.f;
+    for (int q = 0; q < W; ++q) {
+      const float* rec = g + q * stride + kShardHeader;
+      const float Pq = rec[n + r] * expf(rec[r] - M) / S;
+      if (Pq > 0.f) {
+        if (owner < 0 && C + Pq > u) {
+          owner = q; before = C; P = Pq;
+        }
+        last = q; last_before = C; last_P = Pq;
+      }
+      C += Pq;
+    }
+    if (owner < 0) {                   // u rounded past the last cumulative mass: the last rank with mass
+      owner = last; before = last_before; P = last_P;
+    }
+    if (owner != rank) {               // the same decision in every thread
+      if (threadIdx.x == 0) {
+        draw_rec[r] = __int_as_float(-1);
+        draw_rec[n + r] = 0.f;
+      }
+      continue;
+    }
+    const float* row = probs + r * w;
+    float t = 0.f;
+    for (int j = threadIdx.x; j < w; j += blockDim.x) t += row[j];
+    const float total = block_sum(t, red);
+    const float u2 = fminf((u - before) / P, 0x1.fffffep-1f);
+    const int a = inverse_cdf_row(row, w, u2 * total, sh);
+    if (threadIdx.x == 0) {
+      draw_rec[r] = __int_as_float(lo + a);
+      draw_rec[n + r] = clamped_log_prob(row[a] / total * P);
+    }
+    __syncthreads();
+  }
+}
+
+// the log-prob of given global ids, from their owner's block of the softmax; *oob when an id is outside [0, items)
+__global__ void shard_log_prob_kernel(const float* __restrict__ probs, long long n, int w, int lo, int items,
+                                      const long long* __restrict__ action, float* __restrict__ draw_rec, int* oob) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const long long a = action[r];
+  if (a < 0 || a >= items) *oob = 1;
+  const bool mine = a >= lo && a < (long long)lo + w;
+  draw_rec[r] = __int_as_float(mine ? (int)a : -1);
+  draw_rec[n + r] = mine ? clamped_log_prob(probs[r * w + (a - lo)]) : 0.f;
+}
+
+// gathered draw records [W][2][n] -> (id, log-prob) of every row; *disagree unless exactly one rank claimed the row
+__global__ void shard_pick_kernel(const float* __restrict__ g, int W, long long n, long long* __restrict__ action,
+                                  float* __restrict__ logp, int* disagree) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  int claims = 0, id = -1;
+  float lp = 0.f;
+  for (int q = 0; q < W; ++q) {
+    const float* d = g + (long long)q * 2 * n;
+    const int v = __float_as_int(d[r]);
+    if (v >= 0) {
+      if (claims == 0) {
+        id = v;
+        lp = d[n + r];
+      }
+      ++claims;
+    }
+  }
+  if (claims != 1) *disagree = 1;
+  action[r] = id;
+  logp[r] = lp;
 }
 
 static int row_grid(int64_t n) { return (int)(n < (int64_t)kNumSMs * 8 ? n : (int64_t)kNumSMs * 8); }
@@ -397,6 +573,45 @@ static int discrete_logits(const recnn_discrete_dims& d, const float* params, in
   return linear_out(sh, params + l.w2 + (int64_t)c0 * l.ld2, l.ld2, params + l.b2 + c0, w, n, 0, nullptr, z, w, st);
 }
 
+// Pass 1 of the policy gradient over the arena's items in chunks of `chunk`: per-row max / sum of exp of every logit,
+// and the logit of item a_r (a_off: the item id of the arena's first linear2 row).  The last chunk's logits stay in s.z.
+static int reinforce_stats_pass(const recnn_discrete_dims& d, const float* params, int64_t n, const DiscreteScratch& s,
+                                int chunk, const long long* act, long long a_off, float* run_max, float* run_sum,
+                                float* za, cudaStream_t st) {
+  const int I = d.num_items;
+  for (int c0 = 0; c0 < I; c0 += chunk) {
+    const int w = I - c0 < chunk ? I - c0 : chunk;
+    RECNN_PROPAGATE(discrete_logits(d, params, n, s, c0, w, s.z, st));
+    logit_stats_kernel<<<row_grid(n), kRowThreads, 0, st>>>(s.z, w, n, w, c0, act, a_off, run_max, run_sum, za);
+    RECNN_CHECK_LAUNCH("logit_stats_kernel");
+  }
+  return RECNN_OK;
+}
+
+// Pass 2, last chunk first (its logits are still in s.z): dz = d loss / d logits of the chunk from s.run_max, s.run_sum
+// and s.g; dW2[c0:c0+w] = dz^T h, db2[c0:c0+w] = colsum dz; dh (+)= dz W2[c0:c0+w], gated by [h > 0] after the last
+// term; then dW1 = dh^T s, db1 = colsum dh.
+static int reinforce_grad_pass(const recnn_discrete_dims& d, const float* params, float* grads, int64_t n,
+                               const DiscreteScratch& s, int chunk, const long long* act, long long a_off, const Seg& xs,
+                               cudaStream_t st) {
+  const DiscreteLayout l = discrete_layout(d);
+  const int H = d.hidden, I = d.num_items;
+  const int n_chunks = (int)ceil_div(I, chunk);
+  const Seg sh = {s.h, H, H, 0};
+  for (int c = n_chunks - 1; c >= 0; --c) {
+    const int c0 = c * chunk, w = I - c0 < chunk ? I - c0 : chunk;
+    if (c != n_chunks - 1) RECNN_PROPAGATE(discrete_logits(d, params, n, s, c0, w, s.z, st));
+    reinforce_dlogits_kernel<<<row_grid(n), kRowThreads, 0, st>>>(s.z, n, w, (int)(a_off + c0), act, s.run_max,
+                                                                    s.run_sum, s.g);
+    RECNN_CHECK_LAUNCH("reinforce_dlogits_kernel");
+    const int64_t w2 = l.w2 + (int64_t)c0 * l.ld2;
+    RECNN_PROPAGATE(weight_grad(s.z, w, sh, kNoSeg, n, grads + w2, l.ld2, grads + l.b2 + c0, s.partial, st));
+    RECNN_PROPAGATE(backprop_hidden(s.z, w, params + w2, l.ld2, H, 0, H, n, c == 0 ? s.h : nullptr, 1.f, s.dh, st,
+                                    c != n_chunks - 1));
+  }
+  return weight_grad(s.dh, H, xs, kNoSeg, n, grads + l.w1, l.ld1, grads + l.b1, s.partial, st);
+}
+
 }  // namespace recnn
 
 using namespace recnn;
@@ -473,42 +688,19 @@ extern "C" int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d,
   RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
   RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const DiscreteLayout l = discrete_layout(*d);
-  const int H = d->hidden, I = d->num_items, W = chunk_items;
-  const int n_chunks = (int)ceil_div(I, W);
   const long long* act = reinterpret_cast<const long long*>(action);
-  const DiscreteScratch s = discrete_carve(*d, n_rows, W, align_floats(scratch));
+  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, align_floats(scratch));
   RECNN_CHECK_CUDA(cudaMemsetAsync(s.flags, 0, 4 * sizeof(int), st));
   Seg xs;
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, &xs));
-  // pass 1: per-row max / sum of exp over all logits, and the drawn action's logit
-  for (int c = 0; c < n_chunks; ++c) {
-    const int c0 = c * W, w = I - c0 < W ? I - c0 : W;
-    RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, c0, w, s.z, st));
-    logit_stats_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(s.z, w, n_rows, w, c0, act, s.run_max, s.run_sum,
-                                                                  s.za);
-    RECNN_CHECK_LAUNCH("logit_stats_kernel");
-  }
+  RECNN_PROPAGATE(reinforce_stats_pass(*d, params, n_rows, s, chunk_items, act, 0, s.run_max, s.run_sum, s.za, st));
   reinforce_row_weights_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
-      n_rows, I, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss, s.flags);
+      n_rows, d->num_items, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss,
+      s.flags);
   RECNN_CHECK_LAUNCH("reinforce_row_weights_kernel");
   sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n_rows, 1.f, out);
   RECNN_CHECK_LAUNCH("sum_rows_kernel");
-  // pass 2, last chunk first (its logits are still in the buffer): dz = d loss / d logits of the chunk;
-  // dW2[c0:c0+w] = dz^T h, db2[c0:c0+w] = colsum dz; dh (+)= dz W2[c0:c0+w], gated by [h > 0] after the last term
-  const Seg sh = {s.h, H, H, 0};
-  for (int c = n_chunks - 1; c >= 0; --c) {
-    const int c0 = c * W, w = I - c0 < W ? I - c0 : W;
-    if (c != n_chunks - 1) RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, c0, w, s.z, st));
-    reinforce_dlogits_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(s.z, n_rows, w, c0, act, s.run_max, s.run_sum, s.g);
-    RECNN_CHECK_LAUNCH("reinforce_dlogits_kernel");
-    const int64_t w2 = l.w2 + (int64_t)c0 * l.ld2;
-    RECNN_PROPAGATE(weight_grad(s.z, w, sh, kNoSeg, n_rows, grads + w2, l.ld2, grads + l.b2 + c0, s.partial, st));
-    RECNN_PROPAGATE(backprop_hidden(s.z, w, params + w2, l.ld2, H, 0, H, n_rows, c == 0 ? s.h : nullptr, 1.f, s.dh, st,
-                                    c != n_chunks - 1));
-  }
-  // dW1 = dh^T s, db1 = colsum dh
-  RECNN_PROPAGATE(weight_grad(s.dh, H, xs, kNoSeg, n_rows, grads + l.w1, l.ld1, grads + l.b1, s.partial, st));
+  RECNN_PROPAGATE(reinforce_grad_pass(*d, params, grads, n_rows, s, chunk_items, act, 0, xs, st));
   RECNN_CHECK_CUDA(cudaMemcpyAsync(out + 1, s.flags, sizeof(int), cudaMemcpyDeviceToDevice, st));
   return RECNN_OK;
 }
@@ -520,4 +712,140 @@ extern "C" int recnn_reinforce_policy_grad(const recnn_discrete_dims* d, const f
   RECNN_REQUIRE(discrete_dims_ok(d), "null pointer / dims");
   return recnn_reinforce_policy_grad_chunked(d, params, grads, state, action, beta_log_prob, returns, n_rows, method,
                                              top_k, d->num_items, out, scratch, stream);
+}
+
+// ---- the vocabulary-sharded policy: the phases around the two all-gathers (see the header) ----------------------
+static bool shard_ok(const recnn_discrete_dims* d, const recnn_vocab_shard* v) {
+  return v && v->world >= 1 && v->rank >= 0 && v->rank < v->world && v->item_offset >= 0 &&
+         (int64_t)v->item_offset + d->num_items <= (int64_t)v->num_items;
+}
+
+extern "C" int64_t recnn_vocab_record_floats(int64_t n_rows) { return n_rows > 0 ? shard_record_floats(n_rows) : 0; }
+
+static int shard_record_init(const recnn_discrete_dims& d, const recnn_vocab_shard& v, float* record, int64_t n,
+                             cudaStream_t st) {
+  shard_record_init_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(record, n, v.item_offset,
+                                                                      v.item_offset + d.num_items, v.num_items);
+  RECNN_CHECK_LAUNCH("shard_record_init_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_reinforce_shard_stats(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                           const float* state, const int64_t* action, int64_t n_rows,
+                                           int32_t chunk_items, float* record, float* scratch, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && state && action && record && scratch, "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
+  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, align_floats(scratch));
+  RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
+  RECNN_PROPAGATE(shard_record_init(*d, *v, record, n_rows, st));
+  float* m = record + kShardHeader;
+  return reinforce_stats_pass(*d, params, n_rows, s, chunk_items, reinterpret_cast<const long long*>(action),
+                              v->item_offset, m, m + n_rows, m + 2 * n_rows, st);
+}
+
+extern "C" int recnn_reinforce_shard_grad(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                          float* grads, const float* state, const int64_t* action,
+                                          const float* beta_log_prob, const float* returns, int64_t n_rows,
+                                          int32_t method, int32_t top_k, int32_t chunk_items, const float* gathered,
+                                          float* out, float* scratch, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && grads && state && action && returns && gathered && out && scratch,
+                "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || method == RECNN_REINFORCE_CORRECTED || method == RECNN_REINFORCE_TOPK,
+                "unknown REINFORCE method");
+  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || beta_log_prob, "the corrected losses need the behaviour policy's log-probs");
+  RECNN_REQUIRE(method != RECNN_REINFORCE_TOPK || top_k >= 1, "K >= 1");
+  RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
+  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* act = reinterpret_cast<const long long*>(action);
+  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, align_floats(scratch));
+  RECNN_CHECK_CUDA(cudaMemsetAsync(s.flags, 0, 4 * sizeof(int), st));
+  // the stats phase left the state image (when one was needed) in s.img
+  const int S = d->state_dim;
+  const bool direct = S % 4 == 0 && aligned16(state);
+  const Seg xs = direct ? Seg{state, S, S, 0} : Seg{s.img, S, pad4(S), 0};
+  shard_merge_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
+      gathered, v->world, n_rows, v->rank, v->item_offset, v->item_offset + d->num_items, v->num_items, s.run_max,
+      s.run_sum, s.za, s.flags + 1);
+  RECNN_CHECK_LAUNCH("shard_merge_kernel");
+  reinforce_row_weights_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
+      n_rows, v->num_items, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss,
+      s.flags);
+  RECNN_CHECK_LAUNCH("reinforce_row_weights_kernel");
+  sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n_rows, 1.f, out);
+  RECNN_CHECK_LAUNCH("sum_rows_kernel");
+  RECNN_PROPAGATE(reinforce_grad_pass(*d, params, grads, n_rows, s, chunk_items, act, v->item_offset, xs, st));
+  RECNN_CHECK_CUDA(cudaMemcpyAsync(out + 1, s.flags, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_forward(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                            const float* params, const float* state, int64_t n_rows, float* probs_out,
+                                            float* record, float* scratch, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && state && probs_out && record && scratch, "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int I = d->num_items;
+  const DiscreteScratch s = discrete_carve(*d, n_rows, 0, align_floats(scratch));
+  RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
+  RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, 0, I, probs_out, st));
+  RECNN_PROPAGATE(shard_record_init(*d, *v, record, n_rows, st));
+  float* m = record + kShardHeader;
+  logit_stats_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(probs_out, I, n_rows, I, 0, nullptr, 0, m, m + n_rows,
+                                                                nullptr);
+  RECNN_CHECK_LAUNCH("logit_stats_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                           const float* gathered, int64_t n_rows, float* probs, int32_t* error_flag,
+                                           void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && gathered && probs && error_flag, "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  if (n_rows <= 0) return RECNN_OK;
+  shard_softmax_finish_kernel<<<row_grid(n_rows), kRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      probs, n_rows, d->num_items, gathered, v->world, v->rank, v->item_offset, v->num_items, error_flag);
+  RECNN_CHECK_LAUNCH("shard_softmax_finish_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_sample(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                           const float* gathered, const float* probs, int64_t n_rows,
+                                           const float* uniforms, uint64_t seed, int64_t draw, float* draw_record,
+                                           void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && gathered && probs && draw_record, "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  if (n_rows <= 0) return RECNN_OK;
+  shard_sample_kernel<<<row_grid(n_rows), kRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      probs, n_rows, d->num_items, gathered, v->world, v->rank, v->item_offset, uniforms, seed, draw, draw_record);
+  RECNN_CHECK_LAUNCH("shard_sample_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_log_prob(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                             const float* probs, int64_t n_rows, const int64_t* action,
+                                             float* draw_record, int32_t* oob_flag, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && probs && action && draw_record && oob_flag, "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  if (n_rows <= 0) return RECNN_OK;
+  shard_log_prob_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      probs, n_rows, d->num_items, v->item_offset, v->num_items, reinterpret_cast<const long long*>(action),
+      draw_record, oob_flag);
+  RECNN_CHECK_LAUNCH("shard_log_prob_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_pick(int32_t world, const float* gathered_draws, int64_t n_rows,
+                                         int64_t* action_out, float* log_prob_out, int32_t* error_flag, void* stream) {
+  RECNN_REQUIRE(world >= 1 && gathered_draws && action_out && log_prob_out && error_flag, "null pointer / world");
+  if (n_rows <= 0) return RECNN_OK;
+  shard_pick_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      gathered_draws, world, n_rows, reinterpret_cast<long long*>(action_out), log_prob_out, error_flag);
+  RECNN_CHECK_LAUNCH("shard_pick_kernel");
+  return RECNN_OK;
 }

@@ -31,6 +31,7 @@ class PeerComm:
         L = _lib.lib()
         self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
         self.device = torch.device(device)
+        self.capacity = -(-int(capacity_floats) // 4) * 4         # the library rounds the staging capacity up to 4
         self.handle = ctypes.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(L.recnn_comm_create(self.rank, self.world, int(capacity_floats), ctypes.byref(self.handle)))
@@ -59,6 +60,14 @@ class PeerComm:
         _lib.check(_lib.lib().recnn_comm_allreduce(self.handle, t.data_ptr(), t.numel(),
                                                    torch.cuda.current_stream(t.device).cuda_stream))
         return t
+
+    def all_gather(self, t: torch.Tensor) -> torch.Tensor:
+        """[world * n]: every rank's n words of ``t`` in rank order, the same bits on every rank (fp32 or int32)."""
+        assert t.is_cuda and t.dtype in (torch.float32, torch.int32) and t.is_contiguous()
+        out = torch.empty(self.world * t.numel(), dtype=t.dtype, device=t.device)
+        _lib.check(_lib.lib().recnn_comm_allgather(self.handle, t.data_ptr(), t.numel(), out.data_ptr(),
+                                                   torch.cuda.current_stream(t.device).cuda_stream))
+        return out
 
     def close(self):
         if self.handle is not None:
@@ -102,3 +111,113 @@ def enable_data_parallel(agent_or_nets, group=None, sync_weights=True):
         eng.graphs.clear()
         eng._fast.clear()
     return agent_or_nets
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Vocabulary parallelism of the REINFORCE policy (DiscreteActor): rank r holds rows [lo_r, hi_r) of linear2 and their
+# optimizer state; linear1 is replicated.  Every rank is fed the same saved rows.  A policy update exchanges a few
+# floats per row and rank (all-gather) and the layer-1 gradient (all-reduce); see recnn_reinforce_shard_* in
+# include/recnn_b200.h.
+def vocab_shard(num_items: int, rank: int, world: int):
+    """Contiguous item range [lo, hi) of ``rank``: blocks of ceil(num_items / world) items, the last one shorter.
+    Raises ValueError when the rank's block would be empty."""
+    per = -(-num_items // world)
+    lo, hi = min(rank * per, num_items), min((rank + 1) * per, num_items)
+    if hi <= lo:
+        raise ValueError("%d items over %d ranks leave rank %d without items; use fewer ranks" % (num_items, world, rank))
+    return lo, hi
+
+
+def check_vocab_plans(plans):
+    """``plans``: every rank's (lo, hi, num_items) in rank order.  Raises ValueError unless they tile [0, num_items)
+    with non-empty, contiguous blocks and agree on num_items."""
+    items = {p[2] for p in plans}
+    if len(items) != 1:
+        raise ValueError("the ranks disagree on the vocabulary size: %s" % sorted(items))
+    expect = 0
+    for r, (lo, hi, _) in enumerate(plans):
+        if lo != expect or hi <= lo:
+            raise ValueError("rank %d holds items [%d, %d), expected a non-empty block from %d" % (r, lo, hi, expect))
+        expect = hi
+    if expect != items.pop():
+        raise ValueError("the shards end at item %d, not at the vocabulary size" % expect)
+
+
+def layer1_floats(dims) -> int:
+    """Floats of the layer-1 block (linear1 weight and bias) at the head of a DiscreteActor arena."""
+    buf = (ctypes.c_int64 * 7)()
+    _lib.check(_lib.lib().recnn_discrete_layout(dims, buf))
+    return int(buf[2])
+
+
+def vocab_comm_floats(dims, world: int, rows: int) -> int:
+    """Staging capacity a sharded policy's communicator needs for ``rows`` saved rows: the layer-1 all-reduce, or the
+    all-gather of ``world`` records of ``rows`` rows, whichever is larger."""
+    return max(layer1_floats(dims), world * int(_lib.lib().recnn_vocab_record_floats(rows)))
+
+
+class VocabParallel:
+    """What ``enable_vocab_parallel`` records on a policy: its block [lo, hi) of the ``num_items`` items, the process
+    group, rank, world size, and the peer communicator of the exchanges."""
+
+    def __init__(self, lo, hi, num_items, group, rank, world, comm):
+        self.lo, self.hi, self.num_items = lo, hi, num_items
+        self.group, self.rank, self.world, self.comm = group, rank, world, comm
+
+    def shard(self):
+        return _lib.VocabShard(self.lo, self.num_items, self.rank, self.world)
+
+    def all_gather(self, t: torch.Tensor) -> torch.Tensor:
+        """PeerComm.all_gather; the communicator grows (collectively: every rank gathers the same size) when the
+        records outgrow it."""
+        need = self.world * t.numel()
+        if need > self.comm.capacity:
+            grown = PeerComm(self.group, t.device, max(need, 2 * self.comm.capacity))
+            self.comm.close()
+            self.comm = grown
+        return self.comm.all_gather(t)
+
+
+def enable_vocab_parallel(policy, group=None):
+    """Shard a DiscreteActor's item layer over the ranks of ``group``.  Call it on every rank after the policy is on
+    its CUDA device and before its optimizer is built.  The weights are first made identical to rank 0's; then rank r
+    keeps rows vocab_shard(num_items, r, world) of linear2 (so ``state_dict`` holds the local block).  At world 1 the
+    policy computes exactly what it did unsharded.
+
+    On a sharded policy, ``forward`` / ``select_action`` return the rank's COLUMN BLOCK [N, hi - lo] of the softmax
+    over all items (the reference returns [N, num_items]); sampled ids, log-probs, ``saved_log_probs``, ``correction``
+    and ``lambda_k`` are global and identical on every rank.  Every rank must be fed the same states, seeded the same
+    (torch.manual_seed, or the same ``uniform_source``) and must make the same calls in the same order.
+    ``ChooseREINFORCE`` trains it; ``reinforce_update`` / ``Reinforce`` refuse it (their critic consumes dense
+    probabilities)."""
+    from .nn.arena import _is_discrete, _is_beta, grad_arena
+    if not dist.is_initialized():
+        raise RuntimeError("torch.distributed is not initialised")
+    if _is_beta(policy) or not _is_discrete(policy):
+        raise TypeError("enable_vocab_parallel shards a DiscreteActor")
+    if "_recnn_vp" in policy.__dict__:
+        raise RuntimeError("the policy is already vocabulary-parallel")
+    arena = param_arena(policy)
+    if not arena.is_cuda:
+        raise _lib.RecnnError("enable_vocab_parallel needs the policy on its CUDA device")
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    # every rank checks every rank's plan, so a refused plan raises on all of them (none is left in a collective)
+    sizes = [None] * world
+    dist.all_gather_object(sizes, (policy.linear1.in_features, policy.linear1.out_features,
+                                   policy.linear2.out_features), group=group)
+    if len(set(sizes)) != 1:
+        raise ValueError("the ranks' policies differ in shape: %s" % sizes)
+    num_items = sizes[0][2]
+    plans = [vocab_shard(num_items, r, world) + (num_items,) for r in range(world)]
+    check_vocab_plans(plans)
+    lo, hi, _ = plans[rank]
+    broadcast_nets({"policy_net": policy}, group)
+    with torch.no_grad():
+        for p in (policy.linear2.weight, policy.linear2.bias):
+            p.grad = None
+            p.data = p.data[lo:hi].clone()
+    policy.linear2.out_features = hi - lo
+    grad_arena(policy)                                  # the local arenas (param_arena rebuilds on the new shapes)
+    comm = PeerComm(group, arena.device, vocab_comm_floats(policy.dims, world, 1))
+    policy.__dict__["_recnn_vp"] = VocabParallel(lo, hi, num_items, group, rank, world, comm)
+    return policy

@@ -114,6 +114,8 @@ class DiscreteActor(nn.Module):
       change between two policy updates.  ``gc()`` drops both.
     * Categorical draws are inverse-CDF draws on a counter-based Philox stream keyed by ``torch.initial_seed()`` (or on
       ``uniform_source(n_rows) -> tensor[n_rows]`` when set: replayable draws for tests), not torch's global generator.
+    * After ``recnn_b200.dist.enable_vocab_parallel`` each rank holds a block of linear2's rows, and ``forward`` /
+      ``select_action`` return the rank's column block of the probabilities; draws and log-probs stay global.
     """
 
     def __init__(self, input_dim, action_dim, hidden_size, init_w=0):
@@ -136,19 +138,38 @@ class DiscreteActor(nn.Module):
         return discrete_dims(self)
 
     def forward(self, inputs):
+        """probabilities [N, num_items]; on a vocabulary-parallel policy (recnn_b200.dist.enable_vocab_parallel) the
+        rank's column block [N, hi - lo] of them."""
+        return self._pi(inputs)[0]
+
+    def _pi(self, inputs):
+        """(probs, gathered records): the records of the rank-order all-gather when the policy is sharded, else None."""
         dev, (state,) = _device_check(self, inputs)
         n = state.shape[0]
         d = self.dims
         flat = param_arena(self)
         out = torch.empty(n, d.num_items, device=dev, dtype=torch.float32)
         if n == 0:
-            return out
+            return out, None
         L = _lib.lib()
+        vp = self.__dict__.get("_recnn_vp")
         scratch = torch.empty(L.recnn_discrete_scratch_floats(d, n, 0), device=dev, dtype=torch.float32)
         with torch.cuda.device(dev):
-            _lib.check(L.recnn_discrete_forward(d, flat.data_ptr(), state.data_ptr(), n, out.data_ptr(),
-                                                scratch.data_ptr(), _lib.stream_ptr(dev)))
-        return out
+            if vp is None:
+                _lib.check(L.recnn_discrete_forward(d, flat.data_ptr(), state.data_ptr(), n, out.data_ptr(),
+                                                    scratch.data_ptr(), _lib.stream_ptr(dev)))
+                return out, None
+            shard = vp.shard()
+            rec = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+            _lib.check(L.recnn_discrete_shard_forward(d, shard, flat.data_ptr(), state.data_ptr(), n, out.data_ptr(),
+                                                      rec.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
+            gathered = vp.all_gather(rec)
+            flag = torch.zeros(1, dtype=torch.int32, device=dev)
+            _lib.check(L.recnn_discrete_shard_finish(d, shard, gathered.data_ptr(), n, out.data_ptr(), flag.data_ptr(),
+                                                     _lib.stream_ptr(dev)))
+        if int(flag.item()) != 0:
+            raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+        return out, gathered
 
     def gc(self):
         del self.rewards[:]
@@ -158,8 +179,9 @@ class DiscreteActor(nn.Module):
         del self._saved[:]
 
     # -- Categorical(probs).sample() / .log_prob() on the device ----------------------------------------------------
-    def _sample(self, probs):
-        """(action int64 [N], log_prob fp32 [N]) of one draw per row."""
+    def _sample(self, probs, gathered=None):
+        """(action int64 [N], log_prob fp32 [N]) of one draw per row.  ``gathered``: the records of the sharded
+        forward that made ``probs`` (the rank's column block); the draw is then over the whole vocabulary."""
         n, items = probs.shape
         dev = probs.device
         action = torch.empty(n, dtype=torch.int64, device=dev)
@@ -170,11 +192,49 @@ class DiscreteActor(nn.Module):
             if u.shape != (n,):
                 raise ValueError("uniform_source must return %d values" % n)
         self._draws += 1
+        seed = int(torch.initial_seed()) & (2 ** 64 - 1)
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().recnn_categorical_sample(
-                probs.data_ptr(), n, items, probs.stride(0), _lib.ptr(u), int(torch.initial_seed()) & (2 ** 64 - 1),
-                self._draws, action.data_ptr(), logp.data_ptr(), _lib.stream_ptr(dev)))
+            if gathered is None:
+                _lib.check(_lib.lib().recnn_categorical_sample(
+                    probs.data_ptr(), n, items, probs.stride(0), _lib.ptr(u), seed, self._draws, action.data_ptr(),
+                    logp.data_ptr(), _lib.stream_ptr(dev)))
+                return action, logp
+            draw = torch.empty(2 * n, dtype=torch.float32, device=dev)
+            _lib.check(_lib.lib().recnn_discrete_shard_sample(
+                self.dims, self._recnn_vp.shard(), gathered.data_ptr(), probs.data_ptr(), n, _lib.ptr(u), seed,
+                self._draws, draw.data_ptr(), _lib.stream_ptr(dev)))
+        self._shard_pick(draw, n, action, logp, None)
         return action, logp
+
+    def _shard_pick(self, draw, n, action, logp, oob):
+        """The owners' (id, log-prob) of every row from the ranks' draw records (the second all-gather)."""
+        dev = draw.device
+        gathered = self._recnn_vp.all_gather(draw)
+        flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().recnn_discrete_shard_pick(self._recnn_vp.world, gathered.data_ptr(), n,
+                                                            action.data_ptr(), logp.data_ptr(), flag.data_ptr(),
+                                                            _lib.stream_ptr(dev)))
+        if oob is not None and int(oob.item()) != 0:
+            raise IndexError("action index out of range for the policy's output layer")
+        if int(flag.item()) != 0:
+            raise RuntimeError("the ranks of a vocabulary-parallel policy drew different uniforms: seed every rank "
+                               "the same (torch.manual_seed) or give each the same uniform_source")
+
+    def _shard_log_prob(self, probs, action):
+        """_log_prob of global ids on a sharded policy: from the owner's column block, through the second exchange."""
+        n = probs.shape[0]
+        dev = probs.device
+        action = action.to(device=dev, dtype=torch.int64).contiguous()
+        draw = torch.empty(2 * n, dtype=torch.float32, device=dev)
+        oob = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().recnn_discrete_shard_log_prob(self.dims, self._recnn_vp.shard(), probs.data_ptr(), n,
+                                                                action.data_ptr(), draw.data_ptr(), oob.data_ptr(),
+                                                                _lib.stream_ptr(dev)))
+        logp = torch.empty(n, dtype=torch.float32, device=dev)
+        self._shard_pick(draw, n, torch.empty(n, dtype=torch.int64, device=dev), logp, oob)
+        return logp
 
     @staticmethod
     def _log_prob(probs, action):
@@ -199,8 +259,8 @@ class DiscreteActor(nn.Module):
     def _select_action(self, state, **kwargs):
         # REINFORCE without correction: only pi is available, the action source is ignored (models.py:102-111)
         dev, (state,) = _device_check(self, state)
-        pi_probs = self.forward(state)
-        pi_action, pi_log_prob = self._sample(pi_probs)
+        pi_probs, gathered = self._pi(state)
+        pi_action, pi_log_prob = self._sample(pi_probs, gathered)
         self.saved_log_probs.append(pi_log_prob)
         self._saved.append({"state": state.clone(), "action": pi_action, "beta_log_prob": None})
         return pi_probs
@@ -209,14 +269,19 @@ class DiscreteActor(nn.Module):
         """models.py:113-145.  ``beta`` is any callable (state, action=...) -> probabilities [N, action_dim]."""
         dev, (state,) = _device_check(self, state)
         beta_probs = self._as_probs(beta(state.detach(), action=action), dev)
-        pi_probs = self.forward(state)
+        pi_probs, gathered = self._pi(state)
         # the pi draw is made first, then the beta draw (models.py:133-136)
-        pi_draw = self._sample(pi_probs)
+        pi_draw = self._sample(pi_probs, gathered)
         beta_draw = self._sample(beta_probs)
         available = {"pi": (pi_draw, pi_probs), "beta": (beta_draw, beta_probs)}
         (pi_action, pi_lp), src_pi = available[self.action_source["pi"]]
         (beta_action, beta_lp), src_beta = available[self.action_source["beta"]]
-        pi_log_prob = pi_lp if src_pi is pi_probs else self._log_prob(pi_probs, pi_action)
+        if src_pi is pi_probs:
+            pi_log_prob = pi_lp
+        elif gathered is None:
+            pi_log_prob = self._log_prob(pi_probs, pi_action)
+        else:
+            pi_log_prob = self._shard_log_prob(pi_probs, pi_action)
         beta_log_prob = beta_lp if src_beta is beta_probs else self._log_prob(beta_probs, beta_action)
         self._last_sample = {"state": state, "action": pi_action, "beta_log_prob": beta_log_prob}
         return pi_log_prob, beta_log_prob, pi_probs

@@ -63,16 +63,35 @@ def _policy_loss(policy, returns, method):
     L = _lib.lib()
     chunk = _chunk_items(n, d.num_items)
     scratch = torch.empty(L.recnn_reinforce_scratch_floats(d, n, chunk), device=dev, dtype=torch.float32)
-    out = torch.zeros(2, device=dev, dtype=torch.float32)
+    out = torch.zeros(3, device=dev, dtype=torch.float32)
     ks = {r.get("K") for r in saved if r.get("K") is not None}
     if len(ks) > 1:
         raise ValueError("select_action was called with different K since the last policy update: %s" % sorted(ks))
     K = ks.pop() if ks else 1
+    vp = policy.__dict__.get("_recnn_vp")
     with torch.cuda.device(dev):
-        _lib.check(L.recnn_reinforce_policy_grad_chunked(
-            d, flat.data_ptr(), grads.data_ptr(), state.data_ptr(), action.data_ptr(), _lib.ptr(beta_lp),
-            ret_rows.data_ptr(), n, method, K, chunk, out.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
-    if int(out.view(torch.int32)[1].item()) != 0:
+        if vp is None:
+            _lib.check(L.recnn_reinforce_policy_grad_chunked(
+                d, flat.data_ptr(), grads.data_ptr(), state.data_ptr(), action.data_ptr(), _lib.ptr(beta_lp),
+                ret_rows.data_ptr(), n, method, K, chunk, out.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
+        else:
+            # vocabulary-parallel: row statistics of the local items, all-gather, local dW2 / db2 and this rank's
+            # share of the layer-1 gradient, all-reduce of the layer-1 block
+            shard = vp.shard()
+            rec = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+            _lib.check(L.recnn_reinforce_shard_stats(d, shard, flat.data_ptr(), state.data_ptr(), action.data_ptr(), n,
+                                                     chunk, rec.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
+            gathered = vp.all_gather(rec)
+            _lib.check(L.recnn_reinforce_shard_grad(
+                d, shard, flat.data_ptr(), grads.data_ptr(), state.data_ptr(), action.data_ptr(), _lib.ptr(beta_lp),
+                ret_rows.data_ptr(), n, method, K, chunk, gathered.data_ptr(), out.data_ptr(), scratch.data_ptr(),
+                _lib.stream_ptr(dev)))
+            from ...dist import layer1_floats
+            vp.comm.all_reduce(grads[:layer1_floats(d)])
+    flags = out.view(torch.int32)[1:].tolist()
+    if flags[1] != 0:
+        raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the saved rows")
+    if flags[0] != 0:
         raise IndexError("saved action index out of range for the policy's output layer")
     return out[0].clone()
 
@@ -136,6 +155,9 @@ def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"),
     # Due to its mechanics, reinforce doesn't support testing (reinforce.py:80-81)
     learn = True
     policy = nets["policy_net"]
+    if "_recnn_vp" in policy.__dict__:
+        raise RuntimeError("reinforce_update feeds the policy's dense [N, num_items] probabilities to its critic; a "
+                           "vocabulary-parallel policy (enable_vocab_parallel) trains through ChooseREINFORCE only")
     dev = policy.linear1.weight.device
     if dev.type != "cuda":
         raise _lib.RecnnError("recnn_b200 update functions run on CUDA only (policy net is on %s); there is no CPU path" % dev)
