@@ -489,6 +489,32 @@ RECNN_API int64_t recnn_discrete_value_workspace_bytes(const recnn_dims* d, cons
  * except in the selected columns, each the ascending-row sum of its rows' dz1: deterministic), optimizer. */
 RECNN_API int recnn_discrete_value_step(const recnn_discrete_value_args* args, void* stream);
 
+/* ---- REINFORCE: the item-id critic sharded over the item vocabulary, with the policy ---------------
+ * Rank `rank` of `world` holds the action block W1a[:, lo : hi) of the critic and of the target critic, lo =
+ * v->item_offset and hi = lo + args->dims.action_dim, and rows [lo, hi) of the target policy (recnn_vocab_shard above,
+ * the same plan).  args carries the LOCAL dims: each arena is laid out as a Critic(S, hi - lo, H) / DiscreteActor with
+ * hi - lo items; layer 1's state block, its bias and layers 2 and 3 are replicated.  Action ids stay global.  The step
+ * is three phases on one stream with two exchanges between them:
+ *   begin  -> record (recnn_vocab_record_floats(n_rows): header {lo, hi, num_items, n_rows}, then the local max and
+ *             sum of exp of the target policy's logits, and a zero action-logit plane) -> all-gather (recnn_comm_allgather)
+ *   merge  -> terms [2, n_rows, H] = {this rank's part of the target action term, rescaled to the merged max and
+ *             divided by the merged sum; W1a one-hot(action) over the ids this rank holds (0 rows elsewhere)}
+ *          -> all-reduce of terms (recnn_comm_allreduce)
+ *   end    -> the rest of recnn_discrete_value_step from the target critic on, with the summed terms.
+ * After the all-reduce every rank holds the same terms, so the loss and the gradient of every replicated block are the
+ * same bits on every rank and need no exchange; the action block's gradient is rank-local (the columns of the ids it
+ * holds).  The phases share args->workspace (recnn_discrete_value_workspace_bytes of the local dims: it does not grow
+ * with the vocabulary once chunk_items < action_dim), which must be left untouched between them.  At world 1 the three
+ * phases compute exactly what recnn_discrete_value_step does.  losses[4] error bits: 1 as for the step (an id outside
+ * [0, v->num_items), flagged on every rank); 2: the gathered headers do not tile the vocabulary in rank order with this
+ * rank's block, or the ranks disagree on n_rows (the result is then meaningless). */
+RECNN_API int recnn_discrete_value_shard_begin(const recnn_discrete_value_args* args, const recnn_vocab_shard* v,
+                                               float* record, void* stream);
+RECNN_API int recnn_discrete_value_shard_merge(const recnn_discrete_value_args* args, const recnn_vocab_shard* v,
+                                               const float* gathered, float* terms, void* stream);
+RECNN_API int recnn_discrete_value_shard_end(const recnn_discrete_value_args* args, const recnn_vocab_shard* v,
+                                             const float* terms, void* stream);
+
 /* ---- REINFORCE with Top-K correction: the behaviour policy beta ------------------------------------
  * The reference ships beta in its Top-K notebook, not in the library (examples/2. REINFORCE TopK Off Policy
  * Correction/3. TopK Reinforce Off Policy Correction.ipynb, cell 3: class Beta), and DiscreteActor.pi_beta_sample

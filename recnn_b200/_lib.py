@@ -184,6 +184,12 @@ SIGNATURES = {
     "recnn_discrete_value_workspace_bytes": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                          C.c_int32]),
     "recnn_discrete_value_step": (C.c_int, [C.POINTER(DiscreteValueArgs), C.c_void_p]),
+    "recnn_discrete_value_shard_begin": (C.c_int, [C.POINTER(DiscreteValueArgs), C.POINTER(VocabShard), C.c_void_p,
+                                                   C.c_void_p]),
+    "recnn_discrete_value_shard_merge": (C.c_int, [C.POINTER(DiscreteValueArgs), C.POINTER(VocabShard), C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]),
+    "recnn_discrete_value_shard_end": (C.c_int, [C.POINTER(DiscreteValueArgs), C.POINTER(VocabShard), C.c_void_p,
+                                                 C.c_void_p]),
     "recnn_beta_layout": (C.c_int, [C.POINTER(BetaDims), C.POINTER(C.c_int64)]),
     "recnn_beta_workspace_bytes": (C.c_int64, [C.POINTER(BetaDims), C.c_int64, C.c_int32]),
     "recnn_sizeof_beta_args": (C.c_int64, []),

@@ -9,7 +9,9 @@
 //       per chunk c:  P_c = exp(z_c - M_new),  Y <- Y exp(M_old - M_new) + P_c W1a[:, c]^T,  sum <- ...;  Y /= sum
 //   * gradient of the online W1a:            column S + j <- sum over rows m with a_m = j of dz1[m, :]
 //     (sort of (id, row) keys, then one ascending-row sum per distinct id: deterministic, no atomics)
-// Layer 1 then runs over the state block only (K = S) with the addend in the EPI_HIDDEN epilogue.
+// Layer 1 then runs over the state block only (K = S) with the addend in the EPI_HIDDEN epilogue.  Sharded over the
+// item vocabulary (recnn_discrete_value_shard_*), each rank computes both terms over the ids it holds and the ranks'
+// parts are summed; the rest of the step is the same code.
 #pragma once
 
 namespace recnn {
@@ -132,10 +134,11 @@ static int proj_gemm(const float* P, long long ldP, int K, const float* W, long 
 }
 
 // Y[n, H] = softmax(policy logits) W1a^T (policy source: pparams != null, xs = the policy's input) or probs W1a^T
-// (dense source [n, ld_probs]), over item chunks of width W.
+// (dense source [n, ld_probs]), over item chunks of width W.  normalise = false (policy source only) leaves
+// Y = sum exp(z - run_max) W1a^T without the final division by run_sum: a vocabulary shard's part, merged later.
 static int action_term_chunked(const recnn_dims& cd, const float* cparams, const recnn_discrete_dims* pd,
                                const float* pparams, const Seg& xs, const float* probs, long long ld_probs, int64_t n,
-                               int W, const ProjScratch& s, float* Y, cudaStream_t st) {
+                               int W, const ProjScratch& s, float* Y, cudaStream_t st, bool normalise = true) {
   const NetLayout lc = critic_layout(cd);
   const int S = cd.state_dim, I = cd.action_dim, H = cd.hidden, lead = S % 4;
   const int n_chunks = (int)ceil_div(I, W);
@@ -165,34 +168,38 @@ static int action_term_chunked(const recnn_dims& cd, const float* cparams, const
     RECNN_PROPAGATE(proj_gemm(s.P, s.ldP, K, cparams + lc.w1 + (S - lead) + c0, lc.ld1, H, n, proj_splits(n, H, K),
                               s.partial, &splits, st));
     proj_fold_kernel<<<elem_grid(n * H), 256, 0, st>>>(Y, s.partial, splits, n, H, pparams ? s.scale : nullptr,
-                                                       pparams ? s.run_sum : nullptr, c == 0, c == n_chunks - 1);
+                                                       pparams && normalise ? s.run_sum : nullptr, c == 0,
+                                                       c == n_chunks - 1);
     RECNN_CHECK_LAUNCH("proj_fold_kernel");
   }
   return RECNN_OK;
 }
 
-// add[m, :] = W1[:, S + a_m] (the one-hot product); an id outside [0, items) flags *oob and gives a zero row
-__global__ void gather_action_columns_kernel(const float* __restrict__ w1, long long ld1, int S, int H, int items,
-                                             const long long* __restrict__ action, long long n, float* __restrict__ add,
-                                             unsigned* oob) {
+// add[m, :] = W1[:, S + a_m - lo] (the one-hot product) when a_m is one of the `items` ids [lo, lo + items) whose
+// columns this arena holds, else a zero row; an id outside [0, num_items) flags *oob.  Unsharded: lo 0, items ==
+// num_items.
+__global__ void gather_action_columns_kernel(const float* __restrict__ w1, long long ld1, int S, int H, int lo,
+                                             int items, int num_items, const long long* __restrict__ action,
+                                             long long n, float* __restrict__ add, unsigned* oob) {
   const long long total = n * H;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long m = i / H;
     const int h = (int)(i - m * H);
     const long long a = action[m];
-    const bool ok = a >= 0 && a < items;
-    add[i] = ok ? __ldg(w1 + (long long)h * ld1 + S + a) : 0.f;
-    if (!ok && h == 0) *oob = 1u;
+    const long long j = a - lo;
+    add[i] = (j >= 0 && j < items) ? __ldg(w1 + (long long)h * ld1 + S + j) : 0.f;
+    if ((a < 0 || a >= num_items) && h == 0) *oob = 1u;
   }
 }
 
-// keys[i] = (id << 32) | row for i < n (an out-of-range id sorts last as 0xFFFFFFFF), UINT64_MAX in the padding
-__global__ void action_keys_kernel(const long long* __restrict__ action, long long n, long long n2, int items,
+// keys[i] = (id - lo << 32) | row for i < n (an id outside the arena's block [lo, lo + items) sorts last as
+// 0xFFFFFFFF and is skipped), UINT64_MAX in the padding
+__global__ void action_keys_kernel(const long long* __restrict__ action, long long n, long long n2, int lo, int items,
                                    unsigned long long* __restrict__ keys) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += (long long)gridDim.x * blockDim.x) {
     if (i < n) {
-      const long long a = action[i];
-      const unsigned long long id = (a >= 0 && a < items) ? (unsigned long long)a : 0xFFFFFFFFull;
+      const long long j = action[i] - lo;
+      const unsigned long long id = (j >= 0 && j < items) ? (unsigned long long)j : 0xFFFFFFFFull;
       keys[i] = (id << 32) | (unsigned long long)i;
     } else {
       keys[i] = ~0ull;
@@ -227,6 +234,28 @@ __global__ void scatter_action_grad_kernel(const unsigned long long* __restrict_
       float s = 0.f;
       for (long long t = i; t < end; ++t) s += dz1[(long long)(keys[t] & 0xFFFFFFFFull) * H + h];
       gw1a[(long long)h * ld1 + id] = s;
+    }
+  }
+}
+
+// Vocabulary-sharded critic, after the all-gather of the records: terms[0] = Y_r exp(m_r - M) / S (this rank's part of
+// the target action term, merged in rank order as shard_merge_row does for the policy) and terms[1] = add_r.  At W = 1
+// the factor is exp(0) = 1 and S = s_0, and the division is proj_fold_kernel's: the unsharded bits.  One CTA per row.
+__global__ void __launch_bounds__(kRowThreads)
+critic_shard_merge_kernel(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items,
+                          const float* __restrict__ local_max, const float* __restrict__ Y,
+                          const float* __restrict__ add, int H, float* __restrict__ terms, unsigned* plan_bad) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, W, n, rank, lo, hi, items)) *plan_bad = 1u;
+  for (long long r = blockIdx.x; r < n; r += gridDim.x) {
+    float M, S, za;
+    shard_merge_row(g, W, n, r, M, S, za);
+    const float f = expf(local_max[r] - M);
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+      const long long i = r * H + h;
+      float y = Y[i] * f;
+      y /= S;
+      terms[i] = y;
+      terms[n * H + i] = add[i];
     }
   }
 }
@@ -359,15 +388,15 @@ extern "C" int64_t recnn_discrete_value_workspace_bytes(const recnn_dims* d, con
 
 extern "C" int64_t recnn_sizeof_discrete_value_args(void) { return (int64_t)sizeof(recnn_discrete_value_args); }
 
-// misc.py:10-55 in the reference's order: target policy + target critic -> TD target (clamped), online critic, MSE,
-// backward, optimizer.  Everything on `stream`, no allocation, no synchronisation.
-extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, void* stream) {
+// The argument checks of the step and of its sharded phases (dims are the arena's: local ones on a shard); *w <- the
+// carved workspace.
+static int dv_check(const recnn_discrete_value_args* a, DvWorkspace* w) {
   RECNN_REQUIRE(a != nullptr, "args");
   RECNN_REQUIRE(dv_dims_ok(a->dims, a->policy_dims), "dims (critic action_dim == policy num_items, equal state_dim)");
   RECNN_REQUIRE(a->n_rows > 0, "n_rows");
-  const recnn_dims& d = a->dims;
-  const int S = d.state_dim, I = d.action_dim, H = d.hidden;
-  RECNN_REQUIRE(critic_chunk_ok(I, a->chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  const int S = a->dims.state_dim, H = a->dims.hidden;
+  RECNN_REQUIRE(critic_chunk_ok(a->dims.action_dim, a->chunk_items),
+                "chunk_items must be num_items or a positive multiple of 128 below it");
   int64_t widest = pad4(S) > H ? pad4(S) : H;
   if (pad4(S % 4 + a->chunk_items) > widest) widest = pad4(S % 4 + a->chunk_items);
   RECNN_REQUIRE(a->n_rows < (1ll << 31) / (widest + 1), "n_rows too large for int32 tile indexing");
@@ -376,13 +405,46 @@ extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, voi
   RECNN_REQUIRE(!a->learn || a->value.grads, "value net needs a grad arena when learn=1");
   RECNN_REQUIRE(a->losses && a->workspace && a->rng_step, "losses / workspace / rng_step");
   RECNN_REQUIRE((a->masks[0] == nullptr) == (a->masks[1] == nullptr), "give both masks or neither");
-  const int64_t n = a->n_rows;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const DvWorkspace w = dv_carve(d, a->policy_dims, n, a->chunk_items, a->workspace);
-  if (w.bytes > a->workspace_bytes) {
-    set_error("workspace too small: need %lld bytes, got %lld", (long long)w.bytes, (long long)a->workspace_bytes);
+  *w = dv_carve(a->dims, a->policy_dims, a->n_rows, a->chunk_items, a->workspace);
+  if (w->bytes > a->workspace_bytes) {
+    set_error("workspace too small: need %lld bytes, got %lld", (long long)w->bytes, (long long)a->workspace_bytes);
     return RECNN_E_WORKSPACE;
   }
+  return RECNN_OK;
+}
+
+// The action terms of layer 1: the error tickets zeroed, the state images, then
+//   w.Y   = next_action = target_policy_net(next_state) (misc.py:28), consumed only as W1a' next_action -- without its
+//           division by the row sums (normalise = false) on a vocabulary shard;
+//   w.add = W1a one-hot(action) (misc.py:37) over the ids [lo, lo + action_dim) this arena holds.
+static int dv_action_terms(const recnn_discrete_value_args* a, const DvWorkspace& w, int lo, int num_items,
+                           bool normalise, cudaStream_t st) {
+  const recnn_dims& d = a->dims;
+  const int S = d.state_dim, H = d.hidden, ldS = pad4(S);
+  const int64_t n = a->n_rows;
+  const NetLayout lc = critic_layout(d);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(w.tickets, 0, 8 * sizeof(unsigned), st));
+  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(w.S, (size_t)ldS * 4, a->state, (size_t)S * 4, (size_t)S * 4, n,
+                                     cudaMemcpyDeviceToDevice, st));
+  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(w.S2, (size_t)ldS * 4, a->next_state, (size_t)S * 4, (size_t)S * 4, n,
+                                     cudaMemcpyDeviceToDevice, st));
+  const Seg ss2 = {w.S2, S, ldS, 0};
+  RECNN_PROPAGATE(action_term_chunked(d, a->target_value.params, &a->policy_dims, a->target_policy, ss2, nullptr, 0, n,
+                                      a->chunk_items, w.proj, w.Y, st, normalise));
+  gather_action_columns_kernel<<<elem_grid(n * H), 256, 0, st>>>(a->value.params + lc.w1, lc.ld1, S, H, lo, d.action_dim,
+                                                                 num_items, reinterpret_cast<const long long*>(a->action),
+                                                                 n, w.add, w.tickets + kTicketOob);
+  RECNN_CHECK_LAUNCH("gather_action_columns_kernel");
+  return RECNN_OK;
+}
+
+// misc.py:29-44 from the action terms Y and add on, in the reference's order: target critic -> TD target (clamped),
+// online critic, MSE, backward, optimizer.  lo: the global id of the arena's first action column (0 unsharded).
+static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, const float* Y, const float* add, int lo,
+                   cudaStream_t st) {
+  const recnn_dims& d = a->dims;
+  const int S = d.state_dim, I = d.action_dim, H = d.hidden;
+  const int64_t n = a->n_rows;
   const NetLayout lc = critic_layout(d);
   const int ldS = pad4(S);
   const bool train = a->dropout != 0;
@@ -390,28 +452,17 @@ extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, voi
   Rng rng = {nullptr, a->seed, (const long long*)a->rng_step};
   const long long* act = reinterpret_cast<const long long*>(a->action);
   unsigned* oob = w.tickets + kTicketOob;
-  RECNN_CHECK_CUDA(cudaMemsetAsync(w.tickets, 0, 8 * sizeof(unsigned), st));
-  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(w.S, (size_t)ldS * 4, a->state, (size_t)S * 4, (size_t)S * 4, n,
-                                     cudaMemcpyDeviceToDevice, st));
-  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(w.S2, (size_t)ldS * 4, a->next_state, (size_t)S * 4, (size_t)S * 4, n,
-                                     cudaMemcpyDeviceToDevice, st));
   const Seg ss = {w.S, S, ldS, 0}, ss2 = {w.S2, S, ldS, 0};
   const float* Pt = a->target_value.params;
   const float* P = a->value.params;
-
-  // next_action = target_policy_net(next_state) (misc.py:28), consumed only as W1a' next_action = Y
-  RECNN_PROPAGATE(action_term_chunked(d, Pt, &a->policy_dims, a->target_policy, ss2, nullptr, 0, n, a->chunk_items, w.proj,
-                                      w.Y, st));
   // target critic, eval mode (misc.py:29)
   const Seg st1 = {w.t1, H, H, 0};
-  RECNN_PROPAGATE(hidden_layer(ss2, kNoSeg, Pt + lc.w1, lc.ld1, Pt + lc.b1, H, n, false, nullptr, rng, 0, w.t1, st, w.Y));
+  RECNN_PROPAGATE(hidden_layer(ss2, kNoSeg, Pt + lc.w1, lc.ld1, Pt + lc.b1, H, n, false, nullptr, rng, 0, w.t1, st, Y));
   RECNN_PROPAGATE(hidden_layer(st1, kNoSeg, Pt + lc.w2, lc.ld2, Pt + lc.b2, H, n, false, nullptr, rng, 1, w.t2, st));
   // online critic on (state, one-hot(action)) (misc.py:37)
-  gather_action_columns_kernel<<<elem_grid(n * H), 256, 0, st>>>(P + lc.w1, lc.ld1, S, H, I, act, n, w.add, oob);
-  RECNN_CHECK_LAUNCH("gather_action_columns_kernel");
   const Seg sc1 = {w.c1, H, H, 0};
   RECNN_PROPAGATE(hidden_layer(ss, kNoSeg, P + lc.w1, lc.ld1, P + lc.b1, H, n, train, train ? a->masks[0] : nullptr, rng,
-                               0, w.c1, st, w.add));
+                               0, w.c1, st, add));
   RECNN_PROPAGATE(hidden_layer(sc1, kNoSeg, P + lc.w2, lc.ld2, P + lc.b2, H, n, train, train ? a->masks[1] : nullptr, rng,
                                1, w.c2, st));
   // TD target and clamp (misc.py:30-35), MSE (:39), its gradient through the head
@@ -455,7 +506,7 @@ extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, voi
     RECNN_PROPAGATE(weight_grad(w.dz1, H, ss, kNoSeg, n, G + lc.w1, lc.ld1, G + lc.b1, w.partial, st));
     RECNN_CHECK_CUDA(cudaMemset2DAsync(G + lc.w1 + S, (size_t)lc.ld1 * 4, 0, (size_t)I * 4, H, st));
     const int64_t n2 = pow2_at_least(n);
-    action_keys_kernel<<<elem_grid(n2), 256, 0, st>>>(act, n, n2, I, w.keys);
+    action_keys_kernel<<<elem_grid(n2), 256, 0, st>>>(act, n, n2, lo, I, w.keys);
     RECNN_CHECK_LAUNCH("action_keys_kernel");
     for (int64_t k = 2; k <= n2; k <<= 1)
       for (int64_t j = k >> 1; j > 0; j >>= 1) {
@@ -469,9 +520,63 @@ extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, voi
       RECNN_PROPAGATE(launch_optimizer(a->value_optim, a->value, lc.count, nullptr, st, w.tickets + 3));
   }
   // ++rng_step; losses[4] <- error bits (1: an action id outside [0, num_items): its row read a zero action column and
-  // its gradient column was skipped)
+  // its gradient column was skipped; 2: the gathered shard records disagree with the plan)
   RECNN_PROPAGATE(launch_finish((long long*)a->rng_step, oob, w.tickets + kTicketDpMismatch, a->losses + 4, st));
   if (a->losses_host)
     RECNN_CHECK_CUDA(cudaMemcpyAsync(a->losses_host, a->losses, 8 * sizeof(float), cudaMemcpyDeviceToHost, st));
   return RECNN_OK;
+}
+
+// misc.py:10-55: the action terms, then the rest.  Everything on `stream`, no allocation, no synchronisation.
+extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, void* stream) {
+  DvWorkspace w;
+  RECNN_PROPAGATE(dv_check(a, &w));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_PROPAGATE(dv_action_terms(a, w, 0, a->dims.action_dim, true, st));
+  return dv_tail(a, w, w.Y, w.add, 0, st);
+}
+
+// ---- the vocabulary-sharded critic: the phases around the all-gather and the all-reduce (see the header) ---------
+static int dv_shard_check(const recnn_discrete_value_args* a, const recnn_vocab_shard* v, DvWorkspace* w) {
+  RECNN_PROPAGATE(dv_check(a, w));
+  RECNN_REQUIRE(shard_ok(&a->policy_dims, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_value_shard_begin(const recnn_discrete_value_args* a, const recnn_vocab_shard* v,
+                                                float* record, void* stream) {
+  DvWorkspace w;
+  RECNN_PROPAGATE(dv_shard_check(a, v, &w));
+  RECNN_REQUIRE(record != nullptr, "record");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t n = a->n_rows;
+  RECNN_PROPAGATE(dv_action_terms(a, w, v->item_offset, v->num_items, false, st));
+  RECNN_PROPAGATE(shard_record_init(a->policy_dims, *v, record, n, st));
+  RECNN_CHECK_CUDA(cudaMemcpyAsync(record + kShardHeader, w.proj.run_max, n * sizeof(float), cudaMemcpyDeviceToDevice,
+                                   st));
+  RECNN_CHECK_CUDA(cudaMemcpyAsync(record + kShardHeader + n, w.proj.run_sum, n * sizeof(float),
+                                   cudaMemcpyDeviceToDevice, st));
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_value_shard_merge(const recnn_discrete_value_args* a, const recnn_vocab_shard* v,
+                                                const float* gathered, float* terms, void* stream) {
+  DvWorkspace w;
+  RECNN_PROPAGATE(dv_shard_check(a, v, &w));
+  RECNN_REQUIRE(gathered && terms, "gathered / terms");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t n = a->n_rows;
+  critic_shard_merge_kernel<<<row_grid(n), kRowThreads, 0, st>>>(
+      gathered, v->world, n, v->rank, v->item_offset, v->item_offset + a->policy_dims.num_items, v->num_items,
+      w.proj.run_max, w.Y, w.add, a->dims.hidden, terms, w.tickets + kTicketDpMismatch);
+  RECNN_CHECK_LAUNCH("critic_shard_merge_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_value_shard_end(const recnn_discrete_value_args* a, const recnn_vocab_shard* v,
+                                              const float* terms, void* stream) {
+  DvWorkspace w;
+  RECNN_PROPAGATE(dv_shard_check(a, v, &w));
+  RECNN_REQUIRE(terms != nullptr, "terms");
+  return dv_tail(a, w, terms, terms + a->n_rows * a->dims.hidden, v->item_offset, static_cast<cudaStream_t>(stream));
 }

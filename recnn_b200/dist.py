@@ -167,57 +167,178 @@ class VocabParallel:
     def shard(self):
         return _lib.VocabShard(self.lo, self.num_items, self.rank, self.world)
 
+    def _fit(self, need, device):
+        """Grow the communicator (collectively: every rank asks for the same size) to ``need`` floats."""
+        if need > self.comm.capacity:
+            grown = PeerComm(self.group, device, max(need, 2 * self.comm.capacity))
+            self.comm.close()
+            self.comm = grown
+
     def all_gather(self, t: torch.Tensor) -> torch.Tensor:
         """PeerComm.all_gather; the communicator grows (collectively: every rank gathers the same size) when the
         records outgrow it."""
-        need = self.world * t.numel()
-        if need > self.comm.capacity:
-            grown = PeerComm(self.group, t.device, max(need, 2 * self.comm.capacity))
-            self.comm.close()
-            self.comm = grown
+        self._fit(self.world * t.numel(), t.device)
         return self.comm.all_gather(t)
 
+    def all_reduce(self, t: torch.Tensor) -> torch.Tensor:
+        """PeerComm.all_reduce (in place, the same bits on every rank); the communicator grows as for all_gather."""
+        self._fit(t.numel(), t.device)
+        return self.comm.all_reduce(t)
 
-def enable_vocab_parallel(policy, group=None):
-    """Shard a DiscreteActor's item layer over the ranks of ``group``.  Call it on every rank after the policy is on
-    its CUDA device and before its optimizer is built.  The weights are first made identical to rank 0's; then rank r
-    keeps rows vocab_shard(num_items, r, world) of linear2 (so ``state_dict`` holds the local block).  At world 1 the
-    policy computes exactly what it did unsharded.
+    def __deepcopy__(self, memo):
+        # a copied net (a target net) shares the online net's plan and communicator: there is one peer mapping per
+        # process group, and every net of an agent exchanges over it in the same order on every rank
+        return self
 
-    On a sharded policy, ``forward`` / ``select_action`` return the rank's COLUMN BLOCK [N, hi - lo] of the softmax
-    over all items (the reference returns [N, num_items]); sampled ids, log-probs, ``saved_log_probs``, ``correction``
-    and ``lambda_k`` are global and identical on every rank.  Every rank must be fed the same states, seeded the same
-    (torch.manual_seed, or the same ``uniform_source``) and must make the same calls in the same order.
-    ``ChooseREINFORCE`` trains it; ``reinforce_update`` / ``Reinforce`` refuse it (their critic consumes dense
-    probabilities)."""
-    from .nn.arena import _is_discrete, _is_beta, grad_arena
-    if not dist.is_initialized():
-        raise RuntimeError("torch.distributed is not initialised")
-    if _is_beta(policy) or not _is_discrete(policy):
-        raise TypeError("enable_vocab_parallel shards a DiscreteActor")
-    if "_recnn_vp" in policy.__dict__:
-        raise RuntimeError("the policy is already vocabulary-parallel")
-    arena = param_arena(policy)
-    if not arena.is_cuda:
-        raise _lib.RecnnError("enable_vocab_parallel needs the policy on its CUDA device")
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    # every rank checks every rank's plan, so a refused plan raises on all of them (none is left in a collective)
-    sizes = [None] * world
-    dist.all_gather_object(sizes, (policy.linear1.in_features, policy.linear1.out_features,
-                                   policy.linear2.out_features), group=group)
-    if len(set(sizes)) != 1:
-        raise ValueError("the ranks' policies differ in shape: %s" % sizes)
-    num_items = sizes[0][2]
-    plans = [vocab_shard(num_items, r, world) + (num_items,) for r in range(world)]
-    check_vocab_plans(plans)
-    lo, hi, _ = plans[rank]
-    broadcast_nets({"policy_net": policy}, group)
+
+def _shard_policy_rows(policy, lo, hi):
+    from .nn.arena import grad_arena
     with torch.no_grad():
         for p in (policy.linear2.weight, policy.linear2.bias):
             p.grad = None
             p.data = p.data[lo:hi].clone()
     policy.linear2.out_features = hi - lo
+    policy.__dict__.pop("_recnn_engines", None)
     grad_arena(policy)                                  # the local arenas (param_arena rebuilds on the new shapes)
+
+
+def _shard_critic_columns(critic, lo, hi):
+    """Keep the state block of linear1 and the action columns [lo, hi): a Critic(S, hi - lo, H)."""
+    from .nn.arena import grad_arena
+    S = critic.linear1.in_features - critic._action_dim
+    with torch.no_grad():
+        w = critic.linear1.weight
+        w.grad = None
+        w.data = torch.cat([w.data[:, :S], w.data[:, S + lo:S + hi]], 1).contiguous()
+        critic.linear1.bias.grad = None
+    critic.linear1.in_features = S + hi - lo
+    critic._action_dim = hi - lo
+    critic.__dict__.pop("_recnn_ids_steps", None)
+    critic.__dict__.pop("_recnn_engines", None)
+    grad_arena(critic)
+
+
+_AGENT_NETS = ("policy_net", "target_policy_net", "value_net", "target_value_net")
+
+
+def _critic_shape_error(name, net, S, num_items):
+    from .nn.arena import _is_discrete
+    if (_is_discrete(net) or not hasattr(net, "_action_dim") or net.linear3.out_features != 1
+            or net._action_dim != num_items or net.linear1.in_features != S + num_items):
+        return ("nets[%r] must be a Critic(%d, %d, H) (state_dim and num_items of the policy) to be sharded with it"
+                % (name, S, num_items))
+    return None
+
+
+def _rebuild_optimizers(optimizers, nets):
+    """The agent's optimizers on the local arenas: built-in arena optimizers are rebuilt with the same hyperparameters
+    (their state arenas take the local geometry); torch optimizers keep their Parameter objects, which now hold the
+    local blocks.  Optimizers that already hold state are refused (their moments have the unsharded shapes)."""
+    from . import optim as _optim
+    owner = {id(p): name for name, net in nets.items() for p in net.parameters()}
+    for key, opt in list(optimizers.items()):
+        if opt is None:
+            continue
+        if isinstance(opt, _optim._ArenaOptimizer):
+            if opt._t is not None:
+                raise RuntimeError("optimizers[%r] has already stepped; enable vocabulary parallelism before the "
+                                   "first update" % key)
+            group = opt.param_groups[0]
+            net = nets.get(owner.get(id(group["params"][0])))
+            fresh = type(opt)(group["params"], **{k: group[k] for k in opt.defaults})
+            if net is not None:
+                fresh.bind(net)
+            optimizers[key] = fresh
+        elif len(getattr(opt, "state", {})) != 0:
+            raise RuntimeError("optimizers[%r] already holds state; enable vocabulary parallelism before the first "
+                               "update" % key)
+
+
+def enable_vocab_parallel(policy_or_agent, group=None):
+    """Shard a DiscreteActor's item layer -- or a whole REINFORCE agent -- over the ranks of ``group``.  Call it on
+    every rank after the nets are on their CUDA device.  The weights are first made identical to rank 0's.  At world 1
+    everything computes exactly what it did unsharded.
+
+    A DiscreteActor: rank r keeps rows vocab_shard(num_items, r, world) of linear2 (so ``state_dict`` holds the local
+    block); call it before the policy's optimizer is built.  On a sharded policy, ``forward`` / ``select_action``
+    return the rank's COLUMN BLOCK [N, hi - lo] of the softmax over all items (the reference returns [N, num_items]);
+    sampled ids, log-probs, ``saved_log_probs``, ``correction`` and ``lambda_k`` are global and identical on every rank.
+    ``ChooseREINFORCE`` trains it.
+
+    A ``Reinforce`` agent (or its nets dict with policy_net, target_policy_net, value_net and target_value_net): both
+    policies are sharded as above and both critics, which must be Critic(S, num_items, H) for the policy's S and
+    num_items, keep linear1's state block and the action columns [lo, hi) of the same plan: their ``state_dict`` holds
+    the local action block.  The four nets share one ``VocabParallel`` (and so one communicator).  An agent's optimizers
+    are rebuilt on the local arenas with the same hyperparameters (a nets dict's optimizers are the caller's: build them
+    afterwards).  ``value_update`` / ``reinforce_update`` / ``Reinforce.update()`` then run vocabulary-parallel on
+    item-id batch actions (recnn_discrete_value_shard_* in include/recnn_b200.h); a dense [N, num_items] action is
+    refused.  ``debug["next_action"]`` (learn=False) is the rank's column block.
+
+    Every rank must be fed the same batches and states, seeded the same (torch.manual_seed, or the same
+    ``uniform_source``) and must make the same calls in the same order: dropout masks -- given in the batch or drawn --
+    and the masks of reinforce_update's reward line must agree across ranks."""
+    from .nn.arena import _is_discrete, _is_beta
+    if not dist.is_initialized():
+        raise RuntimeError("torch.distributed is not initialised")
+    agent = policy_or_agent if hasattr(policy_or_agent, "nets") else None
+    if agent is not None or isinstance(policy_or_agent, dict):
+        nets = agent.nets if agent is not None else policy_or_agent
+        missing = [k for k in _AGENT_NETS if nets.get(k) is None]
+        if missing:
+            raise ValueError("a REINFORCE agent's nets need %s" % ", ".join(missing))
+        policy = nets["policy_net"]
+    else:
+        nets, policy = None, policy_or_agent
+    if _is_beta(policy) or not _is_discrete(policy):
+        raise TypeError("enable_vocab_parallel shards a DiscreteActor")
+    shard_nets = {"policy_net": policy} if nets is None else {k: nets[k] for k in _AGENT_NETS}
+    for name, net in shard_nets.items():
+        if "_recnn_vp" in net.__dict__:
+            raise RuntimeError("the policy is already vocabulary-parallel" if nets is None
+                               else "nets[%r] is already vocabulary-parallel" % name)
+    S, num_items = policy.linear1.in_features, policy.linear2.out_features
+    if nets is not None:
+        # refused on this rank before any exchange; the shape exchange below makes every rank refuse together
+        tp = nets["target_policy_net"]
+        if (_is_beta(tp) or not _is_discrete(tp) or tp.linear2.weight.shape != policy.linear2.weight.shape
+                or tp.linear1.weight.shape != policy.linear1.weight.shape):
+            raise ValueError("nets['target_policy_net'] must be a DiscreteActor of the policy's shape")
+        for name in ("value_net", "target_value_net"):
+            err = _critic_shape_error(name, nets[name], S, num_items)
+            if err:
+                raise ValueError(err)
+        if nets["target_value_net"].linear1.weight.shape != nets["value_net"].linear1.weight.shape:
+            raise ValueError("nets['target_value_net'] and nets['value_net'] differ in shape")
+    arena = param_arena(policy)
+    if not arena.is_cuda:
+        raise _lib.RecnnError("enable_vocab_parallel needs the policy on its CUDA device")
+    if nets is not None:
+        for name, net in shard_nets.items():
+            if param_arena(net).device != arena.device:
+                raise _lib.RecnnError("nets[%r] is on %s, the policy on %s" % (name, param_arena(net).device,
+                                                                               arena.device))
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    # every rank checks every rank's plan, so a refused plan raises on all of them (none is left in a collective)
+    shape = (S, policy.linear1.out_features, num_items)
+    if nets is not None:
+        shape += (tuple(nets["value_net"].linear1.weight.shape),)
+    sizes = [None] * world
+    dist.all_gather_object(sizes, shape, group=group)
+    if len(set(sizes)) != 1:
+        raise ValueError("the ranks' nets differ in shape: %s" % sizes)
+    plans = [vocab_shard(num_items, r, world) + (num_items,) for r in range(world)]
+    check_vocab_plans(plans)
+    lo, hi, _ = plans[rank]
+    broadcast_nets(shard_nets, group)
+    for name, net in shard_nets.items():
+        if name.endswith("policy_net"):
+            _shard_policy_rows(net, lo, hi)
+        else:
+            _shard_critic_columns(net, lo, hi)
     comm = PeerComm(group, arena.device, vocab_comm_floats(policy.dims, world, 1))
-    policy.__dict__["_recnn_vp"] = VocabParallel(lo, hi, num_items, group, rank, world, comm)
-    return policy
+    vp = VocabParallel(lo, hi, num_items, group, rank, world, comm)
+    for net in shard_nets.values():
+        net.__dict__["_recnn_vp"] = vp
+    if agent is not None and getattr(agent, "optimizers", None):
+        _rebuild_optimizers(agent.optimizers, nets)
+    return policy_or_agent

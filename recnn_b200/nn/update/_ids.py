@@ -91,13 +91,17 @@ def critic_action_term(value_net, probs=None, policy=None, state=None, chunk_ite
 
 def critic_value_of_probs(value_net, state, probs):
     """value_net(state, probs) [N, 1] through the chunked action term instead of a re-pitched [N, num_items] image
-    (same dropout convention as Critic.forward: fresh masks in train mode)."""
+    (same dropout convention as Critic.forward: fresh masks in train mode).  On a vocabulary-parallel critic ``probs``
+    is the rank's column block: the ranks' action terms are all-reduced, and the value is the same on every rank."""
     from ..models import _train_masks
     dev = _stream_device(value_net)
     state = state.detach().to(device=dev, dtype=torch.float32).contiguous()
     n, items = probs.shape
     d = _critic_dims(value_net, items)
     term = critic_action_term(value_net, probs=probs)
+    vp = value_net.__dict__.get("_recnn_vp")
+    if vp is not None and n > 0:
+        vp.all_reduce(term)
     m1, m2 = _train_masks(value_net, n, d.hidden, dev)
     out = torch.empty(n, 1, device=dev, dtype=torch.float32)
     if n == 0:
@@ -200,29 +204,71 @@ class IdsValueStep:
                 self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             a.workspace = self.workspace.data_ptr()
             a.workspace_bytes = self.workspace.numel()
-            _lib.check(L.recnn_discrete_value_step(a, _lib.stream_ptr(dev)))
+            self._launch(L, a, dev)
             if learn and a.value_optim.kind == _lib.OPT_EXTERNAL and vo is not None:
                 grad_arena(value)          # re-attach p.grad views if zero_grad(set_to_none) dropped them
                 vo.step()
             torch.cuda.current_stream(dev).synchronize()
-            if int(self.losses_host.view(torch.int32)[4]) & 1:
+            bits = int(self.losses_host.view(torch.int32)[4])
+            if bits & 2:
+                raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+            if bits & 1:
                 raise IndexError("batch['action'] holds an item id outside [0, num_items) (the update was applied with "
                                  "the offending rows' action term set to zero)")
             if not learn:
                 debug["next_action"] = nets["target_policy_net"](next_state)       # the reference's debug contract
             return float(self.losses_host[0])
 
+    def _launch(self, L, a, dev):
+        _lib.check(L.recnn_discrete_value_step(a, _lib.stream_ptr(dev)))
+
+
+class ShardedIdsValueStep(IdsValueStep):
+    """IdsValueStep of nets sharded over the item vocabulary (recnn_b200.dist.enable_vocab_parallel on the agent): the
+    critics hold the action columns of the rank's item block, the target policy its rows.  The step is the three phases
+    of recnn_discrete_value_shard_* with an all-gather of the records and an all-reduce of the [2, N, H] action terms
+    between them; the loss and the error bits come back with the same single synchronisation and are the same on every
+    rank."""
+
+    def __init__(self, nets, device):
+        super().__init__(nets, device)
+        self.vp = nets["value_net"].__dict__["_recnn_vp"]
+
+    def _launch(self, L, a, dev):
+        vp, shard, st = self.vp, self.vp.shard(), _lib.stream_ptr(dev)
+        n = a.n_rows
+        record = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+        _lib.check(L.recnn_discrete_value_shard_begin(a, shard, record.data_ptr(), st))
+        gathered = vp.all_gather(record)
+        terms = torch.empty(2 * n * a.dims.hidden, device=dev, dtype=torch.float32)
+        _lib.check(L.recnn_discrete_value_shard_merge(a, shard, gathered.data_ptr(), terms.data_ptr(), st))
+        vp.all_reduce(terms)
+        _lib.check(L.recnn_discrete_value_shard_end(a, shard, terms.data_ptr(), st))
+
+
+def vocab_parallel_of(nets, names=("value_net", "target_value_net", "target_policy_net")):
+    """The VocabParallel the named nets share, or None when none is sharded; RuntimeError when only some are, or they
+    were sharded apart."""
+    vps = [nets[k].__dict__.get("_recnn_vp") for k in names]
+    if all(v is None for v in vps):
+        return None
+    if any(v is not vps[0] for v in vps):
+        raise RuntimeError("%s must be sharded together: recnn_b200.dist.enable_vocab_parallel(agent or nets dict)"
+                           % ", ".join(names))
+    return vps[0]
+
 
 def get_ids_step(nets, device) -> IdsValueStep:
     """Cached on the value net, like the step engines on the policy net."""
     if nets["policy_net"].__dict__.get("_recnn_dp") is not None and nets["policy_net"].__dict__["_recnn_dp"][1] > 1:
         raise ValueError("item-id actions run on one GPU: data parallel is not supported in this mode")
+    cls = IdsValueStep if vocab_parallel_of(nets) is None else ShardedIdsValueStep
     value = nets["value_net"]
     cache = value.__dict__.setdefault("_recnn_ids_steps", {})
     dev = torch.device(device)
     key = (dev.type, dev.index)
     s = cache.get(key)
-    if s is None or s.pdims.num_items != nets["target_policy_net"].dims.num_items:
-        s = IdsValueStep(nets, dev)
+    if s is None or type(s) is not cls or s.pdims.num_items != nets["target_policy_net"].dims.num_items:
+        s = cls(nets, dev)
         cache[key] = s
     return s

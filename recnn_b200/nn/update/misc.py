@@ -27,6 +27,8 @@ def value_update(batch, params, nets, optimizer, device=torch.device("cpu"), deb
         if not _ids._is_discrete(nets["target_policy_net"]):
             raise ValueError("item-id actions need a DiscreteActor target policy (nets['target_policy_net'])")
         return torch.tensor(_ids.get_ids_step(nets, device).run(batch, params, nets, optimizer, learn, debug))
+    if nets.get("value_net") is not None and "_recnn_vp" in nets["value_net"].__dict__:
+        raise RuntimeError("a vocabulary-parallel critic (enable_vocab_parallel) is trained on item-id batch actions only")
     eng = get_engine(_lib.ALGO_DDPG, nets, device)
     vals = eng.value_only(batch, params, nets, optimizer, learn, debug)
     return torch.tensor(vals[0])

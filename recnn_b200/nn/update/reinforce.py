@@ -151,13 +151,23 @@ class ChooseREINFORCE:
 def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"), debug=None,
                      writer=DummyWriter(), learn=True, step=-1):
     """Same signature, side effects and return value as the reference (reinforce.py:68-129): returns the losses dict
-    on policy steps (step % policy_step == 0 and step > 0) and None otherwise."""
+    on policy steps (step % policy_step == 0 and step > 0) and None otherwise.
+
+    With nets sharded over the item vocabulary (recnn_b200.dist.enable_vocab_parallel on the agent) the batch action
+    must be item ids: the reward line feeds the critic the policy's column block (action terms all-reduced) and the
+    critic step runs vocabulary-parallel.  Every rank must make the call with the same batch."""
     # Due to its mechanics, reinforce doesn't support testing (reinforce.py:80-81)
     learn = True
     policy = nets["policy_net"]
-    if "_recnn_vp" in policy.__dict__:
-        raise RuntimeError("reinforce_update feeds the policy's dense [N, num_items] probabilities to its critic; a "
-                           "vocabulary-parallel policy (enable_vocab_parallel) trains through ChooseREINFORCE only")
+    vp = policy.__dict__.get("_recnn_vp")
+    if vp is not None:
+        critics = [nets.get(k) for k in ("value_net", "target_value_net", "target_policy_net")]
+        if not _ids.is_item_ids(batch["action"]) or any(c is None or c.__dict__.get("_recnn_vp") is not vp
+                                                        for c in critics):
+            raise RuntimeError("reinforce_update feeds the policy's probabilities to its critic: a vocabulary-parallel "
+                               "policy needs item-id batch actions and its critics, target policy included, sharded "
+                               "with it (enable_vocab_parallel on the agent); on its own it trains through "
+                               "ChooseREINFORCE only")
     dev = policy.linear1.weight.device
     if dev.type != "cuda":
         raise _lib.RecnnError("recnn_b200 update functions run on CUDA only (policy net is on %s); there is no CPU path" % dev)
