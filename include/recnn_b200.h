@@ -12,6 +12,10 @@
  *   - every call takes the CUDA stream to launch on (cudaStream_t as void*);
  *     nothing synchronises, nothing allocates: scratch comes from the caller
  *     (recnn_step_workspace_bytes);
+ *   - workspace / scratch pointers may be any address: the size a
+ *     *_workspace_bytes / *_scratch_floats query reports includes alignment
+ *     slack.  A call that takes workspace_bytes returns RECNN_E_WORKSPACE when
+ *     it is below the reported size, before launching anything;
  *   - return 0 on success, a negative RECNN_E_* code otherwise;
  *     recnn_b200_last_error() returns a thread-local message;
  *   - all floating point data is fp32, item indices are int64 (as the
@@ -318,7 +322,8 @@ enum { RECNN_METRIC_L2 = 0, RECNN_METRIC_IP = 1, RECNN_METRIC_COS = 2 };
 RECNN_API int recnn_item_norms(const float* table, int64_t n_items, int32_t dim, int32_t metric, float* out,
                                void* stream);
 RECNN_API int64_t recnn_retrieve_workspace_bytes(int64_t n_queries, int64_t n_items, int32_t k);
-/* ids_out int64[n_queries, k], dist_out fp32[n_queries, k]; norms from recnn_item_norms (NULL for IP) */
+/* ids_out int64[n_queries, k], dist_out fp32[n_queries, k]; norms from recnn_item_norms (NULL for IP);
+ * workspace: any address, workspace_bytes >= recnn_retrieve_workspace_bytes (else RECNN_E_WORKSPACE) */
 RECNN_API int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
                                   int64_t n_items, const float* norms, int32_t metric, int32_t k,
                                   int64_t* ids_out, float* dist_out, void* workspace, int64_t workspace_bytes,

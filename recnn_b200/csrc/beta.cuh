@@ -45,20 +45,14 @@ struct BetaWorkspace {
 
 static BetaWorkspace beta_carve(const recnn_beta_dims& d, int64_t n, int chunk, void* base) {
   BetaWorkspace w;
-  char* p = static_cast<char*>(base);
-  int64_t off = 0;
-  auto take = [&](int64_t floats) {
-    float* r = base ? reinterpret_cast<float*>(p + off) : nullptr;
-    off += round_up(floats * 4, 256);
-    return r;
-  };
-  w.img = take(n * pad4(d.state_dim));
-  w.dz = take(n * (int64_t)chunk);
+  Carve c(base);
+  w.img = c.take(n * pad4(d.state_dim));
+  w.dz = c.take(n * (int64_t)chunk);
   float** rows[7] = {&w.run_max, &w.run_sum, &w.za, &w.T, &w.pe, &w.pa, &w.row_loss};
-  for (auto r : rows) *r = take(n);
-  w.partial = take(chunked_partial_floats(chunk, d.num_items, d.state_dim, n));
-  w.flags = reinterpret_cast<unsigned*>(take(8));
-  w.bytes = off;
+  for (auto r : rows) *r = c.take(n);
+  w.partial = c.take(chunked_partial_floats(chunk, d.num_items, d.state_dim, n));
+  w.flags = c.take<unsigned>(8);
+  w.bytes = c.bytes();
   return w;
 }
 
@@ -173,10 +167,7 @@ extern "C" int recnn_beta_step(const recnn_beta_args* a, void* stream) {
   const int64_t n = a->n_rows;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const BetaWorkspace w = beta_carve(a->dims, n, W, a->workspace);
-  if (w.bytes > a->workspace_bytes) {
-    set_error("workspace too small: need %lld bytes, got %lld", (long long)w.bytes, (long long)a->workspace_bytes);
-    return RECNN_E_WORKSPACE;
-  }
+  RECNN_PROPAGATE(check_workspace(w.bytes, a->workspace_bytes));
   const BetaLayout l = beta_layout(a->dims);
   const float* P = a->net.params;
   float* G = a->net.grads;

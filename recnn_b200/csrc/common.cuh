@@ -52,6 +52,36 @@ constexpr int kNumSMs = 132;   // H100 SXM: grid caps; kernels that need every C
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
 
+// ---- caller-provided workspace / scratch ------------------------------------
+// Every entry point lays out the memory it is given with ONE layout function over a Carve: run on a null base it only
+// sizes (the *_workspace_bytes / *_scratch_floats queries), run on the caller's pointer it cuts the same slices, so
+// the query and the call cannot disagree.  Every slice starts on a 256-byte boundary (TMA needs 16).  The base is
+// aligned up first and the size counts that slack, so any caller address works.
+constexpr int64_t kCarveAlign = 256;
+struct Carve {
+  char* base;        // aligned; null: sizing only
+  int64_t off = 0;
+  explicit Carve(void* p)
+      : base(p ? reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(p) + kCarveAlign - 1) &
+                                         ~static_cast<uintptr_t>(kCarveAlign - 1))
+               : nullptr) {}
+  template <class T = float>
+  T* take(int64_t count) {
+    T* r = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += round_up(count * (int64_t)sizeof(T), kCarveAlign);
+    return r;
+  }
+  int64_t bytes() const { return off + kCarveAlign; }     // + the slack of aligning an arbitrary base
+  int64_t floats() const { return ceil_div(bytes(), 4); }
+};
+
+// RECNN_E_WORKSPACE (with both sizes in the message) unless the caller's `have` bytes hold a layout of `need` bytes
+static inline int check_workspace(int64_t need, int64_t have) {
+  if (need <= have) return RECNN_OK;
+  set_error("workspace too small: need %lld bytes, got %lld", (long long)need, (long long)have);
+  return RECNN_E_WORKSPACE;
+}
+
 // ---- arena layout of one MLP (nn.Module.parameters() order) -----------------
 // Weight rows are padded to a multiple of 4 floats (16 bytes) so that every matrix in the arena is
 // a legal TMA tensor: linear1.weight of the Actor is [H, 1290] with row pitch 1292, of the Critic

@@ -36,29 +36,21 @@ struct ProjScratch {
   float *run_max, *run_sum, *scale;
   float* partial;                // [splits, n, H]
   long long ldP;
-  int64_t floats;
 };
-static ProjScratch proj_carve(const recnn_dims& cd, const recnn_discrete_dims* pd, int64_t n, int chunk, float* base) {
+static ProjScratch proj_carve(const recnn_dims& cd, const recnn_discrete_dims* pd, int64_t n, int chunk, Carve& c) {
   ProjScratch s;
-  int64_t off = 0;
-  auto take = [&](int64_t floats) {
-    float* r = base ? base + off : nullptr;
-    off += round_up(floats, 64);
-    return r;
-  };
   const int lead = cd.state_dim % 4;
   s.ldP = pad4(lead + chunk);
   s.img = s.ph = nullptr;
   if (pd) {
-    s.img = take(n * pad4(pd->state_dim));
-    s.ph = take(n * pd->hidden);
+    s.img = c.take(n * pad4(pd->state_dim));
+    s.ph = c.take(n * pd->hidden);
   }
-  s.P = take(n * s.ldP);
-  s.run_max = take(n);
-  s.run_sum = take(n);
-  s.scale = take(n);
-  s.partial = take((int64_t)proj_splits(n, cd.hidden, lead + chunk) * n * cd.hidden);
-  s.floats = off + 64;
+  s.P = c.take(n * s.ldP);
+  s.run_max = c.take(n);
+  s.run_sum = c.take(n);
+  s.scale = c.take(n);
+  s.partial = c.take((int64_t)proj_splits(n, cd.hidden, lead + chunk) * n * cd.hidden);
   return s;
 }
 
@@ -281,36 +273,24 @@ struct DvWorkspace {
 
 static DvWorkspace dv_carve(const recnn_dims& d, const recnn_discrete_dims& pd, int64_t n, int chunk, void* base) {
   DvWorkspace w;
-  char* p = static_cast<char*>(base);
-  int64_t off = 0;
-  auto take = [&](int64_t floats) {
-    float* r = base ? reinterpret_cast<float*>(p + off) : nullptr;
-    off += round_up(floats * 4, 256);
-    return r;
-  };
+  Carve c(base);
   const int ldS = pad4(d.state_dim), H = d.hidden;
-  w.S = take(n * ldS);
-  w.S2 = take(n * ldS);
+  w.S = c.take(n * ldS);
+  w.S2 = c.take(n * ldS);
   float** hb[8] = {&w.c1, &w.c2, &w.dz2, &w.dz1, &w.t1, &w.t2, &w.add, &w.Y};
-  for (auto b : hb) *b = take(n * H);
-  w.y = take(n);
-  w.qtmp = take(n);
-  w.dq = take(n);
-  int64_t part = (int64_t)kNumSMs * (H + 2);            // block partials of the fused value-head kernel
+  for (auto b : hb) *b = c.take(n * H);
+  w.y = c.take(n);
+  w.qtmp = c.take(n);
+  w.dq = c.take(n);
+  int64_t part = head_partial_floats(H, n);
   const int shapes[3][2] = {{H, d.state_dim}, {H, H}, {1, H}};
-  for (auto& s : shapes)
-    for (int tcp = 0; tcp < 2; ++tcp) {
-      const int64_t f = (int64_t)dw_splits(s[0], s[1], n, tcp != 0) * s[0] * (s[1] + 1);
-      if (f > part) part = f;
-    }
-  w.partial = take(part);
-  w.block_partials = take(1024);
-  w.tickets = reinterpret_cast<unsigned*>(take(8));
-  w.keys = reinterpret_cast<unsigned long long*>(take(2 * pow2_at_least(n)));
-  const ProjScratch sz = proj_carve(d, &pd, n, chunk, nullptr);
-  float* pb = take(sz.floats);
-  w.proj = proj_carve(d, &pd, n, chunk, pb ? align_floats(pb) : nullptr);
-  w.bytes = off;
+  for (auto& s : shapes) part = std::max(part, dw_partial_floats(s[0], s[1], n));
+  w.partial = c.take(part);
+  w.block_partials = c.take(1024);
+  w.tickets = c.take<unsigned>(8);
+  w.keys = c.take<unsigned long long>(pow2_at_least(n));
+  w.proj = proj_carve(d, &pd, n, chunk, c);
+  w.bytes = c.bytes();
   return w;
 }
 
@@ -326,7 +306,9 @@ using namespace recnn;
 extern "C" int64_t recnn_critic_action_term_scratch_floats(const recnn_dims* d, const recnn_discrete_dims* pd,
                                                            int64_t n_rows, int32_t chunk_items) {
   if (!d || n_rows <= 0 || d->state_dim <= 0 || d->hidden <= 0 || !critic_chunk_ok(d->action_dim, chunk_items)) return 0;
-  return proj_carve(*d, pd, n_rows, chunk_items, nullptr).floats;
+  Carve c(nullptr);
+  proj_carve(*d, pd, n_rows, chunk_items, c);
+  return c.floats();
 }
 
 extern "C" int recnn_critic_action_term_chunked(const recnn_dims* d, const float* critic_params,
@@ -342,7 +324,8 @@ extern "C" int recnn_critic_action_term_chunked(const recnn_dims* d, const float
   RECNN_REQUIRE(critic_chunk_ok(d->action_dim, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   if (n_rows <= 0) return RECNN_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const ProjScratch s = proj_carve(*d, policy_params ? pd : nullptr, n_rows, chunk_items, align_floats(scratch));
+  Carve c(scratch);
+  const ProjScratch s = proj_carve(*d, policy_params ? pd : nullptr, n_rows, chunk_items, c);
   Seg xs = kNoSeg;
   if (policy_params) {
     recnn_dims dd;
@@ -362,20 +345,18 @@ extern "C" int recnn_critic_forward_action_term(const recnn_dims* d, const float
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const NetLayout l = critic_layout(*d);
   const int H = d->hidden;
-  float* h1 = scratch;
-  float* h2 = scratch + n_rows * H;
-  float* img = reinterpret_cast<float*>(round_up(reinterpret_cast<int64_t>(h2 + n_rows * H), 16));
+  const ForwardScratch s = forward_carve(*d, n_rows, false, scratch);
   Rng rng = {nullptr, 0, nullptr};
   const bool train = mask1 != nullptr;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, img, &xs, st));
-  const Seg s1 = {h1, H, H, 0};
-  RECNN_PROPAGATE(hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, h1, st,
-                               action_term));
-  RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, h2, st));
+  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, s.img, &xs, st));
+  const Seg s1 = {s.h1, H, H, 0};
+  RECNN_PROPAGATE(hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, s.h1,
+                               st, action_term));
+  RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, s.h2, st));
   HeadArgs h;
   memset(&h, 0, sizeof(h));
-  h.h2 = h2; h.w3 = params + l.w3; h.b3 = params + l.b3; h.n_rows = n_rows; h.n_rows_global = n_rows;
+  h.h2 = s.h2; h.w3 = params + l.w3; h.b3 = params + l.b3; h.n_rows = n_rows; h.n_rows_global = n_rows;
   h.hidden = H; h.mode = HEAD_PLAIN; h.out = value_out;
   return launch_critic_head(h, st);
 }
@@ -406,11 +387,7 @@ static int dv_check(const recnn_discrete_value_args* a, DvWorkspace* w) {
   RECNN_REQUIRE(a->losses && a->workspace && a->rng_step, "losses / workspace / rng_step");
   RECNN_REQUIRE((a->masks[0] == nullptr) == (a->masks[1] == nullptr), "give both masks or neither");
   *w = dv_carve(a->dims, a->policy_dims, a->n_rows, a->chunk_items, a->workspace);
-  if (w->bytes > a->workspace_bytes) {
-    set_error("workspace too small: need %lld bytes, got %lld", (long long)w->bytes, (long long)a->workspace_bytes);
-    return RECNN_E_WORKSPACE;
-  }
-  return RECNN_OK;
+  return check_workspace(w->bytes, a->workspace_bytes);
 }
 
 // The action terms of layer 1: the error tickets zeroed, the state images, then
@@ -492,9 +469,8 @@ static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, con
     h.w3 = P + lc.w3; h.b3 = P + lc.b3; h.h2 = w.c2; h.mode = HEAD_VALUE; h.loss = a->losses;
     RECNN_PROPAGATE(launch_critic_head(h, st));
     if (a->learn) {
-      const int64_t rows_per = 256;
-      const int splits = (int)ceil_div(n, rows_per);
-      RECNN_PROPAGATE(launch_head_grad_partials(w.dq, w.c2, n, H, rows_per, splits, w.partial, st));
+      const int splits = (int)ceil_div(n, kHeadGradRowsPerSplit);
+      RECNN_PROPAGATE(launch_head_grad_partials(w.dq, w.c2, n, H, kHeadGradRowsPerSplit, splits, w.partial, st));
       RECNN_PROPAGATE(launch_reduce_partials(w.partial, splits, 1, H + 1, G + lc.w3, lc.ld3, G + lc.b3, st));
       RECNN_PROPAGATE(launch_critic_head_bwd(w.dq, 0.f, P + lc.w3, w.c2, gate, w.dz2, n, H, st));
     }

@@ -477,42 +477,20 @@ static bool chunk_ok(const recnn_discrete_dims& d, int64_t chunk) {
   return chunk == d.num_items || (chunk > 0 && chunk % 128 == 0 && chunk < d.num_items);
 }
 
-// split-K partial space of a weight gradient dW[C, K] over `rows` (either back end); *one_split: both use one split
-static int64_t dw_partial_floats(int C, int K, int64_t rows, bool* one_split) {
-  int64_t best = 0;
-  bool one = true;
-  for (int tcp = 0; tcp < 2; ++tcp) {
-    const int s = dw_splits(C, K, rows, tcp != 0);
-    const int64_t f = (int64_t)s * C * (K + 1);
-    if (f > best) best = f;
-    one = one && s == 1;
-  }
-  if (one_split) *one_split = one;
-  return best;
-}
-
-// ... of a weight gradient [num_items, K] computed in row blocks of `chunk` items, the last one possibly narrower.
-// dw_splits sees a block's width only through ceil(width / 128) and the partials grow with the width at a fixed split
-// count, so the widest width of every 128-band bounds that band; once both back ends use one split, the partials only
-// grow with the width.  Independent of num_items when chunk < num_items.
+// split-K partial floats of a weight gradient [num_items, K] computed in row blocks of `chunk` items, the last one
+// possibly narrower.  dw_splits sees a block's width only through ceil(width / 128) and the partials grow with the width
+// at a fixed split count, so the widest width of every 128-band bounds that band; once both back ends use one split
+// (the partials are exactly [c, K + 1]), they only grow with the width.  Independent of num_items when chunk < num_items.
 static int64_t chunked_partial_floats(int chunk, int num_items, int K, int64_t rows) {
-  int64_t best = 0;
+  int64_t best = dw_partial_floats(chunk, K, rows);
   if (chunk != num_items) {
-    bool one = false;
-    for (int64_t c = 128; c < chunk && !one; c += 128) {
-      const int64_t f = dw_partial_floats((int)c, K, rows, &one);
-      if (f > best) best = f;
+    for (int64_t c = 128; c < chunk; c += 128) {
+      const int64_t f = dw_partial_floats((int)c, K, rows);
+      best = std::max(best, f);
+      if (f == c * (K + 1)) break;
     }
   }
-  const int64_t f = dw_partial_floats(chunk, K, rows, nullptr);
-  return f > best ? f : best;
-}
-
-// the two weight gradients of the policy, dW2 in row blocks of `chunk` items
-static int64_t reinforce_partial_floats(const recnn_discrete_dims& d, int64_t rows, int chunk) {
-  const int64_t f1 = dw_partial_floats(d.hidden, d.state_dim, rows, nullptr);
-  const int64_t f2 = chunked_partial_floats(chunk, d.num_items, d.hidden, rows);
-  return f1 > f2 ? f1 : f2;
+  return best;
 }
 
 struct DiscreteScratch {
@@ -520,34 +498,28 @@ struct DiscreteScratch {
   int* flags;
   int64_t floats;
 };
-// chunk == 0: the forward only.  Otherwise the policy gradient over item chunks of `chunk` (z is [n, chunk]).
-static DiscreteScratch discrete_carve(const recnn_discrete_dims& d, int64_t n, int chunk, float* base) {
+// chunk == 0: the forward only.  Otherwise the policy gradient over item chunks of `chunk` (z is [n, chunk]) and its
+// two weight gradients, dW2 in row blocks of `chunk` items.
+static DiscreteScratch discrete_carve(const recnn_discrete_dims& d, int64_t n, int chunk, void* base) {
   DiscreteScratch s;
-  int64_t off = 0;
-  auto take = [&](int64_t floats) {
-    float* r = base ? base + off : nullptr;
-    off += round_up(floats, 64);
-    return r;
-  };
-  s.img = take(n * pad4(d.state_dim));
-  s.h = take(n * d.hidden);
-  s.flags = reinterpret_cast<int*>(take(4));
+  Carve c(base);
+  s.img = c.take(n * pad4(d.state_dim));
+  s.h = c.take(n * d.hidden);
+  s.flags = c.take<int>(4);
   s.z = s.dh = s.row_loss = s.run_max = s.run_sum = s.za = s.g = s.partial = nullptr;
   if (chunk > 0) {
-    s.z = take(n * (int64_t)chunk);
-    s.dh = take(n * d.hidden);
-    s.row_loss = take(n);
-    s.run_max = take(n);
-    s.run_sum = take(n);
-    s.za = take(n);
-    s.g = take(n);
-    s.partial = take(reinforce_partial_floats(d, n, chunk));
+    s.z = c.take(n * (int64_t)chunk);
+    s.dh = c.take(n * d.hidden);
+    s.row_loss = c.take(n);
+    s.run_max = c.take(n);
+    s.run_sum = c.take(n);
+    s.za = c.take(n);
+    s.g = c.take(n);
+    s.partial = c.take(std::max(dw_partial_floats(d.hidden, d.state_dim, n),
+                                chunked_partial_floats(chunk, d.num_items, d.hidden, n)));
   }
-  s.floats = off + 64;
+  s.floats = c.floats();
   return s;
-}
-static float* align_floats(float* p) {      // 256-byte aligned start inside the caller's scratch
-  return reinterpret_cast<float*>(round_up(reinterpret_cast<int64_t>(p), 256));
 }
 
 // h = relu(W1 s + b1) into s.h, kept for the backward; *xs_out = the re-pitched state
@@ -642,7 +614,7 @@ extern "C" int recnn_discrete_forward(const recnn_discrete_dims* d, const float*
   RECNN_REQUIRE(discrete_dims_ok(d) && params && state && probs_out && scratch, "null pointer / dims");
   if (n_rows <= 0) return RECNN_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const DiscreteScratch s = discrete_carve(*d, n_rows, 0, align_floats(scratch));
+  const DiscreteScratch s = discrete_carve(*d, n_rows, 0, scratch);
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
   RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, 0, d->num_items, probs_out, st));
   softmax_rows_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(probs_out, d->num_items, n_rows, d->num_items);
@@ -689,7 +661,7 @@ extern "C" int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d,
   RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long* act = reinterpret_cast<const long long*>(action);
-  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, align_floats(scratch));
+  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, scratch);
   RECNN_CHECK_CUDA(cudaMemsetAsync(s.flags, 0, 4 * sizeof(int), st));
   Seg xs;
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, &xs));
@@ -738,7 +710,7 @@ extern "C" int recnn_reinforce_shard_stats(const recnn_discrete_dims* d, const r
   RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
   RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, align_floats(scratch));
+  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, scratch);
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
   RECNN_PROPAGATE(shard_record_init(*d, *v, record, n_rows, st));
   float* m = record + kShardHeader;
@@ -762,7 +734,7 @@ extern "C" int recnn_reinforce_shard_grad(const recnn_discrete_dims* d, const re
   RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long* act = reinterpret_cast<const long long*>(action);
-  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, align_floats(scratch));
+  const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, scratch);
   RECNN_CHECK_CUDA(cudaMemsetAsync(s.flags, 0, 4 * sizeof(int), st));
   // the stats phase left the state image (when one was needed) in s.img
   const int S = d->state_dim;
@@ -791,7 +763,7 @@ extern "C" int recnn_discrete_shard_forward(const recnn_discrete_dims* d, const 
   RECNN_REQUIRE(n_rows > 0, "n_rows");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int I = d->num_items;
-  const DiscreteScratch s = discrete_carve(*d, n_rows, 0, align_floats(scratch));
+  const DiscreteScratch s = discrete_carve(*d, n_rows, 0, scratch);
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
   RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, 0, I, probs_out, st));
   RECNN_PROPAGATE(shard_record_init(*d, *v, record, n_rows, st));

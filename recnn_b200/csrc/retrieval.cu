@@ -176,6 +176,23 @@ static int64_t slab_rows(int64_t n_items) {
   return r < 128 ? 128 : (r > 4096 ? 4096 : r);
 }
 
+struct RetrieveWorkspace {
+  int64_t slab, ld;    // query rows per slab; row pitch of the scores
+  float* scores;       // [slab, ld]
+  Cand* part;          // [slab, splits <= 32, k] candidates of every (query, column range)
+  int64_t bytes;
+};
+static RetrieveWorkspace retrieve_carve(int64_t n_queries, int64_t n_items, int k, void* base) {
+  RetrieveWorkspace w;
+  Carve c(base);
+  w.slab = n_queries < slab_rows(n_items) ? n_queries : slab_rows(n_items);
+  w.ld = round_up(n_items, 4);
+  w.scores = c.take(w.slab * w.ld);
+  w.part = c.take<Cand>(w.slab * 32 * (int64_t)k);
+  w.bytes = c.bytes();
+  return w;
+}
+
 }  // namespace recnn
 
 using namespace recnn;
@@ -192,10 +209,7 @@ extern "C" int recnn_item_norms(const float* table, int64_t n_items, int32_t dim
 
 extern "C" int64_t recnn_retrieve_workspace_bytes(int64_t n_queries, int64_t n_items, int32_t k) {
   if (n_queries <= 0 || n_items <= 0 || k <= 0) return 0;
-  const int64_t rows = n_queries < slab_rows(n_items) ? round_up(n_queries, 1) : slab_rows(n_items);
-  const int64_t scores = round_up(rows * round_up(n_items, 4) * 4, 256);
-  const int64_t part = round_up(rows * 32 * (int64_t)k * (int64_t)sizeof(Cand), 256);
-  return scores + part;
+  return retrieve_carve(n_queries, n_items, k, nullptr).bytes;
 }
 
 extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
@@ -208,12 +222,12 @@ extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int3
   RECNN_REQUIRE(k >= 1 && k <= 64 && k <= n_items, "1 <= k <= min(64, n_items)");
   RECNN_REQUIRE(n_items < (1ll << 31), "n_items must fit int32");
   if (n_queries == 0) return RECNN_OK;
-  RECNN_REQUIRE(workspace_bytes >= recnn_retrieve_workspace_bytes(n_queries, n_items, k), "workspace too small");
+  const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, k, workspace);
+  RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int64_t ld = round_up(n_items, 4);
-  const int64_t slab = n_queries < slab_rows(n_items) ? n_queries : slab_rows(n_items);
-  float* scores = static_cast<float*>(workspace);
-  Cand* part = reinterpret_cast<Cand*>(static_cast<char*>(workspace) + round_up(slab * ld * 4, 256));
+  const int64_t ld = w.ld, slab = w.slab;
+  float* scores = w.scores;
+  Cand* part = w.part;
   const bool tc_ok = dim % 4 == 0 && (reinterpret_cast<uintptr_t>(queries) & 15) == 0 &&
                      (reinterpret_cast<uintptr_t>(table) & 15) == 0;
   for (int64_t q0 = 0; q0 < n_queries; q0 += slab) {

@@ -14,6 +14,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "gemm_simt.cuh"
 #include "pointwise.cuh"
@@ -109,62 +111,51 @@ static int dw_splits(int C, int K, int64_t n_rows, bool tc_path, int bn = 128) {
   return (int)(s < 1 ? 1 : s);
 }
 
+// split-K partial floats of a weight gradient dW[C, K] over `rows`: the larger of the two back ends' split counts times
+// [C, K + 1] (the bias column).  Every partial buffer a weight_grad() call can use is sized by this.
+static int64_t dw_partial_floats(int C, int K, int64_t rows) {
+  const int s = std::max(dw_splits(C, K, rows, true), dw_splits(C, K, rows, false));
+  return (int64_t)s * C * (K + 1);
+}
+
 // rows per split of the unfused value head's gradient (launch_head_grad_partials)
 constexpr int64_t kHeadGradRowsPerSplit = 256;
 
+// the value head's partials, which no dw_partial_floats() bounds: the fused kernel's block partials, and the unfused
+// head's [splits][1][H+1] of dW3 / db3 at one split per 256 rows (n = 1000, H = 512: 4 splits vs
+// dw_splits(1, 512, 1000, false) = 3)
+static int64_t head_partial_floats(int H, int64_t n_rows) {
+  return std::max((int64_t)kNumSMs * (H + 2), ceil_div(n_rows, kHeadGradRowsPerSplit) * (H + 1));
+}
+
 static int64_t partial_floats(const recnn_dims& d, int64_t n_rows) {
-  const int in_c = d.state_dim + d.action_dim;
-  int64_t best = 0;
-  const int shapes[5][2] = {{d.hidden, in_c}, {d.hidden, d.state_dim}, {d.hidden, d.hidden},
-                            {d.action_dim, d.hidden}, {1, d.hidden}};
-  for (auto& s : shapes)
-    for (int tcp = 0; tcp < 2; ++tcp) {
-      const int64_t f = (int64_t)dw_splits(s[0], s[1], n_rows, tcp != 0) * s[0] * (s[1] + 1);
-      if (f > best) best = f;
-    }
-  const int64_t head = (int64_t)kNumSMs * (d.hidden + 2);     // block partials of the fused value-head kernel
-  // partials [splits][1][H+1] of the unfused value head's dW3 / db3: one split per 256 rows, which is not bounded by
-  // any dw_splits() above (n = 1000, H = 512: 4 splits vs dw_splits(1, 512, 1000, false) = 3)
-  const int64_t head_grad = ceil_div(n_rows, kHeadGradRowsPerSplit) * (d.hidden + 1);
-  if (head > best) best = head;
-  return head_grad > best ? head_grad : best;
+  const int H = d.hidden;
+  int64_t best = head_partial_floats(H, n_rows);
+  const int shapes[5][2] = {{H, d.state_dim + d.action_dim}, {H, d.state_dim}, {H, H}, {d.action_dim, H}, {1, H}};
+  for (auto& s : shapes) best = std::max(best, dw_partial_floats(s[0], s[1], n_rows));
+  return best;
 }
 
 static Workspace carve(const recnn_dims& d, int64_t n, void* base) {
   Workspace w;
-  char* p = static_cast<char*>(base);
-  int64_t off = 0;
-  auto take = [&](int64_t floats) {
-    float* r = base ? reinterpret_cast<float*>(p + off) : nullptr;
-    off += round_up(floats * 4, 256);
-    return r;
-  };
+  Carve c(base);
   const int ldS = pad4(d.state_dim);
   const int ldA = pad4(d.action_dim + d.state_dim % 4);
-  w.S = take(n * ldS);
-  w.S2 = take(n * ldS);
-  w.ACT = take(n * ldA);
-  w.REW = take(n);
-  for (auto& b : w.hb) b = take(n * d.hidden);
-  for (auto& b : w.ab) b = take(n * ldA);
-  w.y = take(n);
-  w.qtmp = take(n);
-  w.dq = take(n);
-  w.partial = take(partial_floats(d, n));
-  {
-    int64_t f2 = 0;
-    const int shp[2][2] = {{d.hidden, d.hidden}, {d.action_dim, d.hidden}};
-    for (auto& s2 : shp)
-      for (int tcp = 0; tcp < 2; ++tcp) {
-        const int64_t f = (int64_t)dw_splits(s2[0], s2[1], n, tcp != 0) * s2[0] * (s2[1] + 1);
-        if (f > f2) f2 = f;
-      }
-    w.partial2 = take(f2);
-  }
-  w.block_partials = take(1024);
-  w.scalars = take(8);
-  w.tickets = reinterpret_cast<unsigned*>(take(8));
-  w.bytes = off;
+  w.S = c.take(n * ldS);
+  w.S2 = c.take(n * ldS);
+  w.ACT = c.take(n * ldA);
+  w.REW = c.take(n);
+  for (auto& b : w.hb) b = c.take(n * d.hidden);
+  for (auto& b : w.ab) b = c.take(n * ldA);
+  w.y = c.take(n);
+  w.qtmp = c.take(n);
+  w.dq = c.take(n);
+  w.partial = c.take(partial_floats(d, n));
+  w.partial2 = c.take(std::max(dw_partial_floats(d.hidden, d.hidden, n), dw_partial_floats(d.action_dim, d.hidden, n)));
+  w.block_partials = c.take(1024);
+  w.scalars = c.take(8);
+  w.tickets = c.take<unsigned>(8);
+  w.bytes = c.bytes();
   return w;
 }
 
@@ -511,7 +502,7 @@ static int phase_value_grad(Ctx& c) {
       RECNN_PROPAGATE(launch_critic_head(h, c.st));
       if (!a.learn) continue;
       // layer 3: dW3 = dq^T h2, db3 = sum dq ; dz2 = (dq w3) * gate(h2)
-      const int splits = (int)ceil_div(c.n, kHeadGradRowsPerSplit);      // partial_floats() reserves splits * (H+1)
+      const int splits = (int)ceil_div(c.n, kHeadGradRowsPerSplit);      // head_partial_floats() reserves splits * (H+1)
       RECNN_PROPAGATE(launch_head_grad_partials(c.ws.dq, c2, c.n, H, kHeadGradRowsPerSplit, splits, c.ws.partial, c.st));
       RECNN_PROPAGATE(launch_reduce_partials(c.ws.partial, splits, 1, H + 1, G + c.lc.w3, c.lc.ld3, G + c.lc.b3, c.st));
       RECNN_PROPAGATE(launch_critic_head_bwd(c.ws.dq, 0.f, P + c.lc.w3, c2, c.gate, dz2, c.n, H, c.st));
@@ -707,10 +698,7 @@ static int run_step(const recnn_step_args* a, int algo, void* stream) {
   c.n = a->n_rows;
   c.st = static_cast<cudaStream_t>(stream);
   c.ws = carve(c.d, c.n, a->workspace);
-  if (c.ws.bytes > a->workspace_bytes) {
-    set_error("workspace too small: need %lld bytes, got %lld", (long long)c.ws.bytes, (long long)a->workspace_bytes);
-    return RECNN_E_WORKSPACE;
-  }
+  RECNN_PROPAGATE(check_workspace(c.ws.bytes, a->workspace_bytes));
   c.rng.masks = a->masks[0] ? a->masks : nullptr;
   c.rng.seed = a->seed;
   c.rng.step = (const long long*)a->rng_step;
@@ -832,10 +820,26 @@ extern "C" int recnn_net_layout(const recnn_dims* d, int is_critic, int64_t* out
 // Inference entry points take densely packed inputs ([n, S] / [n, A]).  A row pitch that is not a 16-byte
 // multiple (S = 1290) cannot be a TMA tensor, so the inputs are first re-pitched into scratch images (one 2-D
 // device copy each, 21 MB at 4096 rows) and every layer runs on the tensor-core path rather than the much slower CUDA-core kernel.
+struct ForwardScratch {
+  float *h1, *h2;      // [n, H] hidden layers
+  float* img;          // [n, pad4(S)] state image
+  float* aimg;         // [n, ldA] the critic's action image, `lead` zero columns in front (null: no action input)
+  int64_t floats;
+};
+static ForwardScratch forward_carve(const recnn_dims& d, int64_t n, bool action_image, void* base) {
+  ForwardScratch s;
+  Carve c(base);
+  s.h1 = c.take(n * d.hidden);
+  s.h2 = c.take(n * d.hidden);
+  s.img = c.take(n * pad4(d.state_dim));
+  s.aimg = action_image ? c.take(n * pad4(d.action_dim + d.state_dim % 4)) : nullptr;
+  s.floats = c.floats();
+  return s;
+}
+
 extern "C" int64_t recnn_forward_scratch_floats(const recnn_dims* d, int64_t n_rows, int is_critic) {
   if (!d || n_rows <= 0) return 0;
-  const int64_t ldS = pad4(d->state_dim), ldA = pad4(d->action_dim + d->state_dim % 4);
-  return 2 * n_rows * d->hidden + n_rows * ldS + (is_critic ? n_rows * ldA : 0) + 64;
+  return forward_carve(*d, n_rows, is_critic != 0, nullptr).floats;
 }
 
 // state [n, S] (row pitch ld; 0: S) -> a pitch-ldS image when needed; returns the Seg to read
@@ -863,16 +867,14 @@ extern "C" int recnn_actor_forward(const recnn_dims* d, const float* params, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const NetLayout l = actor_layout(*d);
   const int H = d->hidden;
-  float* h1 = scratch;
-  float* h2 = scratch + n_rows * H;
-  float* img = reinterpret_cast<float*>(round_up(reinterpret_cast<int64_t>(h2 + n_rows * H), 16));
+  const ForwardScratch s = forward_carve(*d, n_rows, false, scratch);
   Rng rng = {nullptr, 0, nullptr};
   const bool train = mask1 != nullptr;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, img, &xs, st));
-  const Seg s1 = {h1, H, H, 0}, s2 = {h2, H, H, 0};
-  RECNN_PROPAGATE(hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, h1, st));
-  RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, h2, st));
+  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, s.img, &xs, st));
+  const Seg s1 = {s.h1, H, H, 0}, s2 = {s.h2, H, H, 0};
+  RECNN_PROPAGATE(hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, s.h1, st));
+  RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, s.h2, st));
   return linear_out(s2, params + l.w3, l.ld3, params + l.b3, d->action_dim, n_rows, apply_tanh, nullptr, action_out,
                     d->action_dim, st);
 }
@@ -886,28 +888,25 @@ extern "C" int recnn_critic_forward(const recnn_dims* d, const float* params, co
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const NetLayout l = critic_layout(*d);
   const int H = d->hidden, S = d->state_dim, A = d->action_dim;
-  float* h1 = scratch;
-  float* h2 = scratch + n_rows * H;
-  float* img = reinterpret_cast<float*>(round_up(reinterpret_cast<int64_t>(h2 + n_rows * H), 16));
+  const ForwardScratch s = forward_carve(*d, n_rows, true, scratch);
   Rng rng = {nullptr, 0, nullptr};
   const bool train = mask1 != nullptr;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, img, &xs, st));
+  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, s.img, &xs, st));
   // the action block starts at weight column S: with S % 4 != 0 it needs `lead` zero columns in front (see Seg)
   const int lead = S % 4, ldA = pad4(A + lead);
   Seg xa = {action, A, A, 0};
   if (lead != 0 || A % 4 != 0 || !aligned16(action)) {
-    float* aimg = img + n_rows * (int64_t)pad4(S);
-    RECNN_CHECK_CUDA(cudaMemsetAsync(aimg, 0, sizeof(float) * n_rows * ldA, st));
-    RECNN_CHECK_CUDA(cudaMemcpy2DAsync(aimg + lead, (size_t)ldA * 4, action, (size_t)A * 4, (size_t)A * 4, n_rows,
+    RECNN_CHECK_CUDA(cudaMemsetAsync(s.aimg, 0, sizeof(float) * n_rows * ldA, st));
+    RECNN_CHECK_CUDA(cudaMemcpy2DAsync(s.aimg + lead, (size_t)ldA * 4, action, (size_t)A * 4, (size_t)A * 4, n_rows,
                                        cudaMemcpyDeviceToDevice, st));
-    xa = Seg{aimg, A + lead, ldA, lead};
+    xa = Seg{s.aimg, A + lead, ldA, lead};
   }
-  const Seg s1 = {h1, H, H, 0};
-  RECNN_PROPAGATE(hidden_layer(xs, xa, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, h1, st));
-  RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, h2, st));
+  const Seg s1 = {s.h1, H, H, 0};
+  RECNN_PROPAGATE(hidden_layer(xs, xa, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, s.h1, st));
+  RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, s.h2, st));
   HeadArgs h;
-  h.h2 = h2; h.w3 = params + l.w3; h.b3 = params + l.b3; h.n_rows = n_rows; h.n_rows_global = n_rows;
+  h.h2 = s.h2; h.w3 = params + l.w3; h.b3 = params + l.b3; h.n_rows = n_rows; h.n_rows_global = n_rows;
   h.hidden = H; h.mode = HEAD_PLAIN; h.reward = nullptr; h.done = nullptr; h.gamma = 0; h.min_value = 0;
   h.max_value = 0; h.y = nullptr; h.tmp = nullptr; h.out = value_out; h.dq = nullptr; h.loss = nullptr;
   h.block_partials = nullptr; h.ticket = nullptr;

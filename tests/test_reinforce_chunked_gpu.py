@@ -15,6 +15,7 @@ from recnn_b200 import _lib
 from recnn_b200.nn.arena import param_arena, grad_arena
 from recnn_b200.nn.update import reinforce as RF
 from oracle import reinforce_oracle as RO
+from tests._discrete import make_policy
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -22,16 +23,6 @@ METHODS = ["basic_reinforce", "reinforce_with_correction", "reinforce_with_TopK_
 # chunked vs single chunk: both are fp32 with 3xTF32 contractions; only the order of the softmax sum (merged per
 # chunk), the split-K order of dW2 (per chunk width) and of dh (accumulated chunk by chunk) differ
 REORDER_BAR = 1e-5
-
-
-def make_policy(p, S, H, I):
-    m = recnn_b200.nn.DiscreteActor(S, I, H)
-    with torch.no_grad():
-        m.linear1.weight.copy_(torch.from_numpy(p["w1"]))
-        m.linear1.bias.copy_(torch.from_numpy(p["b1"]))
-        m.linear2.weight.copy_(torch.from_numpy(p["w2"]))
-        m.linear2.bias.copy_(torch.from_numpy(p["b2"]))
-    return m.to(DEV)
 
 
 def unpack(g, m):
