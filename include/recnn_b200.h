@@ -561,6 +561,32 @@ RECNN_API int64_t recnn_offsetof_beta_args(int field);
  * running max / sum, then dZ of each chunk from probs_out and that chunk's rows of dW / db.  Deterministic. */
 RECNN_API int recnn_beta_step(const recnn_beta_args* args, void* stream);
 
+/* ---- REINFORCE with Top-K correction: beta sharded over the item vocabulary, with the policy ------
+ * Rank `rank` of `world` holds rows [lo, hi) of net.0.weight / net.0.bias, lo = v->item_offset and hi = lo +
+ * args->dims.num_items (recnn_vocab_shard above, the policy's plan): args carries the LOCAL dims, so the arena is laid
+ * out as a Beta(S, hi - lo) and args->probs_out is the rank's column block [n_rows, hi - lo].  Target ids stay global.
+ * One call of recnn_beta_step becomes three phases on one stream with two exchanges (recnn_comm_allgather) between them:
+ *   begin -> record (recnn_vocab_record_floats(n_rows): header {lo, hi, num_items, n_rows}, the local max and sum of
+ *            exp of the block's logits, the target's logit from the rank that holds it, 0 elsewhere) -> all-gather
+ *   rows  -> merges the gathered records in rank order, turns the block into its column block of p over the whole
+ *            vocabulary, and writes a second record of the same size: the same header, then the block's per-row sums
+ *            of expm1(p) and of p expm1(p) and a zero plane -> all-gather
+ *   end   -> T = num_items + the rank-order sum of the first planes, U likewise, p_a, the loss, dW / db of the local rows
+ *            (overwriting net.grads) and the built-in optimizer over the local arena (RECNN_OPT_EXTERNAL: stop after
+ *            the gradient).
+ * No all-reduce: the loss, T, U and p_a are the same bits on every rank.  The phases share args->workspace
+ * (recnn_beta_workspace_bytes of the local dims: it does not grow with the vocabulary once chunk_items < hi - lo), which
+ * must be left untouched between them; no allocation, no synchronisation.  At world 1 the three phases compute exactly
+ * what recnn_beta_step does.  *error bits (written by end): 1 as for the step (an id outside [0, v->num_items), seen on
+ * every rank); 2: a gathered record's header does not tile the vocabulary in rank order with this rank's block, or
+ * the ranks disagree on n_rows.  With either bit set the built-in optimizer step is skipped (t included). */
+RECNN_API int recnn_beta_shard_begin(const recnn_beta_args* args, const recnn_vocab_shard* v, float* record,
+                                     void* stream);
+RECNN_API int recnn_beta_shard_rows(const recnn_beta_args* args, const recnn_vocab_shard* v, const float* gathered,
+                                    float* record, void* stream);
+RECNN_API int recnn_beta_shard_end(const recnn_beta_args* args, const recnn_vocab_shard* v, const float* gathered,
+                                   void* stream);
+
 /* ---- data parallel: all-reduce over NVLink peer memory ------------------------------------------
  * BASELINE north_star: "partition the embedding gather + update across the 8 GPUs of one box with
  * an allreduce of the Actor/Critic gradients over NVLink".  The reference itself is single-process

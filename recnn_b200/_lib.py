@@ -195,6 +195,10 @@ SIGNATURES = {
     "recnn_sizeof_beta_args": (C.c_int64, []),
     "recnn_offsetof_beta_args": (C.c_int64, [C.c_int]),
     "recnn_beta_step": (C.c_int, [C.POINTER(BetaArgs), C.c_void_p]),
+    "recnn_beta_shard_begin": (C.c_int, [C.POINTER(BetaArgs), C.POINTER(VocabShard), C.c_void_p, C.c_void_p]),
+    "recnn_beta_shard_rows": (C.c_int, [C.POINTER(BetaArgs), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
+    "recnn_beta_shard_end": (C.c_int, [C.POINTER(BetaArgs), C.POINTER(VocabShard), C.c_void_p, C.c_void_p]),
     "recnn_comm_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]),
     "recnn_comm_handle_bytes": (C.c_int32, []),
     "recnn_comm_local_handle": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -843,18 +843,21 @@ extern "C" int64_t recnn_forward_scratch_floats(const recnn_dims* d, int64_t n_r
 }
 
 // state [n, S] (row pitch ld; 0: S) -> a pitch-ldS image when needed; returns the Seg to read
+// The operand repitch_state gives for a state [n, S] of row pitch ld (0: S): the state itself when it is TMA-legal,
+// else img [n, pad4(S)] (which repitch_state fills).  A later phase of the same call recovers it without a copy.
+static Seg state_seg(int S, const float* state, long long ld, float* img) {
+  if (ld == 0) ld = S;
+  if (S % 4 == 0 && ld % 4 == 0 && aligned16(state)) return Seg{state, S, ld, 0};
+  return Seg{img, S, pad4(S), 0};
+}
+
 static int repitch_state(const recnn_dims& d, const float* state, int64_t n, float* img, Seg* out, cudaStream_t st,
                          long long ld = 0) {
   const int S = d.state_dim;
-  if (ld == 0) ld = S;
-  if (S % 4 == 0 && ld % 4 == 0 && aligned16(state)) {
-    *out = Seg{state, S, ld, 0};
-    return RECNN_OK;
-  }
-  const int ldS = pad4(S);
-  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(img, (size_t)ldS * 4, state, (size_t)ld * 4, (size_t)S * 4, n,
+  *out = state_seg(S, state, ld, img);
+  if (out->p == state) return RECNN_OK;
+  RECNN_CHECK_CUDA(cudaMemcpy2DAsync(img, (size_t)out->ld * 4, state, (size_t)(ld == 0 ? S : ld) * 4, (size_t)S * 4, n,
                                      cudaMemcpyDeviceToDevice, st));
-  *out = Seg{img, S, ldS, 0};
   return RECNN_OK;
 }
 

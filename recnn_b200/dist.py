@@ -230,6 +230,17 @@ def _critic_shape_error(name, net, S, num_items):
     return None
 
 
+def _optimizer_state_error(key, opt):
+    """Why ``opt`` cannot be carried to the local arenas, or None: its moments would have the unsharded shapes."""
+    from . import optim as _optim
+    if isinstance(opt, _optim._ArenaOptimizer):
+        if opt._t is not None:
+            return "%s has already stepped; enable vocabulary parallelism before the first update" % key
+    elif len(getattr(opt, "state", {})) != 0:
+        return "%s already holds state; enable vocabulary parallelism before the first update" % key
+    return None
+
+
 def _rebuild_optimizers(optimizers, nets):
     """The agent's optimizers on the local arenas: built-in arena optimizers are rebuilt with the same hyperparameters
     (their state arenas take the local geometry); torch optimizers keep their Parameter objects, which now hold the
@@ -239,22 +250,53 @@ def _rebuild_optimizers(optimizers, nets):
     for key, opt in list(optimizers.items()):
         if opt is None:
             continue
+        err = _optimizer_state_error("optimizers[%r]" % key, opt)
+        if err:
+            raise RuntimeError(err)
         if isinstance(opt, _optim._ArenaOptimizer):
-            if opt._t is not None:
-                raise RuntimeError("optimizers[%r] has already stepped; enable vocabulary parallelism before the "
-                                   "first update" % key)
             group = opt.param_groups[0]
             net = nets.get(owner.get(id(group["params"][0])))
             fresh = type(opt)(group["params"], **{k: group[k] for k in opt.defaults})
             if net is not None:
                 fresh.bind(net)
             optimizers[key] = fresh
-        elif len(getattr(opt, "state", {})) != 0:
-            raise RuntimeError("optimizers[%r] already holds state; enable vocabulary parallelism before the first "
-                               "update" % key)
 
 
-def enable_vocab_parallel(policy_or_agent, group=None):
+def _beta_refusal(beta, S, num_items):
+    """Why ``beta`` cannot be sharded with a policy of state_dim S over num_items items, or None (checked on every rank
+    before any exchange)."""
+    from .nn.arena import _is_beta
+    if not _is_beta(beta):
+        return TypeError("beta must be a recnn_b200.nn.Beta (got %s)" % type(beta).__name__)
+    if "_recnn_vp" in beta.__dict__:
+        return RuntimeError("beta is already vocabulary-parallel")
+    lin = beta.net[0]
+    if (lin.in_features, lin.out_features) != (S, num_items):
+        return ValueError("beta must be a Beta(%d, %d) (state_dim and num_items of the policy) to be sharded with it; "
+                          "got Beta(%d, %d)" % (S, num_items, lin.in_features, lin.out_features))
+    err = _optimizer_state_error("beta.optim", beta.optim)
+    return None if err is None else RuntimeError(err)
+
+
+def _shard_beta_rows(beta, lo, hi):
+    """Keep rows [lo, hi) of net.0 (weight and bias) and rebuild the built-in optimizer on the local arenas."""
+    from . import optim as _optim
+    from .nn.arena import grad_arena
+    lin = beta.net[0]
+    with torch.no_grad():
+        for p in (lin.weight, lin.bias):
+            p.grad = None
+            p.data = p.data[lo:hi].clone()
+    lin.out_features = hi - lo
+    beta._workspace = None
+    grad_arena(beta)
+    opt = beta.optim
+    if isinstance(opt, _optim._ArenaOptimizer):
+        # not bound: the Beta holds its optimizer (see Beta.forward)
+        beta.optim = type(opt)(opt.param_groups[0]["params"], **{k: opt.param_groups[0][k] for k in opt.defaults})
+
+
+def enable_vocab_parallel(policy_or_agent, group=None, beta=None):
     """Shard a DiscreteActor's item layer -- or a whole REINFORCE agent -- over the ranks of ``group``.  Call it on
     every rank after the nets are on their CUDA device.  The weights are first made identical to rank 0's.  At world 1
     everything computes exactly what it did unsharded.
@@ -273,6 +315,13 @@ def enable_vocab_parallel(policy_or_agent, group=None):
     afterwards).  ``value_update`` / ``reinforce_update`` / ``Reinforce.update()`` then run vocabulary-parallel on
     item-id batch actions (recnn_discrete_value_shard_* in include/recnn_b200.h); a dense [N, num_items] action is
     refused.  ``debug["next_action"]`` (learn=False) is the rank's column block.
+
+    ``beta``: the Top-K notebook's behaviour policy (an ``nn.Beta`` of the policy's state_dim and num_items, on its
+    device, whose optimizer has not stepped), sharded in the same call over the policy's plan and sharing its
+    ``VocabParallel``.  Rank r keeps rows [lo, hi) of ``net.0`` (its ``state_dict`` holds the local block) and its
+    built-in RAdam is rebuilt on the local arenas with the same hyperparameters.  ``beta(state, action)`` then returns
+    the rank's column block [N, hi - lo] of the probabilities (recnn_beta_shard_* in include/recnn_b200.h), and
+    ``DiscreteActor.pi_beta_sample`` draws from that block over the whole vocabulary.
 
     Every rank must be fed the same batches and states, seeded the same (torch.manual_seed, or the same
     ``uniform_source``) and must make the same calls in the same order: dropout masks -- given in the batch or drawn --
@@ -309,6 +358,10 @@ def enable_vocab_parallel(policy_or_agent, group=None):
                 raise ValueError(err)
         if nets["target_value_net"].linear1.weight.shape != nets["value_net"].linear1.weight.shape:
             raise ValueError("nets['target_value_net'] and nets['value_net'] differ in shape")
+    if beta is not None:
+        err = _beta_refusal(beta, S, num_items)
+        if err is not None:
+            raise err
     arena = param_arena(policy)
     if not arena.is_cuda:
         raise _lib.RecnnError("enable_vocab_parallel needs the policy on its CUDA device")
@@ -317,11 +370,15 @@ def enable_vocab_parallel(policy_or_agent, group=None):
             if param_arena(net).device != arena.device:
                 raise _lib.RecnnError("nets[%r] is on %s, the policy on %s" % (name, param_arena(net).device,
                                                                                arena.device))
+    if beta is not None and param_arena(beta).device != arena.device:
+        raise ValueError("beta is on %s, the policy on %s" % (param_arena(beta).device, arena.device))
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     # every rank checks every rank's plan, so a refused plan raises on all of them (none is left in a collective)
     shape = (S, policy.linear1.out_features, num_items)
     if nets is not None:
         shape += (tuple(nets["value_net"].linear1.weight.shape),)
+    if beta is not None:
+        shape += (("beta",) + tuple(beta.net[0].weight.shape),)
     sizes = [None] * world
     dist.all_gather_object(sizes, shape, group=group)
     if len(set(sizes)) != 1:
@@ -339,6 +396,12 @@ def enable_vocab_parallel(policy_or_agent, group=None):
     vp = VocabParallel(lo, hi, num_items, group, rank, world, comm)
     for net in shard_nets.values():
         net.__dict__["_recnn_vp"] = vp
+    if beta is not None:
+        from .nn import beta as _beta
+        dist.broadcast(param_arena(beta), src=0, group=group)
+        _shard_beta_rows(beta, lo, hi)
+        beta.__dict__["_recnn_vp"] = vp
+        _beta._SHARDED.add(beta)
     if agent is not None and getattr(agent, "optimizers", None):
         _rebuild_optimizers(agent.optimizers, nets)
     return policy_or_agent

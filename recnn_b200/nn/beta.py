@@ -7,8 +7,14 @@ Correction/3. TopK Reinforce Off Policy Correction.ipynb, cell 3) and passes ``b
 probabilities from before the step -- and runs the whole call as one device step (recnn_beta_step): the items are
 visited in chunks, so besides the dense output nothing of size [N, num_items] is allocated, and the optimizer is the
 built-in RAdam (torch_optimizer is not installable next to the notebook's code here).
+
+``recnn_b200.dist.enable_vocab_parallel(policy_or_agent, beta=beta_net)`` shards a Beta over the item vocabulary with
+the policy: each rank keeps rows [lo, hi) of ``net.0`` and ``forward`` returns the rank's column block [N, hi - lo] of
+the probabilities (recnn_beta_shard_* in include/recnn_b200.h).
 """
 from __future__ import annotations
+
+import weakref
 
 import torch
 import torch.nn as nn
@@ -20,6 +26,20 @@ from .update import _ids
 from .update.reinforce import _chunk_items
 
 
+# The sharded Betas, held weakly: block_records() finds the one that returned a given block.
+_SHARDED = weakref.WeakSet()
+
+
+def block_records(t):
+    """(gathered records of exchange 1, VocabParallel) of the column block ``t`` a sharded Beta's last call returned,
+    or None (``t`` is not such a block: a replicated Beta's output, a copy, or an older block)."""
+    for beta in list(_SHARDED):
+        held = beta.__dict__.get("_recnn_block")
+        if held is not None and held[0]() is t:
+            return held[1], beta.__dict__["_recnn_vp"]
+    return None
+
+
 class Beta(nn.Module):
     """``Beta(input_dim, num_items)``: the notebook's cell 3 with its hard-wired 1290 and ``num_items`` as arguments.
 
@@ -27,7 +47,12 @@ class Beta(nn.Module):
     softmax), and ``action`` is a one-hot [N, num_items] float matrix whose ``argmax(1)`` is the target.  Item ids
     (an integer tensor [N], as ``batch_contstate_discaction(..., one_hot=False)`` gives) are accepted too.  The loss
     of the last call stays on the device in ``last_loss``.  Replacing ``optim`` by a torch optimizer makes the call
-    stop after the gradient (left in ``.grad``) and call its ``step()``."""
+    stop after the gradient (left in ``.grad``) and call its ``step()``.
+
+    Sharded over the item vocabulary (``recnn_b200.dist.enable_vocab_parallel(..., beta=)``), a call returns the rank's
+    column block [N, hi - lo] of the probabilities; ``action`` stays a one-hot [N, num_items] row or global item ids, and
+    ``last_loss`` is the loss over the whole vocabulary, the same on every rank.  Every rank must make the same calls
+    with the same states and actions."""
 
     _recnn_beta = True
 
@@ -64,7 +89,9 @@ class Beta(nn.Module):
         if state.dim() != 2 or state.shape[1] != d.state_dim:
             raise ValueError("state must be [N, %d] (got shape %s)" % (d.state_dim, tuple(state.shape)))
         n = int(state.shape[0])
-        target = self._targets(action, n, d.num_items)
+        vp = self.__dict__.get("_recnn_vp")
+        self.__dict__.pop("_recnn_block", None)
+        target = self._targets(action, n, d.num_items if vp is None else vp.num_items)
         dev = self.net[0].weight.device
         if dev.type != "cuda":
             raise _lib.RecnnError("recnn_b200 nets run on CUDA only (Beta is on %s); call .cuda() first" % dev)
@@ -104,11 +131,33 @@ class Beta(nn.Module):
                 self._workspace = None
                 self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             a.workspace, a.workspace_bytes = self._workspace.data_ptr(), self._workspace.numel()
-            _lib.check(L.recnn_beta_step(a, _lib.stream_ptr(dev)))
+            if vp is None:
+                _lib.check(L.recnn_beta_step(a, _lib.stream_ptr(dev)))
+            else:
+                gathered = self._sharded_step(a, vp, n, dev)
             self.last_loss = loss
-            if int(error.item()) != 0:         # the call's one synchronisation
+            err = int(error.item())            # the call's one synchronisation
+            if err & 2:
+                raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows: no "
+                                   "optimizer step was taken")
+            if err != 0:
                 raise IndexError("action holds an item id outside [0, num_items): no optimizer step was taken")
             if not builtin:
                 grad_arena(self)               # re-attach p.grad views if zero_grad(set_to_none) dropped them
                 opt.step()
+        if vp is not None:
+            self.__dict__["_recnn_block"] = (weakref.ref(probs), gathered)
         return probs
+
+    def _sharded_step(self, a, vp, n, dev):
+        """begin -> all-gather -> rows -> all-gather -> end; returns the gathered records of the first exchange."""
+        L = _lib.lib()
+        shard = vp.shard()
+        st = _lib.stream_ptr(dev)
+        rec = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+        _lib.check(L.recnn_beta_shard_begin(a, shard, rec.data_ptr(), st))
+        gathered = vp.all_gather(rec)
+        sums = torch.empty_like(rec)
+        _lib.check(L.recnn_beta_shard_rows(a, shard, gathered.data_ptr(), sums.data_ptr(), st))
+        _lib.check(L.recnn_beta_shard_end(a, shard, vp.all_gather(sums).data_ptr(), st))
+        return gathered

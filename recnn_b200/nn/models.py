@@ -265,14 +265,43 @@ class DiscreteActor(nn.Module):
         self._saved.append({"state": state.clone(), "action": pi_action, "beta_log_prob": None})
         return pi_probs
 
+    def _beta_records(self, beta_out):
+        """The gathered records of a sharded Beta's column block ``beta_out`` (None for full probabilities); refuses
+        a beta output this policy cannot draw from."""
+        from .beta import block_records
+        vp = self.__dict__.get("_recnn_vp")
+        found = block_records(beta_out)
+        if found is not None:
+            if vp is None:
+                raise ValueError("beta returned the column block of a vocabulary-parallel Beta, but the policy is not "
+                                 "vocabulary-parallel: shard both with enable_vocab_parallel(..., beta=)")
+            bvp = found[1]
+            if (bvp.lo, bvp.hi, bvp.num_items, bvp.rank, bvp.world) != (vp.lo, vp.hi, vp.num_items, vp.rank, vp.world):
+                raise ValueError("beta is sharded on items [%d, %d) of %d, the policy on [%d, %d) of %d: shard them in "
+                                 "one enable_vocab_parallel(..., beta=) call"
+                                 % (bvp.lo, bvp.hi, bvp.num_items, vp.lo, vp.hi, vp.num_items))
+            return found[0]
+        if vp is not None and (beta_out.dim() != 2 or beta_out.shape[1] != vp.num_items):
+            block = beta_out.dim() == 2 and beta_out.shape[1] == vp.hi - vp.lo
+            raise ValueError("beta must return probabilities [N, %d] or the column block of a Beta sharded with the "
+                             "policy (got shape %s)%s"
+                             % (vp.num_items, tuple(beta_out.shape),
+                                ": a column block without its records (a copy, or not the Beta's latest output)"
+                                if block else ""))
+        return None
+
     def pi_beta_sample(self, state, beta, action, **kwargs):
-        """models.py:113-145.  ``beta`` is any callable (state, action=...) -> probabilities [N, action_dim]."""
+        """models.py:113-145.  ``beta`` is any callable (state, action=...) -> probabilities [N, action_dim]; on a
+        vocabulary-parallel policy also the rank's column block a Beta sharded with it returned (its latest output,
+        as returned: the block's draw needs the records of the Beta's call)."""
         dev, (state,) = _device_check(self, state)
-        beta_probs = self._as_probs(beta(state.detach(), action=action), dev)
+        beta_out = beta(state.detach(), action=action)
+        beta_gathered = self._beta_records(beta_out) if torch.is_tensor(beta_out) else None
+        beta_probs = self._as_probs(beta_out, dev)
         pi_probs, gathered = self._pi(state)
         # the pi draw is made first, then the beta draw (models.py:133-136)
         pi_draw = self._sample(pi_probs, gathered)
-        beta_draw = self._sample(beta_probs)
+        beta_draw = self._sample(beta_probs, beta_gathered)
         available = {"pi": (pi_draw, pi_probs), "beta": (beta_draw, beta_probs)}
         (pi_action, pi_lp), src_pi = available[self.action_source["pi"]]
         (beta_action, beta_lp), src_beta = available[self.action_source["beta"]]
@@ -282,7 +311,12 @@ class DiscreteActor(nn.Module):
             pi_log_prob = self._log_prob(pi_probs, pi_action)
         else:
             pi_log_prob = self._shard_log_prob(pi_probs, pi_action)
-        beta_log_prob = beta_lp if src_beta is beta_probs else self._log_prob(beta_probs, beta_action)
+        if src_beta is beta_probs:
+            beta_log_prob = beta_lp
+        elif beta_gathered is None:
+            beta_log_prob = self._log_prob(beta_probs, beta_action)
+        else:
+            beta_log_prob = self._shard_log_prob(beta_probs, beta_action)
         self._last_sample = {"state": state, "action": pi_action, "beta_log_prob": beta_log_prob}
         return pi_log_prob, beta_log_prob, pi_probs
 
