@@ -437,6 +437,45 @@ RECNN_API int recnn_discrete_shard_log_prob(const recnn_discrete_dims* d, const 
 RECNN_API int recnn_discrete_shard_pick(int32_t world, const float* gathered_draws, int64_t n_rows,
                                         int64_t* action_out, float* log_prob_out, int32_t* error_flag, void* stream);
 
+/* ---- REINFORCE: serving the policy's top-k items ---------------------------------------------------
+ * torch.topk(DiscreteActor(state), k) without the [n_rows, num_items] probabilities: the hidden layer once, then the
+ * items in chunks of chunk_items (num_items, or a positive multiple of 128 below it; the last chunk may be narrower).
+ * Each chunk's logits fold into the row's running max and sum of exp (the reduction of recnn_discrete_forward) and its
+ * best candidates merge into a running list of k per row.  Items are ranked by logit, equal logits to the smaller id;
+ * values_out fp32 [n_rows, k] = exp(z - M) / S over ALL items (M, S: the row's max and sum of exp), descending;
+ * ids_out int64 [n_rows, k].  With one chunk the values equal recnn_discrete_forward's probabilities bit for bit.
+ * exclude: NULL or int64 [n_rows, n_exclude] (n_exclude <= 256); those ids are never returned but stay in S (the
+ * values are pi's, not renormalised); negative ids are padding.  When a row has fewer than k eligible items the last
+ * slots are id -1, value 0.  *error_flag <- bits: 1 = an excluded id is >= num_items.  1 <= k <= min(64, num_items).
+ * workspace: any address, workspace_bytes >= recnn_discrete_topk_workspace_bytes (else RECNN_E_WORKSPACE); it holds
+ * one [n_rows, chunk_items] logits block and a few [n_rows, k] lists, so it does not grow with num_items once
+ * chunk_items < num_items.  Deterministic: fixed chunk order, no atomics on the results. */
+RECNN_API int64_t recnn_discrete_topk_workspace_bytes(const recnn_discrete_dims* d, int64_t n_rows, int32_t k,
+                                                      int32_t chunk_items);   /* 0 when k is outside [1, 64] or chunk_items is refused */
+RECNN_API int recnn_discrete_topk(const recnn_discrete_dims* d, const float* params, const float* state,
+                                  int64_t n_rows, int32_t k, const int64_t* exclude, int32_t n_exclude,
+                                  int32_t chunk_items, float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                  void* workspace, int64_t workspace_bytes, void* stream);
+/* The same on a vocabulary-sharded policy (d: the LOCAL dims; k <= the whole vocabulary, and may exceed the rank's
+ * block).  shard_topk runs the passes over the rank's items [lo, hi) with global candidate ids and writes a record of
+ * recnn_vocab_topk_record_floats(n_rows, k) floats: the header {lo, hi, num_items, n_rows}, the local max and sum-of-exp
+ * planes, then k logit planes and k id planes (int32 bits), plane j holding every row's j-th best local candidate (a
+ * block of fewer than k eligible items pads with logit -FLT_MAX, id -1).  workspace as recnn_discrete_topk with the
+ * local dims.  After recnn_comm_allgather of the records (rank order), shard_topk_finish merges M and S in rank order as
+ * recnn_discrete_shard_finish does and k-way merges the W lists (world <= 32): every rank writes the same bits, and at
+ * world 1 the pair computes exactly what recnn_discrete_topk does.  *error_flag <- bits: 1 = an excluded id is >=
+ * num_items; 2 = the headers do not tile the vocabulary in rank order with this rank's block (the result is then
+ * meaningless). */
+RECNN_API int64_t recnn_vocab_topk_record_floats(int64_t n_rows, int32_t k);
+RECNN_API int recnn_discrete_shard_topk(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                        const float* state, int64_t n_rows, int32_t k, const int64_t* exclude,
+                                        int32_t n_exclude, int32_t chunk_items, float* record, void* workspace,
+                                        int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                               const float* gathered, int64_t n_rows, int32_t k,
+                                               const int64_t* exclude, int32_t n_exclude, float* values_out,
+                                               int64_t* ids_out, int32_t* error_flag, void* stream);
+
 /* ---- REINFORCE: the critic side with item-id actions ---------------------------------------------
  * The REINFORCE critic is a Critic(S, num_items, H) (recnn/nn/update/reinforce.py:92-102): layer 1 is W1 [H, S + num_items]
  * on [state | action], the action being a one-hot row (the batch) or a probability row (the target policy's output).

@@ -173,6 +173,17 @@ SIGNATURES = {
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_discrete_shard_pick": (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p]),
+    "recnn_discrete_topk_workspace_bytes": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32, C.c_int32]),
+    "recnn_discrete_topk": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                      C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int64, C.c_void_p]),
+    "recnn_vocab_topk_record_floats": (C.c_int64, [C.c_int64, C.c_int32]),
+    "recnn_discrete_shard_topk": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                            C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                            C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_discrete_shard_topk_finish": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                   C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_critic_action_term_scratch_floats": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                             C.c_int32]),
     "recnn_critic_action_term_chunked": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.POINTER(DiscreteDims), C.c_void_p,

@@ -326,24 +326,32 @@ __global__ void shard_record_init_kernel(float* __restrict__ rec, long long n, i
   }
 }
 
-// the rank-order merge of row r: M = max m_q, S = sum s_q exp(m_q - M), za = sum za_q
-__device__ __forceinline__ void shard_merge_row(const float* __restrict__ g, int W, long long n, long long r, float& M,
-                                                float& S, float& za) {
-  const long long stride = shard_record_floats(n);
+// the rank-order merge of row r's statistics from W records of `stride` floats that start with the header and the
+// m and s planes: M = max m_q, S = sum s_q exp(m_q - M)
+__device__ __forceinline__ void shard_merge_stats(const float* __restrict__ g, long long stride, int W, long long n,
+                                                  long long r, float& M, float& S) {
   M = -INFINITY;
   for (int q = 0; q < W; ++q) M = fmaxf(M, g[q * stride + kShardHeader + r]);
   S = 0.f;
-  za = 0.f;
   for (int q = 0; q < W; ++q) {
     const float* rec = g + q * stride + kShardHeader;
     S += rec[n + r] * expf(rec[r] - M);
-    za += rec[2 * n + r];
   }
 }
 
-// true unless the W headers tile [0, items) in rank order, every rank saw n rows and this rank's entry is [lo, hi)
-__device__ bool shard_plan_bad(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items) {
+// the rank-order merge of row r: M and S as above, za = sum za_q
+__device__ __forceinline__ void shard_merge_row(const float* __restrict__ g, int W, long long n, long long r, float& M,
+                                                float& S, float& za) {
   const long long stride = shard_record_floats(n);
+  shard_merge_stats(g, stride, W, n, r, M, S);
+  za = 0.f;
+  for (int q = 0; q < W; ++q) za += g[q * stride + kShardHeader + 2 * n + r];
+}
+
+// true unless the W headers (records of `stride` floats) tile [0, items) in rank order, every rank saw n rows and this
+// rank's entry is [lo, hi)
+__device__ bool shard_plan_bad_at(const float* __restrict__ g, long long stride, int W, long long n, int rank, int lo,
+                                  int hi, int items) {
   int expect = 0;
   bool bad = false;
   for (int q = 0; q < W; ++q) {
@@ -353,6 +361,9 @@ __device__ bool shard_plan_bad(const float* __restrict__ g, int W, long long n, 
     if (q == rank) bad = bad || h[0] != lo || h[1] != hi;
   }
   return bad || expect != items;
+}
+__device__ bool shard_plan_bad(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items) {
+  return shard_plan_bad_at(g, shard_record_floats(n), W, n, rank, lo, hi, items);
 }
 
 // gathered records -> the merged statistics of every row (into the scratch the unsharded path uses); *plan_bad
@@ -582,6 +593,237 @@ static int reinforce_grad_pass(const recnn_discrete_dims& d, const float* params
                                     c != n_chunks - 1));
   }
   return weight_grad(s.dh, H, xs, kNoSeg, n, grads + l.w1, l.ld1, grads + l.b1, s.partial, st);
+}
+
+
+// ---- The policy's top-k (serving): the k best items of every row by logit, with pi of each, never forming the
+// [n, num_items] probabilities.  The items are visited in chunks as in pass 1 of the policy gradient: each chunk's
+// logits fold into (run_max, run_sum) through logit_stats_kernel, and its best k candidates merge into a running list
+// of k (key = -logit, global id) per row, sorted best first (ties: smaller id).  Finish: pi = exp(z - M) / S, the
+// expression of softmax_rows_kernel.
+constexpr int kMaxExclude = 256;
+constexpr int kTopkSplitCap = 31;     // the running list takes lane 0 of the merge warp
+
+// -logit, with NaN and -inf logits ranked after every finite one (and still before an empty slot, by id)
+__device__ __forceinline__ float logit_key(float z) { return fminf(-z, FLT_MAX); }
+
+__global__ void cand_fill_kernel(Cand* __restrict__ c, long long count) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < count) c[i] = Cand{FLT_MAX, kNoId};
+}
+
+// grid (splits, rows): the best k of columns [lo, hi) of one row of a chunk's logits z [n, w] (ids id0 + j) that beat
+// the row's running k-th best, ascending, into part [n, splits, k] (empty slots: {FLT_MAX, kNoId}).  A candidate is
+// checked against the row's excluded ids only once it beats its thread's list and the running k-th.
+template <int KMAX>
+__global__ void __launch_bounds__(kTopkThreads)
+policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int id0, int k,
+                          const long long* __restrict__ exclude, int n_ex, const Cand* __restrict__ run,
+                          Cand* __restrict__ part) {
+  __shared__ float s_key[32];
+  __shared__ int s_id[32], s_owner[32];
+  __shared__ int s_ex[kMaxExclude];
+  const int sp = blockIdx.x, splits = gridDim.x;
+  const int per = (w + splits - 1) / splits;
+  const int lo = sp * per, hi = min(w, lo + per);
+  for (long long r = blockIdx.y; r < n; r += gridDim.y) {
+    for (int e = threadIdx.x; e < n_ex; e += blockDim.x) {
+      const long long x = exclude[r * n_ex + e];
+      s_ex[e] = (x >= 0 && x < kNoId) ? (int)x : -1;       // padding and out-of-range ids match no item
+    }
+    __syncthreads();
+    const Cand bar = run[r * k + k - 1];
+    float keys[KMAX];
+    int ids[KMAX];
+    list_clear(keys, ids);
+    const float* row = z + r * w;
+    for (int j = lo + threadIdx.x; j < hi; j += blockDim.x) {
+      const float key = logit_key(row[j]);
+      const int id = id0 + j;
+      if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && better(key, id, bar.key, bar.id)) {
+        bool ex = false;
+        for (int e = 0; e < n_ex; ++e) ex |= s_ex[e] == id;
+        if (!ex) list_insert(keys, ids, key, id);
+      }
+    }
+    // merge the CTA's sorted lists: rounds of arg-min over the heads, until k or every list is empty
+    Cand* out = part + (r * splits + sp) * k;
+    int head = 0, i = 0;
+    for (; i < k; ++i) {
+      float hk, wk;
+      int hid, wi, wo;
+      list_at(keys, ids, head, hk, hid);
+      block_argmin(hk, hid, s_key, s_id, s_owner, wk, wi, wo);
+      if (wi == kNoId) break;                               // the same decision in every thread
+      if ((int)threadIdx.x == wo) ++head;
+      if (threadIdx.x == 0) out[i] = Cand{wk, wi};
+    }
+    for (int j = i + threadIdx.x; j < k; j += blockDim.x) out[j] = Cand{FLT_MAX, kNoId};
+    __syncthreads();                                        // s_ex is refilled for the next row
+  }
+}
+
+// one warp per row: run_out = the best k of run_in and the row's `splits` partial lists (all sorted)
+__global__ void __launch_bounds__(128)
+policy_topk_merge_kernel(const Cand* __restrict__ run_in, const Cand* __restrict__ part, int splits, int k, long long n,
+                         Cand* __restrict__ run_out) {
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const Cand* mine = lane == 0 ? run_in + r * k : part + (r * splits + lane - 1) * k;
+  const bool has = lane <= splits;
+  int head = 0;
+  for (int i = 0; i < k; ++i) {
+    float key = FLT_MAX;
+    int id = kNoId, owner = lane;
+    if (has && head < k) {
+      const Cand c = mine[head];
+      key = c.key;
+      id = c.id;
+    }
+    warp_argmin(key, id, owner);
+    if (lane == owner) ++head;
+    if (lane == 0) run_out[r * k + i] = Cand{key, id};
+  }
+}
+
+// ids (-1 for an empty slot) and pi = exp(z - M) / S of the final lists
+__global__ void policy_topk_finish_kernel(const Cand* __restrict__ run, long long n, int k,
+                                          const float* __restrict__ run_max, const float* __restrict__ run_sum,
+                                          float* __restrict__ values, long long* __restrict__ ids) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n * k) return;
+  const long long r = i / k;
+  const Cand c = run[i];
+  const bool none = c.id == kNoId;
+  ids[i] = none ? -1 : c.id;
+  values[i] = none ? 0.f : expf(-c.key - run_max[r]) / run_sum[r];
+}
+
+// *flag |= 1 when an excluded id is >= items (negative ids are padding)
+__global__ void exclude_check_kernel(const long long* __restrict__ exclude, long long count, long long items,
+                                     int* flag) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < count && exclude[i] >= items) atomicOr(flag, 1);
+}
+
+// A rank's top-k record: the header {lo, hi, num_items, n_rows}, the m and s planes (written by the passes), then k
+// logit planes and k id planes (int32 bits; an empty slot is logit -FLT_MAX, id -1), plane j holding every row's j-th.
+__host__ __device__ __forceinline__ int64_t topk_record_floats(int64_t n, int k) {
+  return kShardHeader + (2 + 2 * (int64_t)k) * n;
+}
+
+__global__ void policy_topk_record_kernel(const Cand* __restrict__ run, long long n, int k, int lo, int hi, int items,
+                                          float* __restrict__ rec) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) {
+    int* h = reinterpret_cast<int*>(rec);
+    h[0] = lo; h[1] = hi; h[2] = items; h[3] = (int)n;
+  }
+  if (i >= n * k) return;
+  const long long r = i / k, j = i % k;
+  const Cand c = run[i];
+  float* planes = rec + kShardHeader + 2 * n;
+  planes[j * n + r] = -c.key;
+  planes[(k + j) * n + r] = __int_as_float(c.id == kNoId ? -1 : c.id);
+}
+
+// gathered top-k records -> every rank's (values, ids): M and S merged in rank order (shard_merge_stats), then a k-way
+// merge of the W sorted lists.  One warp per row, lane q reads rank q's list (W <= 32).  *flag |= 2 when the headers do
+// not tile the vocabulary with this rank's block.
+__global__ void __launch_bounds__(128)
+policy_topk_shard_finish_kernel(const float* __restrict__ g, int W, long long n, int k, int rank, int lo, int hi,
+                                int items, float* __restrict__ values, long long* __restrict__ ids, int* flag) {
+  const long long stride = topk_record_floats(n, k);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad_at(g, stride, W, n, rank, lo, hi, items)) atomicOr(flag, 2);
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  float M, S;
+  shard_merge_stats(g, stride, W, n, r, M, S);
+  const float* planes = g + (lane < W ? lane : 0) * stride + kShardHeader + 2 * n;
+  int head = 0;
+  for (int i = 0; i < k; ++i) {
+    float key = FLT_MAX;
+    int id = kNoId, owner = lane;
+    if (lane < W && head < k) {
+      const int v = __float_as_int(planes[(k + head) * n + r]);
+      if (v >= 0) {
+        key = -planes[head * n + r];
+        id = v;
+      }
+    }
+    warp_argmin(key, id, owner);
+    if (lane == owner) ++head;
+    if (lane == 0) {
+      const bool none = id == kNoId;
+      ids[r * k + i] = none ? -1 : id;
+      values[r * k + i] = none ? 0.f : expf(-key - M) / S;
+    }
+  }
+}
+
+struct TopkWorkspace {
+  DiscreteScratch s;           // img, h and z ([n, chunk]) for discrete_hidden / discrete_logits
+  float *run_max, *run_sum;
+  Cand *list[2], *part;        // two running lists [n, k] (ping-pong), the chunk's partial lists [n, splits, k]
+  int64_t bytes;
+};
+static TopkWorkspace topk_carve(const recnn_discrete_dims& d, int64_t n, int k, int chunk, void* base) {
+  TopkWorkspace w;
+  Carve c(base);
+  memset(&w.s, 0, sizeof(w.s));
+  w.s.img = c.take(n * pad4(d.state_dim));
+  w.s.h = c.take(n * d.hidden);
+  w.s.z = c.take(n * (int64_t)chunk);
+  w.run_max = c.take(n);
+  w.run_sum = c.take(n);
+  w.list[0] = c.take<Cand>(n * k);
+  w.list[1] = c.take<Cand>(n * k);
+  w.part = c.take<Cand>(n * topk_splits(n, chunk, kTopkSplitCap) * k);     // the widest chunk has the most splits
+  w.bytes = c.bytes();
+  return w;
+}
+
+// The hidden layer, then every chunk: logits, row statistics into (run_max, run_sum), selection and merge.  Candidate
+// ids are id0 + the local item.  Returns the final lists.
+static int policy_topk_pass(const recnn_discrete_dims& d, const float* params, const float* state, int64_t n, int k,
+                            const long long* exclude, int n_ex, int chunk, int id0, const TopkWorkspace& w,
+                            float* run_max, float* run_sum, const Cand** lists, cudaStream_t st) {
+  const int I = d.num_items;
+  RECNN_PROPAGATE(discrete_hidden(d, params, state, n, w.s, st, nullptr));
+  cand_fill_kernel<<<(unsigned)ceil_div(n * k, 256), 256, 0, st>>>(w.list[0], n * k);
+  RECNN_CHECK_LAUNCH("cand_fill_kernel");
+  int cur = 0;
+  for (int c0 = 0; c0 < I; c0 += chunk) {
+    const int cw = I - c0 < chunk ? I - c0 : chunk;
+    RECNN_PROPAGATE(discrete_logits(d, params, n, w.s, c0, cw, w.s.z, st));
+    logit_stats_kernel<<<row_grid(n), kRowThreads, 0, st>>>(w.s.z, cw, n, cw, c0, nullptr, 0, run_max, run_sum,
+                                                            nullptr);
+    RECNN_CHECK_LAUNCH("logit_stats_kernel");
+    const int splits = topk_splits(n, cw, kTopkSplitCap);
+    const dim3 grid((unsigned)splits, (unsigned)(n < 65535 ? n : 65535));
+    if (k <= 16)
+      policy_topk_select_kernel<16><<<grid, kTopkThreads, 0, st>>>(w.s.z, n, cw, id0 + c0, k, exclude, n_ex,
+                                                                   w.list[cur], w.part);
+    else
+      policy_topk_select_kernel<64><<<grid, kTopkThreads, 0, st>>>(w.s.z, n, cw, id0 + c0, k, exclude, n_ex,
+                                                                   w.list[cur], w.part);
+    RECNN_CHECK_LAUNCH("policy_topk_select_kernel");
+    policy_topk_merge_kernel<<<(unsigned)ceil_div(n, 4), 128, 0, st>>>(w.list[cur], w.part, splits, k, n,
+                                                                       w.list[cur ^ 1]);
+    RECNN_CHECK_LAUNCH("policy_topk_merge_kernel");
+    cur ^= 1;
+  }
+  *lists = w.list[cur];
+  return RECNN_OK;
+}
+
+static int exclude_check(const long long* exclude, int64_t n, int n_ex, int64_t items, int* flag, cudaStream_t st) {
+  if (n_ex == 0) return RECNN_OK;
+  exclude_check_kernel<<<(unsigned)ceil_div(n * n_ex, 256), 256, 0, st>>>(exclude, n * n_ex, items, flag);
+  RECNN_CHECK_LAUNCH("exclude_check_kernel");
+  return RECNN_OK;
 }
 
 }  // namespace recnn
@@ -819,5 +1061,92 @@ extern "C" int recnn_discrete_shard_pick(int32_t world, const float* gathered_dr
   shard_pick_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       gathered_draws, world, n_rows, reinterpret_cast<long long*>(action_out), log_prob_out, error_flag);
   RECNN_CHECK_LAUNCH("shard_pick_kernel");
+  return RECNN_OK;
+}
+
+// ---- the policy's top-k ----------------------------------------------------------------------------------------
+static bool topk_args_ok(const recnn_discrete_dims& d, int64_t n, int k, int chunk) {
+  return n > 0 && k >= 1 && k <= 64 && chunk_ok(d, chunk);
+}
+
+extern "C" int64_t recnn_discrete_topk_workspace_bytes(const recnn_discrete_dims* d, int64_t n_rows, int32_t k,
+                                                       int32_t chunk_items) {
+  if (!discrete_dims_ok(d) || !topk_args_ok(*d, n_rows, k, chunk_items)) return 0;
+  return topk_carve(*d, n_rows, k, chunk_items, nullptr).bytes;
+}
+
+static int topk_check(const recnn_discrete_dims* d, const float* params, const float* state, int64_t n_rows, int32_t k,
+                      const int64_t* exclude, int32_t n_exclude, int32_t chunk_items, void* workspace,
+                      int64_t workspace_bytes) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && state && workspace, "null pointer / dims");
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(k >= 1 && k <= 64, "1 <= k <= 64");
+  RECNN_REQUIRE(n_exclude >= 0 && n_exclude <= kMaxExclude && (n_exclude == 0 || exclude), "0 <= n_exclude <= 256");
+  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  return check_workspace(topk_carve(*d, n_rows, k, chunk_items, nullptr).bytes, workspace_bytes);
+}
+
+extern "C" int recnn_discrete_topk(const recnn_discrete_dims* d, const float* params, const float* state,
+                                   int64_t n_rows, int32_t k, const int64_t* exclude, int32_t n_exclude,
+                                   int32_t chunk_items, float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                   void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(values_out && ids_out && error_flag, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, exclude, n_exclude, chunk_items, workspace, workspace_bytes));
+  RECNN_REQUIRE(k <= d->num_items, "k <= num_items");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* ex = reinterpret_cast<const long long*>(exclude);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(exclude_check(ex, n_rows, n_exclude, d->num_items, error_flag, st));
+  const Cand* lists;
+  RECNN_PROPAGATE(policy_topk_pass(*d, params, state, n_rows, k, ex, n_exclude, chunk_items, 0, w, w.run_max,
+                                   w.run_sum, &lists, st));
+  policy_topk_finish_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(
+      lists, n_rows, k, w.run_max, w.run_sum, values_out, reinterpret_cast<long long*>(ids_out));
+  RECNN_CHECK_LAUNCH("policy_topk_finish_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int64_t recnn_vocab_topk_record_floats(int64_t n_rows, int32_t k) {
+  return n_rows > 0 && k >= 1 && k <= 64 ? topk_record_floats(n_rows, k) : 0;
+}
+
+extern "C" int recnn_discrete_shard_topk(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                         const float* state, int64_t n_rows, int32_t k, const int64_t* exclude,
+                                         int32_t n_exclude, int32_t chunk_items, float* record, void* workspace,
+                                         int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(record, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, exclude, n_exclude, chunk_items, workspace, workspace_bytes));
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  RECNN_REQUIRE(k <= v->num_items, "k <= num_items (the whole vocabulary)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  float* m = record + kShardHeader;
+  const Cand* lists;
+  RECNN_PROPAGATE(policy_topk_pass(*d, params, state, n_rows, k, reinterpret_cast<const long long*>(exclude),
+                                   n_exclude, chunk_items, v->item_offset, w, m, m + n_rows, &lists, st));
+  policy_topk_record_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(
+      lists, n_rows, k, v->item_offset, v->item_offset + d->num_items, v->num_items, record);
+  RECNN_CHECK_LAUNCH("policy_topk_record_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                const float* gathered, int64_t n_rows, int32_t k,
+                                                const int64_t* exclude, int32_t n_exclude, float* values_out,
+                                                int64_t* ids_out, int32_t* error_flag, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && gathered && values_out && ids_out && error_flag, "null pointer / dims");
+  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  RECNN_REQUIRE(v->world <= 32, "world <= 32");
+  RECNN_REQUIRE(n_rows > 0 && k >= 1 && k <= 64, "n_rows / k");
+  RECNN_REQUIRE(n_exclude >= 0 && n_exclude <= kMaxExclude && (n_exclude == 0 || exclude), "0 <= n_exclude <= 256");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(exclude_check(reinterpret_cast<const long long*>(exclude), n_rows, n_exclude, v->num_items,
+                                error_flag, st));
+  policy_topk_shard_finish_kernel<<<(unsigned)ceil_div(n_rows, 4), 128, 0, st>>>(
+      gathered, v->world, n_rows, k, v->rank, v->item_offset, v->item_offset + d->num_items, v->num_items, values_out,
+      reinterpret_cast<long long*>(ids_out), error_flag);
+  RECNN_CHECK_LAUNCH("policy_topk_shard_finish_kernel");
   return RECNN_OK;
 }

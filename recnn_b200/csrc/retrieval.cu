@@ -20,10 +20,9 @@
 #include "common.cuh"
 #include "gemm_simt.cuh"
 #include "tc_gemm.cuh"
+#include "topk.cuh"
 
 namespace recnn {
-
-constexpr int kTopkThreads = 256;
 
 // per item: |t|^2 (L2) or 1/|t| (COS)
 __global__ void __launch_bounds__(256)
@@ -36,45 +35,6 @@ item_norms_kernel(const float* __restrict__ table, long long n_items, int dim, i
   for (int d = lane; d < dim; d += 32) s = fmaf(t[d], t[d], s);
   s = warp_sum(s);
   if (lane == 0) out[row] = metric == RECNN_METRIC_COS ? 1.0f / fmaxf(sqrtf(s), 1e-30f) : s;
-}
-
-struct Cand {
-  float key;
-  int id;
-};
-__device__ __forceinline__ bool better(float ka, int ia, float kb, int ib) { return ka < kb || (ka == kb && ia < ib); }
-
-// block arg-min over one candidate per thread; returns the winner's (key, id, owner thread) to every thread
-__device__ __forceinline__ void block_argmin(float key, int id, float* s_key, int* s_id, int* s_owner, float& wk,
-                                             int& wi, int& wo) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int owner = threadIdx.x;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float k2 = __shfl_xor_sync(0xffffffffu, key, o);
-    const int i2 = __shfl_xor_sync(0xffffffffu, id, o);
-    const int o2 = __shfl_xor_sync(0xffffffffu, owner, o);
-    if (better(k2, i2, key, id)) { key = k2; id = i2; owner = o2; }
-  }
-  __syncthreads();
-  if (lane == 0) { s_key[warp] = key; s_id[warp] = id; s_owner[warp] = owner; }
-  __syncthreads();
-  if (warp == 0) {
-    const int nw = blockDim.x >> 5;
-    key = lane < nw ? s_key[lane] : FLT_MAX;
-    id = lane < nw ? s_id[lane] : 0x7fffffff;
-    owner = lane < nw ? s_owner[lane] : -1;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float k2 = __shfl_xor_sync(0xffffffffu, key, o);
-      const int i2 = __shfl_xor_sync(0xffffffffu, id, o);
-      const int o2 = __shfl_xor_sync(0xffffffffu, owner, o);
-      if (better(k2, i2, key, id)) { key = k2; id = i2; owner = o2; }
-    }
-    if (lane == 0) { s_key[0] = key; s_id[0] = id; s_owner[0] = owner; }
-  }
-  __syncthreads();
-  wk = s_key[0]; wi = s_id[0]; wo = s_owner[0];
 }
 
 // grid (splits, n_queries).  scores [n_queries, ld]; writes k candidates per (query, split), ascending.
@@ -90,33 +50,21 @@ topk_partial_kernel(const float* __restrict__ scores, long long ld, long long n_
   const float* row = scores + (long long)q * ld;
   float keys[KMAX];
   int ids[KMAX];
-#pragma unroll
-  for (int i = 0; i < KMAX; ++i) { keys[i] = FLT_MAX; ids[i] = 0x7fffffff; }
+  list_clear(keys, ids);
   for (long long j = lo + threadIdx.x; j < hi; j += blockDim.x) {
     const float s = __ldcs(row + j);
     float key = metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
               : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s;
     if (!(key == key)) key = FLT_MAX;                 // NaN scores rank last
     int id = (int)j;
-    if (better(key, id, keys[KMAX - 1], ids[KMAX - 1])) {
-      // sorted insertion by a chain of compare-exchanges (fully unrolled: the list stays in registers)
-#pragma unroll
-      for (int i = 0; i < KMAX; ++i) {
-        if (better(key, id, keys[i], ids[i])) {
-          const float tk = keys[i]; const int ti = ids[i];
-          keys[i] = key; ids[i] = id;
-          key = tk; id = ti;
-        }
-      }
-    }
+    if (better(key, id, keys[KMAX - 1], ids[KMAX - 1])) list_insert(keys, ids, key, id);
   }
   // merge the 256 sorted lists: k rounds of arg-min over the heads
   int head = 0;
   Cand* out = part + ((long long)q * splits + sp) * k;
   for (int r = 0; r < k; ++r) {
-    float hk = FLT_MAX; int hid = 0x7fffffff;
-#pragma unroll
-    for (int i = 0; i < KMAX; ++i) if (i == head) { hk = keys[i]; hid = ids[i]; }
+    float hk; int hid;
+    list_at(keys, ids, head, hk, hid);
     float wk; int wi, wo;
     block_argmin(hk, hid, s_key, s_id, s_owner, wk, wi, wo);
     if ((int)threadIdx.x == wo) ++head;
@@ -138,35 +86,22 @@ topk_merge_kernel(const Cand* __restrict__ part, int splits, int k, long long n_
   // lane l walks lists l, l+32, ...: keeps one head per owned list in a small loop (splits <= 32 in practice)
   int head = 0;                                      // lane's position in list `lane` (splits <= 32)
   for (int r = 0; r < k; ++r) {
-    float key = FLT_MAX; int id = 0x7fffffff;
+    float key = FLT_MAX; int id = kNoId;
     if (lane < splits && head < k) { key = mine[(long long)lane * k + head].key; id = mine[(long long)lane * k + head].id; }
     int owner = lane;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float k2 = __shfl_xor_sync(0xffffffffu, key, o);
-      const int i2 = __shfl_xor_sync(0xffffffffu, id, o);
-      const int o2 = __shfl_xor_sync(0xffffffffu, owner, o);
-      if (better(k2, i2, key, id)) { key = k2; id = i2; owner = o2; }
-    }
+    warp_argmin(key, id, owner);
     if (lane == owner) ++head;
     if (lane == 0) {
       float d;
       if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);                 // squared L2 distance
       else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);  // cosine similarity
       else d = -key;                                                           // inner product
-      ids_out[q * k + r] = id == 0x7fffffff ? -1 : (int64_t)id;
+      ids_out[q * k + r] = id == kNoId ? -1 : (int64_t)id;
       dist_out[q * k + r] = d;
     }
   }
 }
 
-static int topk_splits(int64_t n_queries, int64_t n_items) {
-  int64_t s = ceil_div(2 * kNumSMs, n_queries);
-  const int64_t max_by_items = ceil_div(n_items, 4 * kTopkThreads);
-  if (s > max_by_items) s = max_by_items;
-  if (s > 32) s = 32;
-  return (int)(s < 1 ? 1 : s);
-}
 static int64_t slab_rows(int64_t n_items) {
   // a slab of scores should stay L2-resident between the GEMM that writes it and the top-k pass that reads it:
   // 32 MB of the H100's 50 MB L2, leaving room for the item table, its norms and the top-k partials
@@ -248,7 +183,7 @@ extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int3
       RECNN_PROPAGATE((launch_gemm_simt<true, true, EPI_STORE>(mat(Q, dim), mat(table, dim), (int)nq, (int)n_items, dim,
                                                                 1, e, st)));
     }
-    const int splits = topk_splits(nq, n_items);
+    const int splits = topk_splits(nq, n_items, 32);
     dim3 grid((unsigned)splits, (unsigned)nq);
     if (k <= 16)
       topk_partial_kernel<16><<<grid, kTopkThreads, 0, st>>>(scores, ld, n_items, norms, metric, k, part);

@@ -20,6 +20,7 @@
 #include "gemm_simt.cuh"
 #include "pointwise.cuh"
 #include "tc_gemm.cuh"
+#include "topk.cuh"
 
 namespace recnn {
 

@@ -171,6 +171,68 @@ class DiscreteActor(nn.Module):
             raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
         return out, gathered
 
+    def topk(self, state, k, exclude=None):
+        """``(values, indices)`` as ``torch.topk(self(state), k)`` without forming the [N, num_items] probabilities:
+        the k items of highest logit per row (equal logits: the smaller id first), values fp32 [N, k] = pi(a|s),
+        indices int64 [N, k] global item ids, on a vocabulary-parallel policy too (one all-gather of k candidates per
+        row and rank).  ``exclude``: optional integer [N, E] (E <= 256) of ids never returned -- e.g. the frame's
+        items -- that stay in the softmax's normaliser (values are not renormalised); negative ids are padding, an
+        id >= num_items raises IndexError.  A row with fewer than k eligible items ends in id -1, value 0.
+        1 <= k <= min(64, num_items).  Inference only: nothing saved for the policy update is touched."""
+        from .update.reinforce import _chunk_items
+        vp = self.__dict__.get("_recnn_vp")
+        d = self.dims
+        items = d.num_items if vp is None else vp.num_items
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(64, items):
+            raise ValueError("k must be an int in [1, min(64, num_items)] = [1, %d], got %r" % (min(64, items), k))
+        if not torch.is_tensor(state) or state.dim() != 2 or state.shape[1] != d.state_dim:
+            raise ValueError("state must be a [N, %d] tensor" % d.state_dim)
+        n = state.shape[0]
+        n_ex = 0
+        if exclude is not None:
+            if (not torch.is_tensor(exclude) or exclude.dim() != 2 or exclude.shape[0] != n
+                    or exclude.shape[1] > 256 or exclude.dtype.is_floating_point or exclude.dtype == torch.bool):
+                raise ValueError("exclude must be an integer tensor [N, E] with N = %d rows and E <= 256 (got %s)"
+                                 % (n, tuple(exclude.shape) if torch.is_tensor(exclude) else type(exclude).__name__))
+            n_ex = exclude.shape[1]
+        dev = self.linear1.weight.device
+        if dev.type != "cuda":
+            raise _lib.RecnnError("recnn_b200 nets run on CUDA only (module is on %s); call .cuda() first" % dev)
+        values = torch.empty(n, k, device=dev, dtype=torch.float32)
+        ids = torch.empty(n, k, device=dev, dtype=torch.int64)
+        if n == 0:
+            return values, ids
+        _, (state,) = _device_check(self, state)
+        ex = None if n_ex == 0 else exclude.detach().to(device=dev, dtype=torch.int64).contiguous()
+        L = _lib.lib()
+        flat = param_arena(self)
+        chunk = _chunk_items(n, d.num_items)
+        nbytes = L.recnn_discrete_topk_workspace_bytes(d, n, k, chunk)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        flag = torch.empty(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            if vp is None:
+                _lib.check(L.recnn_discrete_topk(d, flat.data_ptr(), state.data_ptr(), n, k, _lib.ptr(ex), n_ex, chunk,
+                                                 values.data_ptr(), ids.data_ptr(), flag.data_ptr(), ws.data_ptr(),
+                                                 nbytes, _lib.stream_ptr(dev)))
+            else:
+                shard = vp.shard()
+                rec = torch.empty(L.recnn_vocab_topk_record_floats(n, k), device=dev, dtype=torch.float32)
+                _lib.check(L.recnn_discrete_shard_topk(d, shard, flat.data_ptr(), state.data_ptr(), n, k, _lib.ptr(ex),
+                                                       n_ex, chunk, rec.data_ptr(), ws.data_ptr(), nbytes,
+                                                       _lib.stream_ptr(dev)))
+                del ws
+                gathered = vp.all_gather(rec)
+                _lib.check(L.recnn_discrete_shard_topk_finish(d, shard, gathered.data_ptr(), n, k, _lib.ptr(ex), n_ex,
+                                                              values.data_ptr(), ids.data_ptr(), flag.data_ptr(),
+                                                              _lib.stream_ptr(dev)))
+        bits = int(flag.item())
+        if bits & 2:
+            raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+        if bits & 1:
+            raise IndexError("an excluded item id is out of range for the policy's %d items" % items)
+        return values, ids
+
     def gc(self):
         del self.rewards[:]
         del self.saved_log_probs[:]
