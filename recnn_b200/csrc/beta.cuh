@@ -146,14 +146,14 @@ beta_dz_kernel(const float* __restrict__ P, long long ld, long long n, int w, in
 // part (the first two planes of the exchange-2 record).  Bit 2 of *err when the headers do not tile the vocabulary.
 // At W = 1, M = m_0 and S = s_0: beta_rows_kernel's p.  One CTA per row.
 __global__ void __launch_bounds__(kRowThreads)
-beta_shard_rows_kernel(float* __restrict__ P, long long n, int w, const float* __restrict__ g, int W, int rank, int lo,
-                       int items, float* __restrict__ run_max, float* __restrict__ run_sum, float* __restrict__ za,
+beta_shard_rows_kernel(float* __restrict__ P, long long n, int w, const float* __restrict__ g, ShardPlan p,
+                       float* __restrict__ run_max, float* __restrict__ run_sum, float* __restrict__ za,
                        float* __restrict__ part, unsigned* err) {
   __shared__ float red[32];
-  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, W, n, rank, lo, lo + w, items)) atomicOr(err, 2u);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, shard_record_floats(n), p, n)) atomicOr(err, 2u);
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
     float M, S, z, s1, s2;
-    shard_merge_row(g, W, n, r, M, S, z);
+    shard_merge_row(g, p.world, n, r, M, S, z);
     beta_normalise_row(P + r * w, w, M, S, red, &s1, &s2);
     if (threadIdx.x == 0) {
       run_max[r] = M;
@@ -168,23 +168,21 @@ beta_shard_rows_kernel(float* __restrict__ P, long long n, int w, const float* _
 
 // Sharded, after exchange 2: the vocabulary sums in rank order (at W = 1, 0 + s1_0 = s1_0: the unsharded bits), then
 // beta_row_terms.  Bit 2 of *err when the headers do not tile the vocabulary.  One thread per row.
-__global__ void beta_shard_terms_kernel(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi,
-                                        int items, const long long* __restrict__ action,
-                                        const float* __restrict__ run_max, const float* __restrict__ run_sum,
-                                        const float* __restrict__ za, float* __restrict__ T_out,
-                                        float* __restrict__ pe_out, float* __restrict__ pa_out,
-                                        float* __restrict__ row_loss, unsigned* err) {
+__global__ void beta_shard_terms_kernel(const float* __restrict__ g, long long n, ShardPlan p,
+                                        const long long* __restrict__ action, const float* __restrict__ run_max,
+                                        const float* __restrict__ run_sum, const float* __restrict__ za,
+                                        float* __restrict__ T_out, float* __restrict__ pe_out,
+                                        float* __restrict__ pa_out, float* __restrict__ row_loss, unsigned* err) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0 && shard_plan_bad(g, W, n, rank, lo, hi, items)) atomicOr(err, 2u);
-  if (r >= n) return;
   const long long stride = shard_record_floats(n);
+  if (r == 0 && shard_plan_bad(g, stride, p, n)) atomicOr(err, 2u);
+  if (r >= n) return;
   float s1 = 0.f, s2 = 0.f;
-  for (int q = 0; q < W; ++q) {
-    const float* rec = g + q * stride + kShardHeader;
-    s1 += rec[r];
-    s2 += rec[n + r];
+  for (int q = 0; q < p.world; ++q) {
+    s1 += shard_plane(g, n, 0, q, stride)[r];
+    s2 += shard_plane(g, n, 1, q, stride)[r];
   }
-  beta_row_terms(r, action[r], items, run_max[r], run_sum[r], za[r], s1, s2, T_out, pe_out, pa_out, row_loss, err);
+  beta_row_terms(r, action[r], p.items, run_max[r], run_sum[r], za[r], s1, s2, T_out, pe_out, pa_out, row_loss, err);
 }
 
 }  // namespace recnn
@@ -199,7 +197,7 @@ extern "C" int recnn_beta_layout(const recnn_beta_dims* d, int64_t* out) {
 }
 
 extern "C" int64_t recnn_beta_workspace_bytes(const recnn_beta_dims* d, int64_t n_rows, int32_t chunk_items) {
-  if (!beta_dims_ok(d) || n_rows <= 0 || !critic_chunk_ok(d->num_items, chunk_items)) return 0;
+  if (!beta_dims_ok(d) || n_rows <= 0 || !chunk_ok(d->num_items, chunk_items)) return 0;
   return beta_carve(*d, n_rows, chunk_items, nullptr).bytes;
 }
 
@@ -227,7 +225,7 @@ static int beta_check(const recnn_beta_args* a, BetaWorkspace* w) {
   RECNN_REQUIRE(beta_dims_ok(&a->dims), "dims");
   RECNN_REQUIRE(a->n_rows > 0, "n_rows");
   const int S = a->dims.state_dim, I = a->dims.num_items, W = a->chunk_items;
-  RECNN_REQUIRE(critic_chunk_ok(I, W), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_REQUIRE(chunk_ok(I, W), "chunk_items must be num_items or a positive multiple of 128 below it");
   const int64_t widest = pad4(S) > W ? pad4(S) : W;
   RECNN_REQUIRE(a->n_rows < (1ll << 31) / (widest + 1), "n_rows too large for int32 tile indexing");
   RECNN_REQUIRE(a->state && a->state_ld >= S && a->action, "state / state_ld / action");
@@ -248,11 +246,8 @@ static int beta_logits_pass(const recnn_beta_args* a, const BetaWorkspace& w, in
   const float* P = a->net.params;
   const long long* act = reinterpret_cast<const long long*>(a->action);
   RECNN_CHECK_CUDA(cudaMemsetAsync(w.flags, 0, 8 * sizeof(unsigned), st));
-  recnn_dims dd;
-  memset(&dd, 0, sizeof(dd));
-  dd.state_dim = S;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(dd, a->state, n, w.img, &xs, st, a->state_ld));
+  RECNN_PROPAGATE(repitch_state(S, a->state, n, w.img, &xs, st, a->state_ld));
   for (int c0 = 0; c0 < I; c0 += W) {
     const int wc = I - c0 < W ? I - c0 : W;
     RECNN_PROPAGATE(linear_out(xs, P + l.w + (int64_t)c0 * l.ldw, l.ldw, P + l.b + c0, wc, n, 0, nullptr,
@@ -306,47 +301,36 @@ extern "C" int recnn_beta_step(const recnn_beta_args* a, void* stream) {
 }
 
 // ---- beta sharded over the item vocabulary: the three phases around the two all-gathers (see the header) ----------
-static int beta_shard_check(const recnn_beta_args* a, const recnn_vocab_shard* v, BetaWorkspace* w) {
+static int beta_shard_check(const recnn_beta_args* a, const recnn_vocab_shard* v, BetaWorkspace* w, ShardPlan* p) {
   RECNN_PROPAGATE(beta_check(a, w));
-  recnn_discrete_dims d;
-  memset(&d, 0, sizeof(d));
-  d.num_items = a->dims.num_items;
-  RECNN_REQUIRE(shard_ok(&d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
-  return RECNN_OK;
-}
-
-// a record's header {lo, hi, num_items, n} and a zero third plane
-static int beta_record_init(const recnn_beta_args* a, const recnn_vocab_shard* v, float* record, cudaStream_t st) {
-  const int64_t n = a->n_rows;
-  shard_record_init_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(record, n, v->item_offset,
-                                                                      v->item_offset + a->dims.num_items, v->num_items);
-  RECNN_CHECK_LAUNCH("shard_record_init_kernel");
-  return RECNN_OK;
+  return shard_plan(a->dims.num_items, v, p);
 }
 
 extern "C" int recnn_beta_shard_begin(const recnn_beta_args* a, const recnn_vocab_shard* v, float* record,
                                       void* stream) {
   BetaWorkspace w;
-  RECNN_PROPAGATE(beta_shard_check(a, v, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(beta_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(record != nullptr, "record");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = a->n_rows;
-  RECNN_PROPAGATE(beta_record_init(a, v, record, st));
-  float* m = record + kShardHeader;
-  return beta_logits_pass(a, w, v->item_offset, m, m + n, m + 2 * n, st);
+  RECNN_PROPAGATE(shard_record_init(p, record, n, st));
+  return beta_logits_pass(a, w, p.lo, shard_plane(record, n, 0), shard_plane(record, n, 1), shard_plane(record, n, 2),
+                          st);
 }
 
 extern "C" int recnn_beta_shard_rows(const recnn_beta_args* a, const recnn_vocab_shard* v, const float* gathered,
                                      float* record, void* stream) {
   BetaWorkspace w;
-  RECNN_PROPAGATE(beta_shard_check(a, v, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(beta_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(gathered && record, "gathered / record");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = a->n_rows;
-  RECNN_PROPAGATE(beta_record_init(a, v, record, st));
-  beta_shard_rows_kernel<<<row_grid(n), kRowThreads, 0, st>>>(a->probs_out, n, a->dims.num_items, gathered, v->world,
-                                                              v->rank, v->item_offset, v->num_items, w.run_max,
-                                                              w.run_sum, w.za, record + kShardHeader, w.flags);
+  RECNN_PROPAGATE(shard_record_init(p, record, n, st));
+  beta_shard_rows_kernel<<<row_grid(n), kRowThreads, 0, st>>>(a->probs_out, n, a->dims.num_items, gathered, p,
+                                                              w.run_max, w.run_sum, w.za, shard_plane(record, n, 0),
+                                                              w.flags);
   RECNN_CHECK_LAUNCH("beta_shard_rows_kernel");
   return RECNN_OK;
 }
@@ -354,13 +338,14 @@ extern "C" int recnn_beta_shard_rows(const recnn_beta_args* a, const recnn_vocab
 extern "C" int recnn_beta_shard_end(const recnn_beta_args* a, const recnn_vocab_shard* v, const float* gathered,
                                     void* stream) {
   BetaWorkspace w;
-  RECNN_PROPAGATE(beta_shard_check(a, v, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(beta_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(gathered != nullptr, "gathered");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = a->n_rows;
   beta_shard_terms_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(
-      gathered, v->world, n, v->rank, v->item_offset, v->item_offset + a->dims.num_items, v->num_items,
-      reinterpret_cast<const long long*>(a->action), w.run_max, w.run_sum, w.za, w.T, w.pe, w.pa, w.row_loss, w.flags);
+      gathered, n, p, reinterpret_cast<const long long*>(a->action), w.run_max, w.run_sum, w.za, w.T, w.pe, w.pa,
+      w.row_loss, w.flags);
   RECNN_CHECK_LAUNCH("beta_shard_terms_kernel");
-  return beta_grad_pass(a, w, v->item_offset, v->num_items, st);
+  return beta_grad_pass(a, w, p.lo, p.items, st);
 }

@@ -16,10 +16,6 @@
 
 namespace recnn {
 
-static bool critic_chunk_ok(int num_items, int64_t chunk) {
-  return chunk == num_items || (chunk > 0 && chunk % 128 == 0 && chunk < num_items);
-}
-
 // split count of one chunk's projection GEMM Y_part[rows, H] = P_c W1a_c^T (K = lead + chunk): the [rows, H] output is
 // only ceil(rows/128) * ceil(H/128) tiles, so the chunk's K is split to fill the SMs (>= 4 k-blocks of 32 per split).
 static int proj_splits(int64_t n, int H, int K) {
@@ -234,13 +230,13 @@ __global__ void scatter_action_grad_kernel(const unsigned long long* __restrict_
 // the target action term, merged in rank order as shard_merge_row does for the policy) and terms[1] = add_r.  At W = 1
 // the factor is exp(0) = 1 and S = s_0, and the division is proj_fold_kernel's: the unsharded bits.  One CTA per row.
 __global__ void __launch_bounds__(kRowThreads)
-critic_shard_merge_kernel(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items,
-                          const float* __restrict__ local_max, const float* __restrict__ Y,
-                          const float* __restrict__ add, int H, float* __restrict__ terms, unsigned* plan_bad) {
-  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, W, n, rank, lo, hi, items)) *plan_bad = 1u;
+critic_shard_merge_kernel(const float* __restrict__ g, long long n, ShardPlan p, const float* __restrict__ local_max,
+                          const float* __restrict__ Y, const float* __restrict__ add, int H, float* __restrict__ terms,
+                          unsigned* plan_bad) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, shard_record_floats(n), p, n)) *plan_bad = 1u;
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
     float M, S, za;
-    shard_merge_row(g, W, n, r, M, S, za);
+    shard_merge_row(g, p.world, n, r, M, S, za);
     const float f = expf(local_max[r] - M);
     for (int h = threadIdx.x; h < H; h += blockDim.x) {
       const long long i = r * H + h;
@@ -305,7 +301,7 @@ using namespace recnn;
 
 extern "C" int64_t recnn_critic_action_term_scratch_floats(const recnn_dims* d, const recnn_discrete_dims* pd,
                                                            int64_t n_rows, int32_t chunk_items) {
-  if (!d || n_rows <= 0 || d->state_dim <= 0 || d->hidden <= 0 || !critic_chunk_ok(d->action_dim, chunk_items)) return 0;
+  if (!d || n_rows <= 0 || d->state_dim <= 0 || d->hidden <= 0 || !chunk_ok(d->action_dim, chunk_items)) return 0;
   Carve c(nullptr);
   proj_carve(*d, pd, n_rows, chunk_items, c);
   return c.floats();
@@ -321,18 +317,13 @@ extern "C" int recnn_critic_action_term_chunked(const recnn_dims* d, const float
   RECNN_REQUIRE((policy_params != nullptr) != (probs != nullptr), "give a policy (policy_params, state) or probs");
   RECNN_REQUIRE(!policy_params || (pd && state && dv_dims_ok(*d, *pd)), "policy dims / state");
   RECNN_REQUIRE(!probs || probs_ld >= d->action_dim, "probs_ld");
-  RECNN_REQUIRE(critic_chunk_ok(d->action_dim, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_REQUIRE(chunk_ok(d->action_dim, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   if (n_rows <= 0) return RECNN_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Carve c(scratch);
   const ProjScratch s = proj_carve(*d, policy_params ? pd : nullptr, n_rows, chunk_items, c);
   Seg xs = kNoSeg;
-  if (policy_params) {
-    recnn_dims dd;
-    memset(&dd, 0, sizeof(dd));
-    dd.state_dim = pd->state_dim; dd.hidden = pd->hidden; dd.action_dim = pd->num_items;
-    RECNN_PROPAGATE(repitch_state(dd, state, n_rows, s.img, &xs, st));
-  }
+  if (policy_params) RECNN_PROPAGATE(repitch_state(pd->state_dim, state, n_rows, s.img, &xs, st));
   return action_term_chunked(*d, critic_params, pd, policy_params, xs, probs, probs_ld, n_rows, chunk_items, s, out, st);
 }
 
@@ -349,7 +340,7 @@ extern "C" int recnn_critic_forward_action_term(const recnn_dims* d, const float
   Rng rng = {nullptr, 0, nullptr};
   const bool train = mask1 != nullptr;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, s.img, &xs, st));
+  RECNN_PROPAGATE(repitch_state(d->state_dim, state, n_rows, s.img, &xs, st));
   const Seg s1 = {s.h1, H, H, 0};
   RECNN_PROPAGATE(hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, s.h1,
                                st, action_term));
@@ -363,7 +354,7 @@ extern "C" int recnn_critic_forward_action_term(const recnn_dims* d, const float
 
 extern "C" int64_t recnn_discrete_value_workspace_bytes(const recnn_dims* d, const recnn_discrete_dims* pd,
                                                         int64_t n_rows, int32_t chunk_items) {
-  if (!d || !pd || n_rows <= 0 || !dv_dims_ok(*d, *pd) || !critic_chunk_ok(d->action_dim, chunk_items)) return 0;
+  if (!d || !pd || n_rows <= 0 || !dv_dims_ok(*d, *pd) || !chunk_ok(d->action_dim, chunk_items)) return 0;
   return dv_carve(*d, *pd, n_rows, chunk_items, nullptr).bytes;
 }
 
@@ -376,7 +367,7 @@ static int dv_check(const recnn_discrete_value_args* a, DvWorkspace* w) {
   RECNN_REQUIRE(dv_dims_ok(a->dims, a->policy_dims), "dims (critic action_dim == policy num_items, equal state_dim)");
   RECNN_REQUIRE(a->n_rows > 0, "n_rows");
   const int S = a->dims.state_dim, H = a->dims.hidden;
-  RECNN_REQUIRE(critic_chunk_ok(a->dims.action_dim, a->chunk_items),
+  RECNN_REQUIRE(chunk_ok(a->dims.action_dim, a->chunk_items),
                 "chunk_items must be num_items or a positive multiple of 128 below it");
   int64_t widest = pad4(S) > H ? pad4(S) : H;
   if (pad4(S % 4 + a->chunk_items) > widest) widest = pad4(S % 4 + a->chunk_items);
@@ -513,24 +504,25 @@ extern "C" int recnn_discrete_value_step(const recnn_discrete_value_args* a, voi
 }
 
 // ---- the vocabulary-sharded critic: the phases around the all-gather and the all-reduce (see the header) ---------
-static int dv_shard_check(const recnn_discrete_value_args* a, const recnn_vocab_shard* v, DvWorkspace* w) {
+static int dv_shard_check(const recnn_discrete_value_args* a, const recnn_vocab_shard* v, DvWorkspace* w,
+                          ShardPlan* p) {
   RECNN_PROPAGATE(dv_check(a, w));
-  RECNN_REQUIRE(shard_ok(&a->policy_dims, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
-  return RECNN_OK;
+  return shard_plan(a->policy_dims.num_items, v, p);
 }
 
 extern "C" int recnn_discrete_value_shard_begin(const recnn_discrete_value_args* a, const recnn_vocab_shard* v,
                                                 float* record, void* stream) {
   DvWorkspace w;
-  RECNN_PROPAGATE(dv_shard_check(a, v, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(dv_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(record != nullptr, "record");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = a->n_rows;
-  RECNN_PROPAGATE(dv_action_terms(a, w, v->item_offset, v->num_items, false, st));
-  RECNN_PROPAGATE(shard_record_init(a->policy_dims, *v, record, n, st));
-  RECNN_CHECK_CUDA(cudaMemcpyAsync(record + kShardHeader, w.proj.run_max, n * sizeof(float), cudaMemcpyDeviceToDevice,
-                                   st));
-  RECNN_CHECK_CUDA(cudaMemcpyAsync(record + kShardHeader + n, w.proj.run_sum, n * sizeof(float),
+  RECNN_PROPAGATE(dv_action_terms(a, w, p.lo, p.items, false, st));
+  RECNN_PROPAGATE(shard_record_init(p, record, n, st));
+  RECNN_CHECK_CUDA(cudaMemcpyAsync(shard_plane(record, n, 0), w.proj.run_max, n * sizeof(float),
+                                   cudaMemcpyDeviceToDevice, st));
+  RECNN_CHECK_CUDA(cudaMemcpyAsync(shard_plane(record, n, 1), w.proj.run_sum, n * sizeof(float),
                                    cudaMemcpyDeviceToDevice, st));
   return RECNN_OK;
 }
@@ -538,13 +530,13 @@ extern "C" int recnn_discrete_value_shard_begin(const recnn_discrete_value_args*
 extern "C" int recnn_discrete_value_shard_merge(const recnn_discrete_value_args* a, const recnn_vocab_shard* v,
                                                 const float* gathered, float* terms, void* stream) {
   DvWorkspace w;
-  RECNN_PROPAGATE(dv_shard_check(a, v, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(dv_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(gathered && terms, "gathered / terms");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = a->n_rows;
-  critic_shard_merge_kernel<<<row_grid(n), kRowThreads, 0, st>>>(
-      gathered, v->world, n, v->rank, v->item_offset, v->item_offset + a->policy_dims.num_items, v->num_items,
-      w.proj.run_max, w.Y, w.add, a->dims.hidden, terms, w.tickets + kTicketDpMismatch);
+  critic_shard_merge_kernel<<<row_grid(n), kRowThreads, 0, st>>>(gathered, n, p, w.proj.run_max, w.Y, w.add,
+                                                                  a->dims.hidden, terms, w.tickets + kTicketDpMismatch);
   RECNN_CHECK_LAUNCH("critic_shard_merge_kernel");
   return RECNN_OK;
 }
@@ -552,7 +544,8 @@ extern "C" int recnn_discrete_value_shard_merge(const recnn_discrete_value_args*
 extern "C" int recnn_discrete_value_shard_end(const recnn_discrete_value_args* a, const recnn_vocab_shard* v,
                                               const float* terms, void* stream) {
   DvWorkspace w;
-  RECNN_PROPAGATE(dv_shard_check(a, v, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(dv_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(terms != nullptr, "terms");
-  return dv_tail(a, w, terms, terms + a->n_rows * a->dims.hidden, v->item_offset, static_cast<cudaStream_t>(stream));
+  return dv_tail(a, w, terms, terms + a->n_rows * a->dims.hidden, p.lo, static_cast<cudaStream_t>(stream));
 }

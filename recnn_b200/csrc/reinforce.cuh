@@ -316,14 +316,50 @@ __global__ void __launch_bounds__(1024) sum_rows_kernel(const float* __restrict_
 constexpr int kShardHeader = 4;
 __host__ __device__ __forceinline__ int64_t shard_record_floats(int64_t n) { return kShardHeader + 3 * n; }
 
-// header, and a zero action-logit plane (the owners overwrite their rows in pass 1)
-__global__ void shard_record_init_kernel(float* __restrict__ rec, long long n, int lo, int hi, int items) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) rec[kShardHeader + 2 * n + i] = 0.f;
-  if (i == 0) {
-    int* h = reinterpret_cast<int*>(rec);
-    h[0] = lo; h[1] = hi; h[2] = items; h[3] = (int)n;
+// This rank's place in the plan: rank `rank` of `world` holds items [lo, hi) of the `items`-item vocabulary.
+struct ShardPlan {
+  int world, rank, lo, hi, items;
+};
+
+// The plan of an arena holding `local_items` items on shard v; RECNN_E_INVALID when v does not describe one.
+static int shard_plan(int local_items, const recnn_vocab_shard* v, ShardPlan* p) {
+  RECNN_REQUIRE(v && v->world >= 1 && v->rank >= 0 && v->rank < v->world && v->item_offset >= 0 &&
+                    (int64_t)v->item_offset + local_items <= (int64_t)v->num_items,
+                "shard: rank / world / item_offset + num_items outside the vocabulary");
+  *p = ShardPlan{v->world, v->rank, v->item_offset, v->item_offset + local_items, v->num_items};
+  return RECNN_OK;
+}
+
+// Plane j (of n floats) of a record; in gathered records of `stride` floats, of rank q's record.
+template <typename T>
+__host__ __device__ __forceinline__ T* shard_plane(T* rec, long long n, long long j, int q = 0, long long stride = 0) {
+  return rec + q * stride + kShardHeader + j * n;
+}
+
+__device__ __forceinline__ void shard_header_write(float* rec, const ShardPlan& p, long long n) {
+  int* h = reinterpret_cast<int*>(rec);
+  h[0] = p.lo; h[1] = p.hi; h[2] = p.items; h[3] = (int)n;
+}
+
+// true unless the p.world headers (records of `stride` floats) tile [0, p.items) in rank order, every rank saw n rows
+// and this rank's entry is [p.lo, p.hi)
+__device__ bool shard_plan_bad(const float* __restrict__ g, long long stride, const ShardPlan& p, long long n) {
+  int expect = 0;
+  bool bad = false;
+  for (int q = 0; q < p.world; ++q) {
+    const int* h = reinterpret_cast<const int*>(g + q * stride);
+    bad = bad || h[0] != expect || h[1] <= h[0] || h[2] != p.items || h[3] != (int)n;
+    expect = h[1];
+    if (q == p.rank) bad = bad || h[0] != p.lo || h[1] != p.hi;
   }
+  return bad || expect != p.items;
+}
+
+// header, and a zero action-logit plane (the owners overwrite their rows in pass 1)
+__global__ void shard_record_init_kernel(float* __restrict__ rec, long long n, ShardPlan p) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) shard_plane(rec, n, 2)[i] = 0.f;
+  if (i == 0) shard_header_write(rec, p, n);
 }
 
 // the rank-order merge of row r's statistics from W records of `stride` floats that start with the header and the
@@ -331,12 +367,9 @@ __global__ void shard_record_init_kernel(float* __restrict__ rec, long long n, i
 __device__ __forceinline__ void shard_merge_stats(const float* __restrict__ g, long long stride, int W, long long n,
                                                   long long r, float& M, float& S) {
   M = -INFINITY;
-  for (int q = 0; q < W; ++q) M = fmaxf(M, g[q * stride + kShardHeader + r]);
+  for (int q = 0; q < W; ++q) M = fmaxf(M, shard_plane(g, n, 0, q, stride)[r]);
   S = 0.f;
-  for (int q = 0; q < W; ++q) {
-    const float* rec = g + q * stride + kShardHeader;
-    S += rec[n + r] * expf(rec[r] - M);
-  }
+  for (int q = 0; q < W; ++q) S += shard_plane(g, n, 1, q, stride)[r] * expf(shard_plane(g, n, 0, q, stride)[r] - M);
 }
 
 // the rank-order merge of row r: M and S as above, za = sum za_q
@@ -345,36 +378,17 @@ __device__ __forceinline__ void shard_merge_row(const float* __restrict__ g, int
   const long long stride = shard_record_floats(n);
   shard_merge_stats(g, stride, W, n, r, M, S);
   za = 0.f;
-  for (int q = 0; q < W; ++q) za += g[q * stride + kShardHeader + 2 * n + r];
-}
-
-// true unless the W headers (records of `stride` floats) tile [0, items) in rank order, every rank saw n rows and this
-// rank's entry is [lo, hi)
-__device__ bool shard_plan_bad_at(const float* __restrict__ g, long long stride, int W, long long n, int rank, int lo,
-                                  int hi, int items) {
-  int expect = 0;
-  bool bad = false;
-  for (int q = 0; q < W; ++q) {
-    const int* h = reinterpret_cast<const int*>(g + q * stride);
-    bad = bad || h[0] != expect || h[1] <= h[0] || h[2] != items || h[3] != (int)n;
-    expect = h[1];
-    if (q == rank) bad = bad || h[0] != lo || h[1] != hi;
-  }
-  return bad || expect != items;
-}
-__device__ bool shard_plan_bad(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items) {
-  return shard_plan_bad_at(g, shard_record_floats(n), W, n, rank, lo, hi, items);
+  for (int q = 0; q < W; ++q) za += shard_plane(g, n, 2, q, stride)[r];
 }
 
 // gathered records -> the merged statistics of every row (into the scratch the unsharded path uses); *plan_bad
-__global__ void shard_merge_kernel(const float* __restrict__ g, int W, long long n, int rank, int lo, int hi, int items,
-                                   float* __restrict__ run_max, float* __restrict__ run_sum, float* __restrict__ za,
-                                   int* plan_bad) {
+__global__ void shard_merge_kernel(const float* __restrict__ g, long long n, ShardPlan p, float* __restrict__ run_max,
+                                   float* __restrict__ run_sum, float* __restrict__ za, int* plan_bad) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r == 0 && shard_plan_bad(g, W, n, rank, lo, hi, items)) *plan_bad = 1;
+  if (r == 0 && shard_plan_bad(g, shard_record_floats(n), p, n)) *plan_bad = 1;
   if (r >= n) return;
   float M, S, z;
-  shard_merge_row(g, W, n, r, M, S, z);
+  shard_merge_row(g, p.world, n, r, M, S, z);
   run_max[r] = M;
   run_sum[r] = S;
   za[r] = z;
@@ -382,12 +396,12 @@ __global__ void shard_merge_kernel(const float* __restrict__ g, int W, long long
 
 // the rank's logits block [n, w] -> its block of the softmax, exp(z - M) / S (the last loop of softmax_rows_kernel)
 __global__ void __launch_bounds__(kRowThreads)
-shard_softmax_finish_kernel(float* __restrict__ z, long long n, int w, const float* __restrict__ g, int W, int rank,
-                            int lo, int items, int* plan_bad) {
-  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, W, n, rank, lo, lo + w, items)) *plan_bad = 1;
+shard_softmax_finish_kernel(float* __restrict__ z, long long n, int w, const float* __restrict__ g, ShardPlan p,
+                            int* plan_bad) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, shard_record_floats(n), p, n)) *plan_bad = 1;
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
     float M, S, za;
-    shard_merge_row(g, W, n, r, M, S, za);
+    shard_merge_row(g, p.world, n, r, M, S, za);
     float* row = z + r * w;
     for (int j = threadIdx.x; j < w; j += blockDim.x) row[j] = expf(row[j] - M) / S;
   }
@@ -400,21 +414,20 @@ shard_softmax_finish_kernel(float* __restrict__ z, long long n, int w, const flo
 // inside its block at u' = (u - C_{owner-1}) / P_owner with the inverse CDF of categorical_sample_kernel.  At W = 1,
 // P_0 = 1 and u' = u exactly.  One CTA per row.
 __global__ void __launch_bounds__(kRowThreads)
-shard_sample_kernel(const float* __restrict__ probs, long long n, int w, const float* __restrict__ g, int W, int rank,
-                    int lo, const float* __restrict__ uniforms, unsigned long long seed, long long draw,
+shard_sample_kernel(const float* __restrict__ probs, long long n, int w, const float* __restrict__ g, ShardPlan p,
+                    const float* __restrict__ uniforms, unsigned long long seed, long long draw,
                     float* __restrict__ draw_rec) {
   __shared__ float red[32];
   __shared__ CdfShared sh;
   const long long stride = shard_record_floats(n);
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
     float M, S, za;
-    shard_merge_row(g, W, n, r, M, S, za);
+    shard_merge_row(g, p.world, n, r, M, S, za);
     const float u = draw_uniform(uniforms, seed, draw, r);
     int owner = -1, last = -1;
     float C = 0.f, before = 0.f, P = 0.f, last_before = 0.f, last_P = 0.f;
-    for (int q = 0; q < W; ++q) {
-      const float* rec = g + q * stride + kShardHeader;
-      const float Pq = rec[n + r] * expf(rec[r] - M) / S;
+    for (int q = 0; q < p.world; ++q) {
+      const float Pq = shard_plane(g, n, 1, q, stride)[r] * expf(shard_plane(g, n, 0, q, stride)[r] - M) / S;
       if (Pq > 0.f) {
         if (owner < 0 && C + Pq > u) {
           owner = q; before = C; P = Pq;
@@ -426,7 +439,7 @@ shard_sample_kernel(const float* __restrict__ probs, long long n, int w, const f
     if (owner < 0) {                   // u rounded past the last cumulative mass: the last rank with mass
       owner = last; before = last_before; P = last_P;
     }
-    if (owner != rank) {               // the same decision in every thread
+    if (owner != p.rank) {             // the same decision in every thread
       if (threadIdx.x == 0) {
         draw_rec[r] = __int_as_float(-1);
         draw_rec[n + r] = 0.f;
@@ -440,7 +453,7 @@ shard_sample_kernel(const float* __restrict__ probs, long long n, int w, const f
     const float u2 = fminf((u - before) / P, 0x1.fffffep-1f);
     const int a = inverse_cdf_row(row, w, u2 * total, sh);
     if (threadIdx.x == 0) {
-      draw_rec[r] = __int_as_float(lo + a);
+      draw_rec[r] = __int_as_float(p.lo + a);
       draw_rec[n + r] = clamped_log_prob(row[a] / total * P);
     }
     __syncthreads();
@@ -484,8 +497,8 @@ __global__ void shard_pick_kernel(const float* __restrict__ g, int W, long long 
 
 static int row_grid(int64_t n) { return (int)(n < (int64_t)kNumSMs * 8 ? n : (int64_t)kNumSMs * 8); }
 
-static bool chunk_ok(const recnn_discrete_dims& d, int64_t chunk) {
-  return chunk == d.num_items || (chunk > 0 && chunk % 128 == 0 && chunk < d.num_items);
+static bool chunk_ok(int num_items, int64_t chunk) {
+  return chunk == num_items || (chunk > 0 && chunk % 128 == 0 && chunk < num_items);
 }
 
 // split-K partial floats of a weight gradient [num_items, K] computed in row blocks of `chunk` items, the last one
@@ -537,11 +550,8 @@ static DiscreteScratch discrete_carve(const recnn_discrete_dims& d, int64_t n, i
 static int discrete_hidden(const recnn_discrete_dims& d, const float* params, const float* state, int64_t n,
                            const DiscreteScratch& s, cudaStream_t st, Seg* xs_out) {
   const DiscreteLayout l = discrete_layout(d);
-  recnn_dims dd;
-  memset(&dd, 0, sizeof(dd));
-  dd.state_dim = d.state_dim; dd.hidden = d.hidden; dd.action_dim = d.num_items;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(dd, state, n, s.img, &xs, st));
+  RECNN_PROPAGATE(repitch_state(d.state_dim, state, n, s.img, &xs, st));
   if (xs_out) *xs_out = xs;
   Rng rng = {nullptr, 0, nullptr};
   return hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, d.hidden, n, false, nullptr, rng, 0, s.h, st);
@@ -713,17 +723,14 @@ __host__ __device__ __forceinline__ int64_t topk_record_floats(int64_t n, int k)
   return kShardHeader + (2 + 2 * (int64_t)k) * n;
 }
 
-__global__ void policy_topk_record_kernel(const Cand* __restrict__ run, long long n, int k, int lo, int hi, int items,
+__global__ void policy_topk_record_kernel(const Cand* __restrict__ run, long long n, int k, ShardPlan p,
                                           float* __restrict__ rec) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0) {
-    int* h = reinterpret_cast<int*>(rec);
-    h[0] = lo; h[1] = hi; h[2] = items; h[3] = (int)n;
-  }
+  if (i == 0) shard_header_write(rec, p, n);
   if (i >= n * k) return;
   const long long r = i / k, j = i % k;
   const Cand c = run[i];
-  float* planes = rec + kShardHeader + 2 * n;
+  float* planes = shard_plane(rec, n, 2);
   planes[j * n + r] = -c.key;
   planes[(k + j) * n + r] = __int_as_float(c.id == kNoId ? -1 : c.id);
 }
@@ -732,16 +739,17 @@ __global__ void policy_topk_record_kernel(const Cand* __restrict__ run, long lon
 // merge of the W sorted lists.  One warp per row, lane q reads rank q's list (W <= 32).  *flag |= 2 when the headers do
 // not tile the vocabulary with this rank's block.
 __global__ void __launch_bounds__(128)
-policy_topk_shard_finish_kernel(const float* __restrict__ g, int W, long long n, int k, int rank, int lo, int hi,
-                                int items, float* __restrict__ values, long long* __restrict__ ids, int* flag) {
+policy_topk_shard_finish_kernel(const float* __restrict__ g, long long n, int k, ShardPlan p,
+                                float* __restrict__ values, long long* __restrict__ ids, int* flag) {
   const long long stride = topk_record_floats(n, k);
-  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad_at(g, stride, W, n, rank, lo, hi, items)) atomicOr(flag, 2);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && shard_plan_bad(g, stride, p, n)) atomicOr(flag, 2);
   const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (r >= n) return;
+  const int W = p.world;
   float M, S;
   shard_merge_stats(g, stride, W, n, r, M, S);
-  const float* planes = g + (lane < W ? lane : 0) * stride + kShardHeader + 2 * n;
+  const float* planes = shard_plane(g, n, 2, lane < W ? lane : 0, stride);
   int head = 0;
   for (int i = 0; i < k; ++i) {
     float key = FLT_MAX;
@@ -847,7 +855,7 @@ extern "C" int64_t recnn_discrete_scratch_floats(const recnn_discrete_dims* d, i
 }
 
 extern "C" int64_t recnn_reinforce_scratch_floats(const recnn_discrete_dims* d, int64_t n_rows, int32_t chunk_items) {
-  if (!discrete_dims_ok(d) || n_rows <= 0 || !chunk_ok(*d, chunk_items)) return 0;
+  if (!discrete_dims_ok(d) || n_rows <= 0 || !chunk_ok(d->num_items, chunk_items)) return 0;
   return discrete_carve(*d, n_rows, chunk_items, nullptr).floats;
 }
 
@@ -888,6 +896,34 @@ extern "C" int recnn_categorical_log_prob(const float* probs, int64_t n_rows, in
   return RECNN_OK;
 }
 
+// The checks of both policy-gradient entry points after their pointers (and shard plan): the loss, rows and chunk.
+static int reinforce_check(const recnn_discrete_dims& d, int64_t n_rows, int method, int top_k,
+                           const float* beta_log_prob, int chunk_items) {
+  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || method == RECNN_REINFORCE_CORRECTED || method == RECNN_REINFORCE_TOPK,
+                "unknown REINFORCE method");
+  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || beta_log_prob, "the corrected losses need the behaviour policy's log-probs");
+  RECNN_REQUIRE(method != RECNN_REINFORCE_TOPK || top_k >= 1, "K >= 1");
+  RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
+  RECNN_REQUIRE(chunk_ok(d.num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  return RECNN_OK;
+}
+
+// After the row statistics (s.run_max, s.run_sum, s.za): the row weights, out[0] = the loss, pass 2, then the first
+// `flag_words` int32 flags of s.flags into out[1..].  items: the whole vocabulary; a_off as in reinforce_stats_pass.
+static int reinforce_finish(const recnn_discrete_dims& d, const float* params, float* grads, int64_t n,
+                            const DiscreteScratch& s, int chunk, const long long* act, long long a_off, int items,
+                            const float* beta_log_prob, const float* returns, int method, int top_k, const Seg& xs,
+                            float* out, int flag_words, cudaStream_t st) {
+  reinforce_row_weights_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(
+      n, items, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss, s.flags);
+  RECNN_CHECK_LAUNCH("reinforce_row_weights_kernel");
+  sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n, 1.f, out);
+  RECNN_CHECK_LAUNCH("sum_rows_kernel");
+  RECNN_PROPAGATE(reinforce_grad_pass(d, params, grads, n, s, chunk, act, a_off, xs, st));
+  RECNN_CHECK_CUDA(cudaMemcpyAsync(out + 1, s.flags, flag_words * sizeof(int), cudaMemcpyDeviceToDevice, st));
+  return RECNN_OK;
+}
+
 // out[0] = policy loss, out[1] = 1.0 if an action id was outside [0, num_items) (that row contributes nothing)
 extern "C" int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d, const float* params, float* grads,
                                                    const float* state, const int64_t* action, const float* beta_log_prob,
@@ -895,12 +931,7 @@ extern "C" int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d,
                                                    int32_t chunk_items, float* out, float* scratch, void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && params && grads && state && action && returns && out && scratch,
                 "null pointer / dims");
-  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || method == RECNN_REINFORCE_CORRECTED || method == RECNN_REINFORCE_TOPK,
-                "unknown REINFORCE method");
-  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || beta_log_prob, "the corrected losses need the behaviour policy's log-probs");
-  RECNN_REQUIRE(method != RECNN_REINFORCE_TOPK || top_k >= 1, "K >= 1");
-  RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
-  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_PROPAGATE(reinforce_check(*d, n_rows, method, top_k, beta_log_prob, chunk_items));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long* act = reinterpret_cast<const long long*>(action);
   const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, scratch);
@@ -908,15 +939,8 @@ extern "C" int recnn_reinforce_policy_grad_chunked(const recnn_discrete_dims* d,
   Seg xs;
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, &xs));
   RECNN_PROPAGATE(reinforce_stats_pass(*d, params, n_rows, s, chunk_items, act, 0, s.run_max, s.run_sum, s.za, st));
-  reinforce_row_weights_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
-      n_rows, d->num_items, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss,
-      s.flags);
-  RECNN_CHECK_LAUNCH("reinforce_row_weights_kernel");
-  sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n_rows, 1.f, out);
-  RECNN_CHECK_LAUNCH("sum_rows_kernel");
-  RECNN_PROPAGATE(reinforce_grad_pass(*d, params, grads, n_rows, s, chunk_items, act, 0, xs, st));
-  RECNN_CHECK_CUDA(cudaMemcpyAsync(out + 1, s.flags, sizeof(int), cudaMemcpyDeviceToDevice, st));
-  return RECNN_OK;
+  return reinforce_finish(*d, params, grads, n_rows, s, chunk_items, act, 0, d->num_items, beta_log_prob, returns,
+                          method, top_k, xs, out, 1, st);
 }
 
 extern "C" int recnn_reinforce_policy_grad(const recnn_discrete_dims* d, const float* params, float* grads,
@@ -929,17 +953,10 @@ extern "C" int recnn_reinforce_policy_grad(const recnn_discrete_dims* d, const f
 }
 
 // ---- the vocabulary-sharded policy: the phases around the two all-gathers (see the header) ----------------------
-static bool shard_ok(const recnn_discrete_dims* d, const recnn_vocab_shard* v) {
-  return v && v->world >= 1 && v->rank >= 0 && v->rank < v->world && v->item_offset >= 0 &&
-         (int64_t)v->item_offset + d->num_items <= (int64_t)v->num_items;
-}
-
 extern "C" int64_t recnn_vocab_record_floats(int64_t n_rows) { return n_rows > 0 ? shard_record_floats(n_rows) : 0; }
 
-static int shard_record_init(const recnn_discrete_dims& d, const recnn_vocab_shard& v, float* record, int64_t n,
-                             cudaStream_t st) {
-  shard_record_init_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(record, n, v.item_offset,
-                                                                      v.item_offset + d.num_items, v.num_items);
+static int shard_record_init(const ShardPlan& p, float* record, int64_t n, cudaStream_t st) {
+  shard_record_init_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(record, n, p);
   RECNN_CHECK_LAUNCH("shard_record_init_kernel");
   return RECNN_OK;
 }
@@ -948,16 +965,17 @@ extern "C" int recnn_reinforce_shard_stats(const recnn_discrete_dims* d, const r
                                            const float* state, const int64_t* action, int64_t n_rows,
                                            int32_t chunk_items, float* record, float* scratch, void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && params && state && action && record && scratch, "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
   RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
-  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, scratch);
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
-  RECNN_PROPAGATE(shard_record_init(*d, *v, record, n_rows, st));
-  float* m = record + kShardHeader;
-  return reinforce_stats_pass(*d, params, n_rows, s, chunk_items, reinterpret_cast<const long long*>(action),
-                              v->item_offset, m, m + n_rows, m + 2 * n_rows, st);
+  RECNN_PROPAGATE(shard_record_init(p, record, n_rows, st));
+  return reinforce_stats_pass(*d, params, n_rows, s, chunk_items, reinterpret_cast<const long long*>(action), p.lo,
+                              shard_plane(record, n_rows, 0), shard_plane(record, n_rows, 1),
+                              shard_plane(record, n_rows, 2), st);
 }
 
 extern "C" int recnn_reinforce_shard_grad(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
@@ -967,51 +985,38 @@ extern "C" int recnn_reinforce_shard_grad(const recnn_discrete_dims* d, const re
                                           float* out, float* scratch, void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && params && grads && state && action && returns && gathered && out && scratch,
                 "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
-  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || method == RECNN_REINFORCE_CORRECTED || method == RECNN_REINFORCE_TOPK,
-                "unknown REINFORCE method");
-  RECNN_REQUIRE(method == RECNN_REINFORCE_BASIC || beta_log_prob, "the corrected losses need the behaviour policy's log-probs");
-  RECNN_REQUIRE(method != RECNN_REINFORCE_TOPK || top_k >= 1, "K >= 1");
-  RECNN_REQUIRE(n_rows > 0, "no saved rows: select_action was never called since the last update");
-  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_PROPAGATE(reinforce_check(*d, n_rows, method, top_k, beta_log_prob, chunk_items));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long* act = reinterpret_cast<const long long*>(action);
   const DiscreteScratch s = discrete_carve(*d, n_rows, chunk_items, scratch);
   RECNN_CHECK_CUDA(cudaMemsetAsync(s.flags, 0, 4 * sizeof(int), st));
   // the stats phase left the state image (when one was needed) in s.img
-  const int S = d->state_dim;
-  const bool direct = S % 4 == 0 && aligned16(state);
-  const Seg xs = direct ? Seg{state, S, S, 0} : Seg{s.img, S, pad4(S), 0};
-  shard_merge_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
-      gathered, v->world, n_rows, v->rank, v->item_offset, v->item_offset + d->num_items, v->num_items, s.run_max,
-      s.run_sum, s.za, s.flags + 1);
+  const Seg xs = state_seg(d->state_dim, state, 0, s.img);
+  shard_merge_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(gathered, n_rows, p, s.run_max, s.run_sum, s.za,
+                                                                      s.flags + 1);
   RECNN_CHECK_LAUNCH("shard_merge_kernel");
-  reinforce_row_weights_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
-      n_rows, v->num_items, act, s.run_max, s.run_sum, s.za, beta_log_prob, returns, method, top_k, s.g, s.row_loss,
-      s.flags);
-  RECNN_CHECK_LAUNCH("reinforce_row_weights_kernel");
-  sum_rows_kernel<<<1, 1024, 0, st>>>(s.row_loss, n_rows, 1.f, out);
-  RECNN_CHECK_LAUNCH("sum_rows_kernel");
-  RECNN_PROPAGATE(reinforce_grad_pass(*d, params, grads, n_rows, s, chunk_items, act, v->item_offset, xs, st));
-  RECNN_CHECK_CUDA(cudaMemcpyAsync(out + 1, s.flags, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
-  return RECNN_OK;
+  return reinforce_finish(*d, params, grads, n_rows, s, chunk_items, act, p.lo, p.items, beta_log_prob, returns,
+                          method, top_k, xs, out, 2, st);
 }
 
 extern "C" int recnn_discrete_shard_forward(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
                                             const float* params, const float* state, int64_t n_rows, float* probs_out,
                                             float* record, float* scratch, void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && params && state && probs_out && record && scratch, "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
   RECNN_REQUIRE(n_rows > 0, "n_rows");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int I = d->num_items;
   const DiscreteScratch s = discrete_carve(*d, n_rows, 0, scratch);
   RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, s, st, nullptr));
   RECNN_PROPAGATE(discrete_logits(*d, params, n_rows, s, 0, I, probs_out, st));
-  RECNN_PROPAGATE(shard_record_init(*d, *v, record, n_rows, st));
-  float* m = record + kShardHeader;
-  logit_stats_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(probs_out, I, n_rows, I, 0, nullptr, 0, m, m + n_rows,
-                                                                nullptr);
+  RECNN_PROPAGATE(shard_record_init(p, record, n_rows, st));
+  logit_stats_kernel<<<row_grid(n_rows), kRowThreads, 0, st>>>(probs_out, I, n_rows, I, 0, nullptr, 0,
+                                                                shard_plane(record, n_rows, 0),
+                                                                shard_plane(record, n_rows, 1), nullptr);
   RECNN_CHECK_LAUNCH("logit_stats_kernel");
   return RECNN_OK;
 }
@@ -1020,10 +1025,11 @@ extern "C" int recnn_discrete_shard_finish(const recnn_discrete_dims* d, const r
                                            const float* gathered, int64_t n_rows, float* probs, int32_t* error_flag,
                                            void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && gathered && probs && error_flag, "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
   if (n_rows <= 0) return RECNN_OK;
   shard_softmax_finish_kernel<<<row_grid(n_rows), kRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      probs, n_rows, d->num_items, gathered, v->world, v->rank, v->item_offset, v->num_items, error_flag);
+      probs, n_rows, d->num_items, gathered, p, error_flag);
   RECNN_CHECK_LAUNCH("shard_softmax_finish_kernel");
   return RECNN_OK;
 }
@@ -1033,10 +1039,11 @@ extern "C" int recnn_discrete_shard_sample(const recnn_discrete_dims* d, const r
                                            const float* uniforms, uint64_t seed, int64_t draw, float* draw_record,
                                            void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && gathered && probs && draw_record, "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
   if (n_rows <= 0) return RECNN_OK;
   shard_sample_kernel<<<row_grid(n_rows), kRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      probs, n_rows, d->num_items, gathered, v->world, v->rank, v->item_offset, uniforms, seed, draw, draw_record);
+      probs, n_rows, d->num_items, gathered, p, uniforms, seed, draw, draw_record);
   RECNN_CHECK_LAUNCH("shard_sample_kernel");
   return RECNN_OK;
 }
@@ -1045,11 +1052,11 @@ extern "C" int recnn_discrete_shard_log_prob(const recnn_discrete_dims* d, const
                                              const float* probs, int64_t n_rows, const int64_t* action,
                                              float* draw_record, int32_t* oob_flag, void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && probs && action && draw_record && oob_flag, "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
   if (n_rows <= 0) return RECNN_OK;
   shard_log_prob_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      probs, n_rows, d->num_items, v->item_offset, v->num_items, reinterpret_cast<const long long*>(action),
-      draw_record, oob_flag);
+      probs, n_rows, d->num_items, p.lo, p.items, reinterpret_cast<const long long*>(action), draw_record, oob_flag);
   RECNN_CHECK_LAUNCH("shard_log_prob_kernel");
   return RECNN_OK;
 }
@@ -1066,7 +1073,7 @@ extern "C" int recnn_discrete_shard_pick(int32_t world, const float* gathered_dr
 
 // ---- the policy's top-k ----------------------------------------------------------------------------------------
 static bool topk_args_ok(const recnn_discrete_dims& d, int64_t n, int k, int chunk) {
-  return n > 0 && k >= 1 && k <= 64 && chunk_ok(d, chunk);
+  return n > 0 && k >= 1 && k <= 64 && chunk_ok(d.num_items, chunk);
 }
 
 extern "C" int64_t recnn_discrete_topk_workspace_bytes(const recnn_discrete_dims* d, int64_t n_rows, int32_t k,
@@ -1075,14 +1082,21 @@ extern "C" int64_t recnn_discrete_topk_workspace_bytes(const recnn_discrete_dims
   return topk_carve(*d, n_rows, k, chunk_items, nullptr).bytes;
 }
 
+// the rows, k and exclusion checks of every top-k entry point
+static int topk_rows_check(int64_t n_rows, int32_t k, const int64_t* exclude, int32_t n_exclude) {
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(k >= 1 && k <= 64, "1 <= k <= 64");
+  RECNN_REQUIRE(n_exclude >= 0 && n_exclude <= kMaxExclude && (n_exclude == 0 || exclude), "0 <= n_exclude <= 256");
+  return RECNN_OK;
+}
+
+// ... and those of the two that run the passes
 static int topk_check(const recnn_discrete_dims* d, const float* params, const float* state, int64_t n_rows, int32_t k,
                       const int64_t* exclude, int32_t n_exclude, int32_t chunk_items, void* workspace,
                       int64_t workspace_bytes) {
   RECNN_REQUIRE(discrete_dims_ok(d) && params && state && workspace, "null pointer / dims");
-  RECNN_REQUIRE(n_rows > 0, "n_rows");
-  RECNN_REQUIRE(k >= 1 && k <= 64, "1 <= k <= 64");
-  RECNN_REQUIRE(n_exclude >= 0 && n_exclude <= kMaxExclude && (n_exclude == 0 || exclude), "0 <= n_exclude <= 256");
-  RECNN_REQUIRE(chunk_ok(*d, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_PROPAGATE(topk_rows_check(n_rows, k, exclude, n_exclude));
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
   return check_workspace(topk_carve(*d, n_rows, k, chunk_items, nullptr).bytes, workspace_bytes);
 }
 
@@ -1117,16 +1131,16 @@ extern "C" int recnn_discrete_shard_topk(const recnn_discrete_dims* d, const rec
                                          int64_t workspace_bytes, void* stream) {
   RECNN_REQUIRE(record, "null pointer");
   RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, exclude, n_exclude, chunk_items, workspace, workspace_bytes));
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
-  RECNN_REQUIRE(k <= v->num_items, "k <= num_items (the whole vocabulary)");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(k <= p.items, "k <= num_items (the whole vocabulary)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
-  float* m = record + kShardHeader;
   const Cand* lists;
   RECNN_PROPAGATE(policy_topk_pass(*d, params, state, n_rows, k, reinterpret_cast<const long long*>(exclude),
-                                   n_exclude, chunk_items, v->item_offset, w, m, m + n_rows, &lists, st));
-  policy_topk_record_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(
-      lists, n_rows, k, v->item_offset, v->item_offset + d->num_items, v->num_items, record);
+                                   n_exclude, chunk_items, p.lo, w, shard_plane(record, n_rows, 0),
+                                   shard_plane(record, n_rows, 1), &lists, st));
+  policy_topk_record_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(lists, n_rows, k, p, record);
   RECNN_CHECK_LAUNCH("policy_topk_record_kernel");
   return RECNN_OK;
 }
@@ -1136,17 +1150,16 @@ extern "C" int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, co
                                                 const int64_t* exclude, int32_t n_exclude, float* values_out,
                                                 int64_t* ids_out, int32_t* error_flag, void* stream) {
   RECNN_REQUIRE(discrete_dims_ok(d) && gathered && values_out && ids_out && error_flag, "null pointer / dims");
-  RECNN_REQUIRE(shard_ok(d, v), "shard: rank / world / item_offset + num_items outside the vocabulary");
-  RECNN_REQUIRE(v->world <= 32, "world <= 32");
-  RECNN_REQUIRE(n_rows > 0 && k >= 1 && k <= 64, "n_rows / k");
-  RECNN_REQUIRE(n_exclude >= 0 && n_exclude <= kMaxExclude && (n_exclude == 0 || exclude), "0 <= n_exclude <= 256");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(p.world <= 32, "world <= 32");
+  RECNN_PROPAGATE(topk_rows_check(n_rows, k, exclude, n_exclude));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
-  RECNN_PROPAGATE(exclude_check(reinterpret_cast<const long long*>(exclude), n_rows, n_exclude, v->num_items,
-                                error_flag, st));
+  RECNN_PROPAGATE(exclude_check(reinterpret_cast<const long long*>(exclude), n_rows, n_exclude, p.items, error_flag,
+                                st));
   policy_topk_shard_finish_kernel<<<(unsigned)ceil_div(n_rows, 4), 128, 0, st>>>(
-      gathered, v->world, n_rows, k, v->rank, v->item_offset, v->item_offset + d->num_items, v->num_items, values_out,
-      reinterpret_cast<long long*>(ids_out), error_flag);
+      gathered, n_rows, k, p, values_out, reinterpret_cast<long long*>(ids_out), error_flag);
   RECNN_CHECK_LAUNCH("policy_topk_shard_finish_kernel");
   return RECNN_OK;
 }

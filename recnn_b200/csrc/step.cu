@@ -852,9 +852,8 @@ static Seg state_seg(int S, const float* state, long long ld, float* img) {
   return Seg{img, S, pad4(S), 0};
 }
 
-static int repitch_state(const recnn_dims& d, const float* state, int64_t n, float* img, Seg* out, cudaStream_t st,
+static int repitch_state(int S, const float* state, int64_t n, float* img, Seg* out, cudaStream_t st,
                          long long ld = 0) {
-  const int S = d.state_dim;
   *out = state_seg(S, state, ld, img);
   if (out->p == state) return RECNN_OK;
   RECNN_CHECK_CUDA(cudaMemcpy2DAsync(img, (size_t)out->ld * 4, state, (size_t)(ld == 0 ? S : ld) * 4, (size_t)S * 4, n,
@@ -875,7 +874,7 @@ extern "C" int recnn_actor_forward(const recnn_dims* d, const float* params, con
   Rng rng = {nullptr, 0, nullptr};
   const bool train = mask1 != nullptr;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, s.img, &xs, st));
+  RECNN_PROPAGATE(repitch_state(d->state_dim, state, n_rows, s.img, &xs, st));
   const Seg s1 = {s.h1, H, H, 0}, s2 = {s.h2, H, H, 0};
   RECNN_PROPAGATE(hidden_layer(xs, kNoSeg, params + l.w1, l.ld1, params + l.b1, H, n_rows, train, mask1, rng, 0, s.h1, st));
   RECNN_PROPAGATE(hidden_layer(s1, kNoSeg, params + l.w2, l.ld2, params + l.b2, H, n_rows, train, mask2, rng, 1, s.h2, st));
@@ -896,7 +895,7 @@ extern "C" int recnn_critic_forward(const recnn_dims* d, const float* params, co
   Rng rng = {nullptr, 0, nullptr};
   const bool train = mask1 != nullptr;
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(*d, state, n_rows, s.img, &xs, st));
+  RECNN_PROPAGATE(repitch_state(S, state, n_rows, s.img, &xs, st));
   // the action block starts at weight column S: with S % 4 != 0 it needs `lead` zero columns in front (see Seg)
   const int lead = S % 4, ldA = pad4(A + lead);
   Seg xa = {action, A, A, 0};

@@ -87,7 +87,7 @@ def _policy_loss(policy, returns, method):
                 ret_rows.data_ptr(), n, method, K, chunk, gathered.data_ptr(), out.data_ptr(), scratch.data_ptr(),
                 _lib.stream_ptr(dev)))
             from ...dist import layer1_floats
-            vp.comm.all_reduce(grads[:layer1_floats(d)])
+            vp.all_reduce(grads[:layer1_floats(d)])
     flags = out.view(torch.int32)[1:].tolist()
     if flags[1] != 0:
         raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the saved rows")
