@@ -191,12 +191,53 @@ class VocabParallel:
         return self
 
 
+def _item_axes(net):
+    """Per parameter of ``net`` (arena order), the (axis, first) of its item coordinate -- item j sits at index
+    first + j of that axis -- or None when the parameter is replicated over the ranks: rows of the policy's linear2
+    and of β's net.0, the action columns of a critic's linear1 (after its S state columns)."""
+    from .nn.arena import _is_beta, _is_discrete
+    if _is_beta(net):
+        return [(0, 0), (0, 0)]
+    if _is_discrete(net):
+        return [None, None, (0, 0), (0, 0)]
+    return [(1, net.linear1.in_features - net._action_dim)] + [None] * 5
+
+
+def _item_part(t, ax, lo, n):
+    """Items [lo, lo + n) of ``t`` along its item axis ``ax`` (a view)."""
+    return t.narrow(ax[0], ax[1] + lo, n)
+
+
+def _shared_part(t, ax):
+    """The replicated part of ``t`` (a view): all of it, the critic's state columns, or None."""
+    if ax is None:
+        return t
+    return t.narrow(ax[0], 0, ax[1]) if ax[1] else None
+
+
+def _block(t, ax, lo, hi):
+    """What the rank holding items [lo, hi) keeps of the full tensor ``t``: a new contiguous tensor (``t`` itself when
+    it is replicated)."""
+    if ax is None:
+        return t
+    shared = _shared_part(t, ax)
+    item = _item_part(t, ax, lo, hi - lo)
+    return item.clone(memory_format=torch.contiguous_format) if shared is None else torch.cat([shared, item], ax[0])
+
+
+def _shard_params(net, lo, hi):
+    """Replace every sharded parameter of ``net`` by its block [lo, hi) (the module's features are the caller's)."""
+    from .nn.arena import _params
+    with torch.no_grad():
+        for p, ax in zip(_params(net), _item_axes(net)):
+            if ax is not None:
+                p.grad = None
+                p.data = _block(p.data, ax, lo, hi)
+
+
 def _shard_policy_rows(policy, lo, hi):
     from .nn.arena import grad_arena
-    with torch.no_grad():
-        for p in (policy.linear2.weight, policy.linear2.bias):
-            p.grad = None
-            p.data = p.data[lo:hi].clone()
+    _shard_params(policy, lo, hi)
     policy.linear2.out_features = hi - lo
     policy.__dict__.pop("_recnn_engines", None)
     grad_arena(policy)                                  # the local arenas (param_arena rebuilds on the new shapes)
@@ -206,11 +247,8 @@ def _shard_critic_columns(critic, lo, hi):
     """Keep the state block of linear1 and the action columns [lo, hi): a Critic(S, hi - lo, H)."""
     from .nn.arena import grad_arena
     S = critic.linear1.in_features - critic._action_dim
-    with torch.no_grad():
-        w = critic.linear1.weight
-        w.grad = None
-        w.data = torch.cat([w.data[:, :S], w.data[:, S + lo:S + hi]], 1).contiguous()
-        critic.linear1.bias.grad = None
+    _shard_params(critic, lo, hi)
+    critic.linear1.bias.grad = None
     critic.linear1.in_features = S + hi - lo
     critic._action_dim = hi - lo
     critic.__dict__.pop("_recnn_ids_steps", None)
@@ -282,12 +320,8 @@ def _shard_beta_rows(beta, lo, hi):
     """Keep rows [lo, hi) of net.0 (weight and bias) and rebuild the built-in optimizer on the local arenas."""
     from . import optim as _optim
     from .nn.arena import grad_arena
-    lin = beta.net[0]
-    with torch.no_grad():
-        for p in (lin.weight, lin.bias):
-            p.grad = None
-            p.data = p.data[lo:hi].clone()
-    lin.out_features = hi - lo
+    _shard_params(beta, lo, hi)
+    beta.net[0].out_features = hi - lo
     beta._workspace = None
     grad_arena(beta)
     opt = beta.optim
@@ -405,3 +439,382 @@ def enable_vocab_parallel(policy_or_agent, group=None, beta=None):
     if agent is not None and getattr(agent, "optimizers", None):
         _rebuild_optimizers(agent.optimizers, nets)
     return policy_or_agent
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Full checkpoints of vocabulary-parallel nets.  A sharded net's arenas hold the rank's block; a checkpoint holds what
+# the unsharded net would: the reference's state_dict keys and shapes, and the built-in optimizers' arenas in the full
+# arena's geometry.  Every tensor is converted per parameter (arena._views on the local and on the full geometry),
+# since the critic's layer-1 pitch is pad4(S + hi - lo) locally and pad4(S + num_items) in full.  Each tensor has a
+# replicated part (taken from one rank) and an item part (rank r's items [lo_r, hi_r)), moved in row slices of at most
+# _SLICE_FLOATS floats, so no device holds more than its arenas and one slice beyond them.
+_SLICE_FLOATS = (256 << 20) // 4
+
+
+def _slices(t):
+    """Views of ``t`` over consecutive ranges of its first axis, at most _SLICE_FLOATS elements each (one row at
+    least)."""
+    rows = t.shape[0]
+    per = max(1, _SLICE_FLOATS // max(1, t[0].numel() if rows else 1))
+    for r in range(0, rows, per):
+        yield t.narrow(0, r, min(per, rows - r))
+
+
+def _copy_sliced(dst, src):
+    """``dst.copy_(src)`` one slice at a time: a copy between host and device stages at most one slice."""
+    for d, s in zip(_slices(dst), _slices(src)):
+        d.copy_(s)
+
+
+class _Leaf:
+    """One tensor of a checkpoint: the rank's local tensor, the full tensor (on the gathering rank; None elsewhere) and
+    the item axis of its parameter (None: replicated)."""
+    __slots__ = ("local", "full", "ax")
+
+    def __init__(self, local, full, ax):
+        self.local, self.full, self.ax = local, full, ax
+
+
+def _outbox(leaves, n):
+    """Sender half: the rank's item parts (``n`` = hi - lo items) as contiguous slices, in leaf order."""
+    for leaf in leaves:
+        if leaf.ax is not None:
+            for s in _slices(_item_part(leaf.local, leaf.ax, 0, n)):
+                yield s.contiguous()
+
+
+def _inbox(leaves, lo, hi):
+    """Receiver half: the full tensors' views rank [lo, hi)'s slices land in, in _outbox's order and shapes."""
+    for leaf in leaves:
+        if leaf.ax is not None:
+            yield from _slices(_item_part(leaf.full, leaf.ax, lo, hi - lo))
+
+
+def _copy_shared(leaves):
+    """The gathering rank's replicated parts into the full tensors."""
+    for leaf in leaves:
+        shared = _shared_part(leaf.local, leaf.ax)
+        if shared is not None:
+            _copy_sliced(_shared_part(leaf.full, leaf.ax), shared)
+
+
+def _load_leaves(locals_, fulls, axes, lo, hi):
+    """Full -> local: each local tensor takes its replicated part whole and items [lo, hi) of the full tensor."""
+    for local, full, ax in zip(locals_, fulls, axes):
+        shared = _shared_part(local, ax)
+        if shared is not None:
+            _copy_sliced(shared, _shared_part(full, ax))
+        if ax is not None:
+            _copy_sliced(_item_part(local, ax, 0, hi - lo), _item_part(full, ax, lo, hi - lo))
+
+
+def _full_twin(net, num_items):
+    """A parameter-less (meta) net of ``net``'s class with all ``num_items`` items: the full geometry."""
+    from .nn.arena import _is_beta, _is_discrete
+    from .nn import models
+    from .nn.beta import Beta
+    with torch.device("meta"):
+        if _is_beta(net):
+            return Beta(net.net[0].in_features, num_items)
+        if _is_discrete(net):
+            return models.DiscreteActor(net.linear1.in_features, num_items, net.linear1.out_features)
+        return models.Critic(net.linear1.in_features - net._action_dim, num_items, net.linear1.out_features)
+
+
+def _checkpoint_parts(agent_or_policy, beta):
+    """({name: net} of every sharded net, β included as "beta", {key: optimizer} of an agent or None, VocabParallel).
+    Raises unless every net is vocabulary-parallel on the policy's plan."""
+    from .nn.arena import _is_beta, _is_discrete
+    agent = agent_or_policy if hasattr(agent_or_policy, "nets") else None
+    if agent is not None or isinstance(agent_or_policy, dict):
+        src = agent.nets if agent is not None else agent_or_policy
+        missing = [k for k in _AGENT_NETS if src.get(k) is None]
+        if missing:
+            raise ValueError("a REINFORCE agent's nets need %s" % ", ".join(missing))
+        nets = {k: src[k] for k in _AGENT_NETS}
+    elif _is_beta(agent_or_policy) or not _is_discrete(agent_or_policy):
+        raise TypeError("a vocabulary-parallel checkpoint is of a DiscreteActor or a REINFORCE agent")
+    else:
+        nets = {"policy_net": agent_or_policy}
+    if beta is not None:
+        if not _is_beta(beta):
+            raise TypeError("beta must be a recnn_b200.nn.Beta (got %s)" % type(beta).__name__)
+        nets["beta"] = beta
+    vp = nets["policy_net"].__dict__.get("_recnn_vp")
+    for name, net in nets.items():
+        if vp is None or net.__dict__.get("_recnn_vp") is not vp:
+            raise RuntimeError("%s is not vocabulary-parallel with the policy: call enable_vocab_parallel first"
+                               % (name if name == "beta" else "nets[%r]" % name))
+    optimizers = None
+    if agent is not None:
+        optimizers = {k: o for k, o in (getattr(agent, "optimizers", None) or {}).items() if o is not None}
+    return nets, optimizers, vp
+
+
+def _owners(nets):
+    """{id(parameter): (net name, index in the arena order)}."""
+    from .nn.arena import _params
+    return {id(p): (name, i) for name, net in nets.items() for i, p in enumerate(_params(net))}
+
+
+def _opt_params(opt):
+    return [p for g in opt.param_groups for p in g["params"]]
+
+
+def _arena_owner(opt, owners, label):
+    """The net name whose whole arena a built-in optimizer steps."""
+    name = owners.get(id(opt.param_groups[0]["params"][0]), (None,))[0]
+    if name is None:
+        raise ValueError("%s does not step one of the nets" % label)
+    return name
+
+
+def _scalar(v):
+    return float(v) if torch.is_tensor(v) and v.numel() == 1 else (repr(v) if torch.is_tensor(v) else v)
+
+
+def _gather_begin(nets, optimizers, num_items, gathering):
+    """Every rank: the checkpoint's leaves in one order (local tensors; full host tensors on the gathering rank), the
+    scalar state the ranks must agree on, and the checkpoint that the transport fills (None on the other ranks)."""
+    from collections import OrderedDict
+    from . import optim as _optim
+    from .nn.arena import _params, _views, net_layout, param_arena
+    twins = {name: _full_twin(net, num_items) for name, net in nets.items()}
+    owners = _owners(nets)
+    leaves, agree = [], []
+
+    def arena(name, flat):
+        net, twin = nets[name], twins[name]
+        full = torch.zeros(net_layout(twin)[2], dtype=torch.float32) if gathering else None
+        fulls = _views(full, twin) if gathering else [None] * len(_params(net))
+        leaves.extend(_Leaf(l, f, ax) for l, f, ax in zip(_views(flat, net), fulls, _item_axes(net)))
+        return full
+
+    def net_state(name):
+        full = arena(name, param_arena(nets[name]))
+        if gathering:
+            keys = [k for k, _ in twins[name].named_parameters()]
+            return OrderedDict(zip(keys, _views(full, twins[name])))
+
+    def opt_state(label, opt):
+        if isinstance(opt, _optim._ArenaOptimizer):
+            name = _arena_owner(opt, owners, label)
+            sd = torch.optim.Optimizer.state_dict(opt) if gathering else None
+            t = None if opt._t is None else int(opt._t.item())
+            agree.append((label, "t", t))
+            if t is not None:
+                arenas = {k: None if getattr(opt, "_" + k) is None else arena(name, getattr(opt, "_" + k))
+                          for k in ("m", "v", "slow")}
+                if gathering:
+                    sd["recnn_arenas"] = dict(arenas, t=t)
+            return sd
+        sd = opt.state_dict()
+        params = _opt_params(opt)
+        state = {}
+        for idx in sorted(sd["state"]):
+            if id(params[idx]) not in owners:
+                raise ValueError("%s steps a parameter outside the nets" % label)
+            name, i = owners[id(params[idx])]
+            ax, full_shape = _item_axes(nets[name])[i], _params(twins[name])[i].shape
+            entry = {}
+            for k, v in sd["state"][idx].items():
+                if torch.is_tensor(v) and v.dim() > 0 and v.shape == params[idx].shape:
+                    entry[k] = torch.zeros(full_shape, dtype=v.dtype) if gathering else None
+                    leaves.append(_Leaf(v.detach(), entry[k], ax))
+                    agree.append((label, idx, k, "block"))
+                else:
+                    entry[k] = v.detach().cpu().clone() if torch.is_tensor(v) else v
+                    agree.append((label, idx, k, _scalar(v)))
+            state[idx] = entry
+        return {"state": state, "param_groups": sd["param_groups"]} if gathering else None
+
+    out = {"nets": {name: net_state(name) for name in nets if name != "beta"}}
+    if optimizers is not None:
+        out["optimizers"] = {k: opt_state("optimizers[%r]" % k, optimizers[k]) for k in sorted(optimizers)}
+    if "beta" in nets:
+        out["beta"] = {"net": net_state("beta"), "optim": opt_state("beta.optim", nets["beta"].optim)}
+    return leaves, agree, (out if gathering else None)
+
+
+def gather_vocab_parallel_state(agent_or_policy, beta=None, dst=0):
+    """The full checkpoint of a vocabulary-parallel DiscreteActor or REINFORCE agent (and ``beta``), on rank ``dst``
+    of the policy's group; None on the other ranks.  A collective: call it on every rank.
+
+    The checkpoint is what the unsharded nets would give, in host memory (CPU tensors)::
+
+        {"nets": {name: net.state_dict()}, "optimizers": {key: opt.state_dict()},
+         "beta": {"net": beta.state_dict(), "optim": beta.optim.state_dict()}}
+
+    with only the parts passed in (a lone policy is ``nets["policy_net"]``; "optimizers" comes with an agent).  Net
+    keys and shapes are the reference's.  Built-in optimizers' ``recnn_arenas`` have the full arena's geometry (pads
+    zero); a torch optimizer's per-parameter state (``exp_avg``, ...) is gathered along the item axis.  Replicated
+    parameters and their state are rank ``dst``'s.  The ranks must hold the same step counts and scalar optimizer
+    state, else every rank raises RuntimeError.  Take it after a policy update: rows saved for the next one (``_saved``,
+    rewards) are not part of it, nor are the agent's step and the policy's draw counter, as for the unsharded
+    ``state_dict``.  The item blocks travel by point-to-point sends in slices of at most 256 MB."""
+    nets, optimizers, vp = _checkpoint_parts(agent_or_policy, beta)
+    if not 0 <= dst < vp.world:
+        raise ValueError("dst %d is not a rank of the policy's group of %d" % (dst, vp.world))
+    gathering = vp.rank == dst
+    leaves, agree, out = _gather_begin(nets, optimizers, vp.num_items, gathering)
+    everyone = [None] * vp.world
+    dist.all_gather_object(everyone, agree, group=vp.group)
+    if any(a != everyone[0] for a in everyone):
+        bad = next(q for q, a in enumerate(everyone) if a != everyone[0])
+        raise RuntimeError("the ranks' optimizer states disagree (step counts or scalar state): rank 0 holds %s, rank "
+                           "%d holds %s" % (everyone[0], bad, everyone[bad]))
+    if gathering:
+        _copy_shared(leaves)
+    # each slice is released before the next one is made, one slice on the device at a time (not zip: its reused
+    # result tuple would hold the previous slice while the next one is made)
+    for q in range(vp.world):
+        if q == vp.rank == dst:
+            mine = _outbox(leaves, vp.hi - vp.lo)
+            for v in _inbox(leaves, vp.lo, vp.hi):
+                v.copy_(next(mine))
+        elif q == vp.rank:
+            for s in _outbox(leaves, vp.hi - vp.lo):
+                dist.send(s, group=vp.group, group_dst=dst)
+                if s.is_cuda:
+                    torch.cuda.current_stream(s.device).synchronize()
+                del s
+        elif gathering:
+            lo, hi = vocab_shard(vp.num_items, q, vp.world)
+            dev = leaves[0].local.device
+            for v in _inbox(leaves, lo, hi):
+                buf = torch.empty(v.shape, dtype=v.dtype, device=dev)
+                dist.recv(buf, group=vp.group, group_src=q)
+                v.copy_(buf)
+                del buf
+    return out
+
+
+def _load_refusal(nets, optimizers, state, num_items):
+    """Why ``state`` cannot be loaded into these nets and optimizers, or None."""
+    from . import optim as _optim
+    from .nn.arena import net_layout
+    if not isinstance(state, dict) or not isinstance(state.get("nets"), dict):
+        return "the checkpoint has no 'nets' dict"
+    sections = {name: (("beta", "net") if name == "beta" else ("nets", name)) for name in nets}
+    twins = {name: _full_twin(net, num_items) for name, net in nets.items()}
+    owners = _owners(nets)
+
+    def entry(path):
+        d = state
+        for k in path:
+            if not isinstance(d, dict) or d.get(k) is None:
+                return None
+            d = d[k]
+        return d
+
+    for name in nets:
+        sd = entry(sections[name])
+        if sd is None:
+            return "the checkpoint has no state[%s]" % "][".join(map(repr, sections[name]))
+        for k, p in twins[name].named_parameters():
+            if not torch.is_tensor(sd.get(k)) or tuple(sd[k].shape) != tuple(p.shape):
+                return ("state[%s][%r] is %s; the nets need %s (their state_dim, hidden size and num_items)"
+                        % ("][".join(map(repr, sections[name])), k,
+                           tuple(sd[k].shape) if torch.is_tensor(sd.get(k)) else "missing", tuple(p.shape)))
+    opts = [(("optimizers", k), v) for k, v in sorted((optimizers or {}).items())]
+    if "beta" in nets:
+        opts.append((("beta", "optim"), nets["beta"].optim))
+    for path, opt in opts:
+        label = "state[%s]" % "][".join(map(repr, path))
+        sd = entry(path)
+        if sd is None:
+            return "the checkpoint has no %s" % label
+        groups = sd.get("param_groups")
+        if (not isinstance(groups, list) or len(groups) != len(opt.param_groups)
+                or any(len(g["params"]) != len(o["params"]) for g, o in zip(groups, opt.param_groups))):
+            return "%s has other parameter groups than the optimizer" % label
+        arenas = sd.get("recnn_arenas")
+        if isinstance(opt, _optim._ArenaOptimizer):
+            if sd.get("state"):
+                return "%s is a torch optimizer's state; the optimizer is a built-in %s" % (label, type(opt).__name__)
+            if arenas is None:
+                continue
+            name = _arena_owner(opt, owners, label)
+            need = {"m": True, "v": opt._recnn_kind in (_lib.OPT_ADAM, _lib.OPT_RANGER, _lib.OPT_RADAM),
+                    "slow": opt._recnn_kind == _lib.OPT_RANGER}
+            have = {k: arenas.get(k) is not None for k in need}
+            if have != need:
+                return ("%s holds the arenas %s, a %s needs %s" % (label, sorted(k for k in have if have[k]),
+                                                                   type(opt).__name__,
+                                                                   sorted(k for k in need if need[k])))
+            count = net_layout(twins[name])[2]
+            for k in need:
+                if need[k] and arenas[k].numel() != count:
+                    return "%s['recnn_arenas'][%r] has %d floats, the full arena %d" % (label, k, arenas[k].numel(),
+                                                                                         count)
+            if not isinstance(arenas.get("t"), int):
+                return "%s['recnn_arenas'] has no step count" % label
+        else:
+            if arenas is not None:
+                return "%s holds a built-in optimizer's arenas; the optimizer is a %s" % (label, type(opt).__name__)
+            params = _opt_params(opt)
+            for idx, st in (sd.get("state") or {}).items():
+                if not isinstance(idx, int) or not 0 <= idx < len(params) or id(params[idx]) not in owners:
+                    return "%s has state for parameter %r, which the optimizer does not step" % (label, idx)
+                name, i = owners[id(params[idx])]
+                full = tuple(list(twins[name].parameters())[i].shape)
+                for k, v in st.items():
+                    if torch.is_tensor(v) and v.dim() > 0 and tuple(v.shape) != full:
+                        return "%s['state'][%d][%r] is %s; the parameter is %s" % (label, idx, k, tuple(v.shape),
+                                                                                  full)
+    return None
+
+
+def load_vocab_parallel_state(agent_or_policy, state, beta=None):
+    """Load a full checkpoint -- from gather_vocab_parallel_state, or an unsharded agent's own ``state_dict()``s in the
+    same layout -- into a vocabulary-parallel DiscreteActor or REINFORCE agent (and ``beta``), at any world size.  Call
+    it on every rank after enable_vocab_parallel, each with the whole ``state``.  Each rank takes its block [lo, hi) of
+    every sharded tensor and the replicated parts whole; built-in optimizers get their arenas in the local geometry and
+    their step count, torch optimizers their per-parameter state sliced the same way.  A checkpoint whose nets'
+    state_dim, hidden size or num_items differ from these nets', that lacks a net or an optimizer, or whose optimizer
+    state is of another kind (Ranger arenas into an Adam, a torch optimizer's state into a built-in one, ...) is refused
+    on every rank (ValueError) before anything is loaded."""
+    from . import optim as _optim
+    from .nn.arena import _params, _views, param_arena
+    nets, optimizers, vp = _checkpoint_parts(agent_or_policy, beta)
+    err = _load_refusal(nets, optimizers, state, vp.num_items)
+    everyone = [None] * vp.world
+    dist.all_gather_object(everyone, err, group=vp.group)
+    bad = [(q, e) for q, e in enumerate(everyone) if e]
+    if bad:
+        raise ValueError("rank %d refuses the checkpoint: %s" % bad[0])
+    lo, hi = vp.lo, vp.hi
+    twins = {name: _full_twin(net, vp.num_items) for name, net in nets.items()}
+    owners = _owners(nets)
+    with torch.no_grad():
+        for name, net in nets.items():
+            sd = state["beta"]["net"] if name == "beta" else state["nets"][name]
+            fulls = [sd[k] for k, _ in twins[name].named_parameters()]
+            _load_leaves(_views(param_arena(net), net), fulls, _item_axes(net), lo, hi)
+        opts = [(optimizers[k], state["optimizers"][k]) for k in sorted(optimizers or {})]
+        if "beta" in nets:
+            opts.append((nets["beta"].optim, state["beta"]["optim"]))
+        for opt, sd in opts:
+            if isinstance(opt, _optim._ArenaOptimizer):
+                arenas = sd.get("recnn_arenas")
+                opt.load_state_dict({k: v for k, v in sd.items() if k != "recnn_arenas"})
+                if arenas is None:
+                    continue
+                name = _arena_owner(opt, owners, "")
+                net = nets[name]
+                opt._state_arenas(param_arena(net))
+                for k in ("m", "v", "slow"):
+                    local = getattr(opt, "_" + k)
+                    if local is not None:
+                        _load_leaves(_views(local, net), _views(arenas[k], twins[name]), _item_axes(net), lo, hi)
+                opt._t.fill_(int(arenas["t"]))
+                continue
+            params = _opt_params(opt)
+            local = {}
+            for idx, st in sd["state"].items():
+                name, i = owners[id(params[idx])]
+                ax = _item_axes(nets[name])[i]
+                local[idx] = {k: _block(v, ax, lo, hi) if torch.is_tensor(v) and v.dim() > 0 else v
+                              for k, v in st.items()}
+            opt.load_state_dict({"state": local, "param_groups": sd["param_groups"]})
+    return agent_or_policy
