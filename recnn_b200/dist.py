@@ -301,11 +301,8 @@ def _rebuild_optimizers(optimizers, nets):
 
 
 def _beta_refusal(beta, S, num_items):
-    """Why ``beta`` cannot be sharded with a policy of state_dim S over num_items items, or None (checked on every rank
-    before any exchange)."""
-    from .nn.arena import _is_beta
-    if not _is_beta(beta):
-        return TypeError("beta must be a recnn_b200.nn.Beta (got %s)" % type(beta).__name__)
+    """Why the Beta ``beta`` cannot be sharded with a policy of state_dim S over num_items items, or None (checked on
+    every rank before any exchange)."""
     if "_recnn_vp" in beta.__dict__:
         return RuntimeError("beta is already vocabulary-parallel")
     lin = beta.net[0]
@@ -360,27 +357,18 @@ def enable_vocab_parallel(policy_or_agent, group=None, beta=None):
     Every rank must be fed the same batches and states, seeded the same (torch.manual_seed, or the same
     ``uniform_source``) and must make the same calls in the same order: dropout masks -- given in the batch or drawn --
     and the masks of reinforce_update's reward line must agree across ranks."""
-    from .nn.arena import _is_discrete, _is_beta
+    from .nn.arena import _is_beta, _is_discrete
     if not dist.is_initialized():
         raise RuntimeError("torch.distributed is not initialised")
-    agent = policy_or_agent if hasattr(policy_or_agent, "nets") else None
-    if agent is not None or isinstance(policy_or_agent, dict):
-        nets = agent.nets if agent is not None else policy_or_agent
-        missing = [k for k in _AGENT_NETS if nets.get(k) is None]
-        if missing:
-            raise ValueError("a REINFORCE agent's nets need %s" % ", ".join(missing))
-        policy = nets["policy_net"]
-    else:
-        nets, policy = None, policy_or_agent
-    if _is_beta(policy) or not _is_discrete(policy):
-        raise TypeError("enable_vocab_parallel shards a DiscreteActor")
-    shard_nets = {"policy_net": policy} if nets is None else {k: nets[k] for k in _AGENT_NETS}
-    for name, net in shard_nets.items():
+    agent, nets = _vocab_nets(policy_or_agent, beta, "enable_vocab_parallel shards a DiscreteActor")
+    lone = "value_net" not in nets
+    policy = nets["policy_net"]
+    for name, net in nets.items():
         if "_recnn_vp" in net.__dict__:
-            raise RuntimeError("the policy is already vocabulary-parallel" if nets is None
+            raise RuntimeError("the policy is already vocabulary-parallel" if lone
                                else "nets[%r] is already vocabulary-parallel" % name)
     S, num_items = policy.linear1.in_features, policy.linear2.out_features
-    if nets is not None:
+    if not lone:
         # refused on this rank before any exchange; the shape exchange below makes every rank refuse together
         tp = nets["target_policy_net"]
         if (_is_beta(tp) or not _is_discrete(tp) or tp.linear2.weight.shape != policy.linear2.weight.shape
@@ -399,17 +387,16 @@ def enable_vocab_parallel(policy_or_agent, group=None, beta=None):
     arena = param_arena(policy)
     if not arena.is_cuda:
         raise _lib.RecnnError("enable_vocab_parallel needs the policy on its CUDA device")
-    if nets is not None:
-        for name, net in shard_nets.items():
-            if param_arena(net).device != arena.device:
-                raise _lib.RecnnError("nets[%r] is on %s, the policy on %s" % (name, param_arena(net).device,
-                                                                               arena.device))
+    for name, net in nets.items():
+        if param_arena(net).device != arena.device:
+            raise _lib.RecnnError("nets[%r] is on %s, the policy on %s" % (name, param_arena(net).device,
+                                                                           arena.device))
     if beta is not None and param_arena(beta).device != arena.device:
         raise ValueError("beta is on %s, the policy on %s" % (param_arena(beta).device, arena.device))
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     # every rank checks every rank's plan, so a refused plan raises on all of them (none is left in a collective)
     shape = (S, policy.linear1.out_features, num_items)
-    if nets is not None:
+    if not lone:
         shape += (tuple(nets["value_net"].linear1.weight.shape),)
     if beta is not None:
         shape += (("beta",) + tuple(beta.net[0].weight.shape),)
@@ -420,25 +407,58 @@ def enable_vocab_parallel(policy_or_agent, group=None, beta=None):
     plans = [vocab_shard(num_items, r, world) + (num_items,) for r in range(world)]
     check_vocab_plans(plans)
     lo, hi, _ = plans[rank]
-    broadcast_nets(shard_nets, group)
-    for name, net in shard_nets.items():
-        if name.endswith("policy_net"):
-            _shard_policy_rows(net, lo, hi)
-        else:
-            _shard_critic_columns(net, lo, hi)
+    # the communicator first: a peer mapping that fails leaves the nets as they were (its size is the layer-1 block's,
+    # which sharding does not change)
     comm = PeerComm(group, arena.device, vocab_comm_floats(policy.dims, world, 1))
-    vp = VocabParallel(lo, hi, num_items, group, rank, world, comm)
-    for net in shard_nets.values():
+    broadcast_nets(nets, group)
+    if beta is not None:
+        dist.broadcast(param_arena(beta), src=0, group=group)
+    shard_in_place(nets, VocabParallel(lo, hi, num_items, group, rank, world, comm), beta,
+                   getattr(agent, "optimizers", None))
+    return policy_or_agent
+
+
+def _vocab_nets(policy_or_agent, beta, refusal):
+    """(the agent or None, {name: net}) of what enable_vocab_parallel and the checkpoint functions take: a lone
+    DiscreteActor as "policy_net", or an agent's (or nets dict's) policy_net, target_policy_net, value_net and
+    target_value_net.  Raises ValueError when an agent lacks one of them, TypeError(``refusal``) when the policy is not
+    a DiscreteActor, TypeError when ``beta`` is given and is not a Beta."""
+    from .nn.arena import _is_beta, _is_discrete
+    agent = policy_or_agent if hasattr(policy_or_agent, "nets") else None
+    if agent is not None or isinstance(policy_or_agent, dict):
+        src = agent.nets if agent is not None else policy_or_agent
+        missing = [k for k in _AGENT_NETS if src.get(k) is None]
+        if missing:
+            raise ValueError("a REINFORCE agent's nets need %s" % ", ".join(missing))
+        nets = {k: src[k] for k in _AGENT_NETS}
+    else:
+        nets = {"policy_net": policy_or_agent}
+    if _is_beta(nets["policy_net"]) or not _is_discrete(nets["policy_net"]):
+        raise TypeError(refusal)
+    if beta is not None and not _is_beta(beta):
+        raise TypeError("beta must be a recnn_b200.nn.Beta (got %s)" % type(beta).__name__)
+    return agent, nets
+
+
+def shard_in_place(nets, vp, beta=None, optimizers=None):
+    """The local half of enable_vocab_parallel, with no exchange: shard ``nets`` ({name: net}: DiscreteActors under
+    names ending in "policy_net", Critic(S, num_items, H)s otherwise) and ``beta`` to the block [vp.lo, vp.hi) of the
+    VocabParallel ``vp`` and record ``vp`` on each.  ``optimizers`` ({key: optimizer} of those nets, or None): built-in
+    ones are rebuilt on the local arenas (see enable_vocab_parallel).  The nets must hold full, identical weights on
+    every rank."""
+    for name, net in nets.items():
+        if name.endswith("policy_net"):
+            _shard_policy_rows(net, vp.lo, vp.hi)
+        else:
+            _shard_critic_columns(net, vp.lo, vp.hi)
         net.__dict__["_recnn_vp"] = vp
     if beta is not None:
         from .nn import beta as _beta
-        dist.broadcast(param_arena(beta), src=0, group=group)
-        _shard_beta_rows(beta, lo, hi)
+        _shard_beta_rows(beta, vp.lo, vp.hi)
         beta.__dict__["_recnn_vp"] = vp
         _beta._SHARDED.add(beta)
-    if agent is not None and getattr(agent, "optimizers", None):
-        _rebuild_optimizers(agent.optimizers, nets)
-    return policy_or_agent
+    if optimizers:
+        _rebuild_optimizers(optimizers, nets)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -524,21 +544,9 @@ def _full_twin(net, num_items):
 def _checkpoint_parts(agent_or_policy, beta):
     """({name: net} of every sharded net, β included as "beta", {key: optimizer} of an agent or None, VocabParallel).
     Raises unless every net is vocabulary-parallel on the policy's plan."""
-    from .nn.arena import _is_beta, _is_discrete
-    agent = agent_or_policy if hasattr(agent_or_policy, "nets") else None
-    if agent is not None or isinstance(agent_or_policy, dict):
-        src = agent.nets if agent is not None else agent_or_policy
-        missing = [k for k in _AGENT_NETS if src.get(k) is None]
-        if missing:
-            raise ValueError("a REINFORCE agent's nets need %s" % ", ".join(missing))
-        nets = {k: src[k] for k in _AGENT_NETS}
-    elif _is_beta(agent_or_policy) or not _is_discrete(agent_or_policy):
-        raise TypeError("a vocabulary-parallel checkpoint is of a DiscreteActor or a REINFORCE agent")
-    else:
-        nets = {"policy_net": agent_or_policy}
+    agent, nets = _vocab_nets(agent_or_policy, beta,
+                              "a vocabulary-parallel checkpoint is of a DiscreteActor or a REINFORCE agent")
     if beta is not None:
-        if not _is_beta(beta):
-            raise TypeError("beta must be a recnn_b200.nn.Beta (got %s)" % type(beta).__name__)
         nets["beta"] = beta
     vp = nets["policy_net"].__dict__.get("_recnn_vp")
     for name, net in nets.items():

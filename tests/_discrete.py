@@ -1,5 +1,6 @@
 """Builders of the DiscreteActor and item-id critic cases that several GPU tests share: a DiscreteActor from numpy
-parameters, and the seeded item-id critic case laid out as vocabulary-shard ranks with their DiscreteValueArgs."""
+parameters, the seeded item-id critic case, and that case laid out as vocabulary-shard ranks with their
+DiscreteValueArgs (test_workspace_bounds_gpu.py calls the C step and phases on them to bound their workspace)."""
 from __future__ import annotations
 
 import numpy as np

@@ -1,8 +1,8 @@
 """The behaviour policy beta sharded over the item vocabulary (recnn_beta_shard_*) on the GPU.
 
-As for the sharded policy (test_reinforce_vocab_parallel_gpu.py), the maths is checked with VIRTUAL ranks on one
-device: the three phases of W shards run in one process and each all-gather is stood in for by concatenating the
-ranks' records in rank order (what recnn_comm_allgather delivers).  The transport and the Python API run at world 1;
+As for the sharded policy (test_reinforce_vocab_parallel_gpu.py), W > 1 runs as VIRTUAL ranks on one device
+(tests/_ranks.py): W copies of the sharded Beta's public API in one process, each all-gather delivering the ranks'
+records in rank order (what recnn_comm_allgather delivers).  The transport and the Python API also run at world 1;
 W > 1 processes need W GPUs."""
 from __future__ import annotations
 
@@ -22,6 +22,7 @@ from recnn_b200.nn.arena import param_arena, grad_arena
 from recnn_b200.nn.update import reinforce as RF
 from oracle import beta_oracle as B
 from oracle import reinforce_oracle as RO
+from tests._ranks import bits, chunked, one_rank_group, returned, run_ranks, shard, spawn  # noqa: F401
 from tests.test_beta_gpu import REORDER_BAR, make_beta, onehot
 
 pytestmark = pytest.mark.gpu
@@ -37,64 +38,35 @@ def _t(x):
     return torch.from_numpy(np.ascontiguousarray(x)).to(DEV)
 
 
-class Call:
-    """The args of one Beta's call on its own arena (built-in RAdam, or external), with its own workspace."""
-
-    def __init__(self, beta, state, ids, chunk):
-        d = beta.dims
-        n = state.shape[0]
-        self.chunk = chunk if chunk < d.num_items else d.num_items
-        self.probs = torch.empty(n, d.num_items, device=DEV)
-        self.loss = torch.empty((), device=DEV)
-        self.error = torch.zeros(1, dtype=torch.int32, device=DEV)
-        self.ws = torch.empty(L.recnn_beta_workspace_bytes(d, n, self.chunk), dtype=torch.uint8, device=DEV)
-        a = _lib.BetaArgs()
-        a.dims, a.n_rows, a.chunk_items = d, n, self.chunk
-        a.net, a.optim = beta.optim.c_net(beta), beta.optim.c_optim()
-        a.state, a.state_ld = state.data_ptr(), state.stride(0)
-        a.action, a.probs_out = ids.data_ptr(), self.probs.data_ptr()
-        a.loss, a.error = self.loss.data_ptr(), self.error.data_ptr()
-        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
-        self.args = a
+def _radam_beta(w, b):
+    beta = make_beta(w, b)
+    beta.optim = recnn_b200.optim.RAdam(beta.net.parameters(), lr=1e-2, weight_decay=1e-5)
+    return beta
 
 
-class Virtual:
-    """W shards of one Beta as W Betas on one device, each with its built-in RAdam."""
-
-    def __init__(self, w, b, world, lr=1e-2):
-        self.items, self.world = w.shape[0], world
-        self.plan = [D.vocab_shard(self.items, r, world) for r in range(world)]
-        self.mods = [make_beta(w[lo:hi], b[lo:hi]) for lo, hi in self.plan]
-        for m in self.mods:
-            m.optim = recnn_b200.optim.RAdam(m.net.parameters(), lr=lr, weight_decay=1e-5)
-
-    def vs(self, r):
-        return _lib.VocabShard(self.plan[r][0], self.items, r, self.world)
-
-    def call(self, state, ids, chunk, order=None, order2=None):
-        """begin / rows / end on every rank; returns (calls, gathered records of exchange 1)."""
-        st = _lib.stream_ptr()
-        n = state.shape[0]
-        calls = [Call(m, state, ids, chunk) for m in self.mods]
-        recs = [torch.empty(L.recnn_vocab_record_floats(n), device=DEV) for _ in self.mods]
-        for r, c in enumerate(calls):
-            _lib.check(L.recnn_beta_shard_begin(c.args, self.vs(r), recs[r].data_ptr(), st))
-        g1 = torch.cat([recs[q] for q in (order or range(self.world))])
-        sums = [torch.empty_like(x) for x in recs]
-        for r, c in enumerate(calls):
-            _lib.check(L.recnn_beta_shard_rows(c.args, self.vs(r), g1.data_ptr(), sums[r].data_ptr(), st))
-        g2 = torch.cat([sums[q] for q in (order2 or range(self.world))])
-        for r, c in enumerate(calls):
-            _lib.check(L.recnn_beta_shard_end(c.args, self.vs(r), g2.data_ptr(), st))
-        torch.cuda.synchronize()
-        return calls, g1
+def _state_of(m):
+    return {"p": param_arena(m).clone(), "g": grad_arena(m).clone(), "m": m.optim._m.clone(), "v": m.optim._v.clone(),
+            "t": int(m.optim._t.item())}
 
 
-def full_call(beta, state, ids, chunk):
-    c = Call(beta, state, ids, chunk)
-    _lib.check(L.recnn_beta_step(c.args, _lib.stream_ptr()))
-    torch.cuda.synchronize()
-    return c
+def sharded_calls(full, world, calls, chunk=None, order=None):
+    """On W virtual ranks, a Beta sharded from ``full`` is called on each (state, ids) of ``calls``: per rank, per call
+    (column block or the call's exception, loss, arenas after the call, net.0's {w, b, gw, gb} after the call)."""
+    def rank(r):
+        beta = shard({}, full)[1]
+        out = []
+        for s, ids in calls:
+            try:
+                got = beta(s, ids)
+            except (RuntimeError, IndexError) as exc:
+                got = exc
+            lin = beta.net[0]
+            out.append((got, beta.last_loss.clone(), _state_of(beta),
+                        {"w": lin.weight.detach().clone(), "b": lin.bias.detach().clone(),
+                         "gw": lin.weight.grad.clone(), "gb": lin.bias.grad.clone()}))
+        return out
+    with chunked(calls[0][0].shape[0], chunk):
+        return run_ranks(world, rank, order=order)
 
 
 def _case(S, items, n, seed, world):
@@ -115,42 +87,44 @@ def _rel(got, want):
 
 def run_virtual_sweep():
     """Every shape x W: two calls each; the loss has the same bits on every rank; the concatenated blocks, dW, db and
-    the stepped weights against the unsharded recnn_beta_step (reordering bar) and the float64 oracle."""
+    the stepped weights against the unsharded Beta (reordering bar) and the float64 oracle."""
     for S, items, n, chunk in SHAPES:
         for world in (2, 3, 8):
             rng, w, b, ids = _case(S, items, n, S + items + world, world)
-            v = Virtual(w, b, world)
-            full = make_beta(w, b)
-            full.optim = recnn_b200.optim.RAdam(full.net.parameters(), lr=1e-2, weight_decay=1e-5)
+            full = _radam_beta(w, b)
             params, o = {"w": w.copy(), "b": b.copy()}, B.make_radam(lr=1e-2)
-            for t in range(2):
-                s = _t(rng.normal(0, 1, (n, S)).astype(np.float32))
-                it = _t(ids)
+            it = _t(ids)
+            calls = [(_t(rng.normal(0, 1, (n, S)).astype(np.float32)), it) for _ in range(2)]
+            res = returned(sharded_calls(full, world, calls, chunk))
+            for t, (s, _) in enumerate(calls):
                 prev = {k: getattr(full.net[0], k).detach().clone() for k in ("weight", "bias")}
-                calls, _ = v.call(s, it, chunk)
-                want = full_call(full, s, it, chunk)
-                assert [int(c.error) for c in calls] == [0] * world
-                assert len({c.loss.cpu().numpy().tobytes() for c in calls}) == 1
-                assert float(calls[0].loss) == pytest.approx(float(want.loss), rel=1e-6)
-                probs = torch.cat([c.probs for c in calls], 1)
-                assert _rel(probs, want.probs) <= REORDER_BAR
+                with chunked(n, chunk):
+                    want = full(s, it)
+                got = [x[t] for x in res]
+                assert not any(isinstance(g[0], Exception) for g in got), got
+                assert len({bits(g[1]).item() for g in got}) == 1
+                loss = float(got[0][1])
+                assert loss == pytest.approx(float(full.last_loss), rel=1e-6)
+                probs = torch.cat([g[0] for g in got], 1)
+                assert _rel(probs, want) <= REORDER_BAR
                 wp, wl, grads = B.beta_call(params, o, s.cpu().numpy(), ids)
-                assert abs(float(calls[0].loss) - wl) <= 1e-5 * (abs(wl) + 0.1)
+                assert abs(loss - wl) <= 1e-5 * (abs(wl) + 0.1)
                 assert np.max(np.abs(probs.double().cpu().numpy() - wp) / (wp + 1e-2 * wp.max())) <= 1e-5
-                gw = torch.cat([m.net[0].weight.grad for m in v.mods])
-                gb = torch.cat([m.net[0].bias.grad for m in v.mods])
+                local = [g[3] for g in got]
+                gw = torch.cat([x["gw"] for x in local])
+                gb = torch.cat([x["gb"] for x in local])
                 assert _rel(gw, full.net[0].weight.grad) <= REORDER_BAR, (S, items, world, t)
                 assert _rel(gb, full.net[0].bias.grad) <= REORDER_BAR, (S, items, world, t)
-                for got, k in ((gw, "w"), (gb, "b")):
+                for g, k in ((gw, "w"), (gb, "b")):
                     ref = grads[k]
-                    assert np.abs(got.double().cpu().numpy() - ref).max() <= 1e-4 * np.abs(ref).max(), k
+                    assert np.abs(g.double().cpu().numpy() - ref).max() <= 1e-4 * np.abs(ref).max(), k
                 # the stepped weights: two roundings of the weight plus the gradients' reordering share of the step
-                for k in ("weight", "bias"):
-                    got = torch.cat([getattr(m.net[0], k).detach() for m in v.mods])
+                for k, key in (("weight", "w"), ("bias", "b")):
+                    g = torch.cat([x[key] for x in local])
                     ref = getattr(full.net[0], k).detach()
                     tol = 2 * torch.finfo(torch.float32).eps * ref.abs() + REORDER_BAR * float((ref - prev[k]).abs().max())
-                    assert bool(((got - ref).abs() <= tol).all()), k
-                assert all(m.optim.steps_taken() == t + 1 for m in v.mods)
+                    assert bool(((g - ref).abs() <= tol).all()), k
+                assert all(g[2]["t"] == t + 1 for g in got)
             print("virtual beta S %d I %d W %d: ok" % (S, items, world))
 
 
@@ -169,100 +143,104 @@ def test_virtual_ranks_on_the_cuda_core_back_end():
     assert r.returncode == 0
 
 
-def _state_of(m):
-    return {"p": param_arena(m).clone(), "g": grad_arena(m).clone(), "m": m.optim._m.clone(), "v": m.optim._v.clone(),
-            "t": int(m.optim._t.item())}
-
-
 @pytest.mark.parametrize("S,items,n,chunk", SHAPES)
 def test_world1_is_bit_identical_to_the_step(S, items, n, chunk):
     rng, w, b, ids = _case(S, items, n, 3 * S, 1)
-    v = Virtual(w, b, 1)
-    full = make_beta(w, b)
-    full.optim = recnn_b200.optim.RAdam(full.net.parameters(), lr=1e-2, weight_decay=1e-5)
-    for t in range(3):
-        s = _t(rng.normal(0, 1, (n, S)).astype(np.float32))
-        it = _t(rng.integers(0, items, n))
-        calls, _ = v.call(s, it, chunk)
-        want = full_call(full, s, it, chunk)
-        assert torch.equal(calls[0].probs, want.probs)
-        assert calls[0].loss.cpu().numpy().tobytes() == want.loss.cpu().numpy().tobytes()
-        assert int(calls[0].error) == 0
-        a, e = _state_of(v.mods[0]), _state_of(full)
-        for k in a:
-            assert (a[k] == e[k]) if k == "t" else torch.equal(a[k], e[k]), (t, k)
+    full = _radam_beta(w, b)
+    calls = [(_t(rng.normal(0, 1, (n, S)).astype(np.float32)), _t(rng.integers(0, items, n))) for _ in range(3)]
+    (res,) = returned(sharded_calls(full, 1, calls, chunk))
+    for t, ((s, it), (probs, loss, state, _)) in enumerate(zip(calls, res)):
+        with chunked(n, chunk):
+            want = full(s, it)
+        assert torch.equal(probs, want)
+        assert bits(loss).item() == bits(full.last_loss).item()
+        e = _state_of(full)
+        for k in state:
+            assert (state[k] == e[k]) if k == "t" else torch.equal(state[k], e[k]), (t, k)
 
 
 def test_records_out_of_rank_order_and_bad_ids_skip_the_step():
     S, items, n, chunk = 37, 1003, 33, 128
     rng, w, b, ids = _case(S, items, n, 5, 3)
-    v = Virtual(w, b, 3)
     s = _t(rng.normal(0, 1, (n, S)).astype(np.float32))
-    v.call(s, _t(ids), chunk)
-    before = [_state_of(m) for m in v.mods]
-    for order, order2, bad, bit in (([1, 0, 2], None, None, 2), (None, [0, 2, 1], None, 2), (None, None, items, 1),
-                                    (None, None, -1, 1)):
-        it = ids.copy()
-        if bad is not None:
-            it[7] = bad
-        calls, _ = v.call(s, _t(it), chunk, order, order2)
-        assert [int(c.error) & bit for c in calls] == [bit] * 3, (order, order2, bad)
-        if bit == 1:
-            assert len({c.loss.cpu().numpy().tobytes() for c in calls}) == 1
-        for m, x in zip(v.mods, before):
-            y = _state_of(m)
+    bad = [ids.copy(), ids.copy()]
+    bad[0][7], bad[1][7] = items, -1
+    # call 0 is good; the first gather of call 1 and the second of call 2 come out of rank order; calls 3 and 4 hold
+    # an id out of range
+    calls = [(s, _t(x)) for x in (ids, ids, ids, bad[0], bad[1])]
+    res = returned(sharded_calls(_radam_beta(w, b), 3, calls, chunk, order={2: [1, 0, 2], 5: [0, 2, 1]}))
+    for c, want in ((1, RuntimeError), (2, RuntimeError), (3, IndexError), (4, IndexError)):
+        errs = [x[c][0] for x in res]
+        assert all(isinstance(e, want) for e in errs), (c, errs)
+        if want is RuntimeError:
+            assert all("disagree on the vocabulary shard plan" in str(e) for e in errs)
+        else:
+            assert len({bits(x[c][1]).item() for x in res}) == 1
+        for x in res:
+            before, after = x[0][2], x[c][2]
             for k in ("p", "m", "v", "t"):
-                assert (x[k] == y[k]) if k == "t" else torch.equal(x[k], y[k]), (order, bad, k)
+                assert (before[k] == after[k]) if k == "t" else torch.equal(before[k], after[k]), (c, k)
 
 
 def test_sharded_draws_pick_the_unsharded_item():
-    """W = 3: the policy's sharded draw (recnn_discrete_shard_sample + shard_pick) on beta's blocks and records, from
-    replayed uniforms, against recnn_categorical_sample on the unsharded probabilities."""
+    """W = 3: DiscreteActor.pi_beta_sample with a Beta sharded with the policy, the action drawn from beta (the
+    {pi: beta, beta: beta} source): the draw from beta's blocks and records, from replayed uniforms, against the
+    unsharded policy's draw on the unsharded probabilities, and pi's log-prob of it from the policy's blocks."""
     S, items, n = 37, 1003, 300
     rng, w, b, ids = _case(S, items, n, 8, 3)
     w = (w * 6).astype(np.float32)
-    v = Virtual(w, b, 3)
     s = _t(rng.normal(0, 1, (n, S)).astype(np.float32))
-    calls, g1 = v.call(s, _t(ids), 128)
-    full = make_beta(w, b)
-    want = full_call(full, s, _t(ids), 128).probs
     u = _t(rng.random(n).astype(np.float32))
-    draws = []
-    for r, c in enumerate(calls):
-        d = _lib.DiscreteDims(S, 1, c.probs.shape[1], 0)
-        draws.append(torch.empty(2 * n, device=DEV))
-        _lib.check(L.recnn_discrete_shard_sample(d, v.vs(r), g1.data_ptr(), c.probs.data_ptr(), n, u.data_ptr(), 0, 1,
-                                                 draws[r].data_ptr(), _lib.stream_ptr()))
-    a, lp = torch.empty(n, dtype=torch.int64, device=DEV), torch.empty(n, device=DEV)
-    flag = torch.zeros(1, dtype=torch.int32, device=DEV)
-    _lib.check(L.recnn_discrete_shard_pick(3, torch.cat(draws).data_ptr(), n, a.data_ptr(), lp.data_ptr(),
-                                           flag.data_ptr(), _lib.stream_ptr()))
-    ra, rl = torch.empty_like(a), torch.empty_like(lp)
-    _lib.check(L.recnn_categorical_sample(want.data_ptr(), n, items, items, u.data_ptr(), 0, 1, ra.data_ptr(),
-                                          rl.data_ptr(), _lib.stream_ptr()))
-    assert int(flag) == 0
+    full = make_beta(w, b)
+    policy = recnn_b200.nn.DiscreteActor(S, items, 16).to(DEV)
+
+    def rank(r):
+        nets, beta = shard({"policy_net": policy}, full)
+        pol = nets["policy_net"]
+        pol.uniform_source = lambda n: u
+        pol.action_source = {"pi": "beta", "beta": "beta"}
+        pi_lp, beta_lp, _ = pol.pi_beta_sample(s, beta, _t(ids))
+        return pol._last_sample["action"], beta_lp, pi_lp
+    with chunked(n, 128):
+        res = returned(run_ranks(3, rank))
+        want = full(s, _t(ids))
+    a, lp, pi_lp = res[0]
+    for x in res[1:]:
+        assert torch.equal(x[0], a) and torch.equal(x[1], lp) and torch.equal(x[2], pi_lp)
+    policy.uniform_source = lambda n: u
+    ra, rl = policy._sample(want)
     _, _, margin = RO.categorical_sample(want.double().cpu().numpy(), u.cpu().numpy())
     keep = torch.from_numpy(margin > 1e-5).to(DEV)
     assert int(keep.sum()) > 0.9 * n
     assert torch.equal(a[keep], ra[keep])
     assert float((lp[keep] - rl[keep]).abs().max()) <= 1e-5
+    want_pi = RO.categorical_log_prob(policy(s).double().cpu().numpy(), a.cpu().numpy())
+    assert np.abs(pi_lp.cpu().numpy() - want_pi).max() <= 1e-5
+
+
+class Call:
+    """The args of one Beta's call on its own arena (built-in RAdam, or external), with its own workspace: the rank
+    share memory test runs the C phases itself."""
+
+    def __init__(self, beta, state, ids, chunk):
+        d = beta.dims
+        n = state.shape[0]
+        self.chunk = chunk if chunk < d.num_items else d.num_items
+        self.probs = torch.empty(n, d.num_items, device=DEV)
+        self.loss = torch.empty((), device=DEV)
+        self.error = torch.zeros(1, dtype=torch.int32, device=DEV)
+        self.ws = torch.empty(L.recnn_beta_workspace_bytes(d, n, self.chunk), dtype=torch.uint8, device=DEV)
+        a = _lib.BetaArgs()
+        a.dims, a.n_rows, a.chunk_items = d, n, self.chunk
+        a.net, a.optim = beta.optim.c_net(beta), beta.optim.c_optim()
+        a.state, a.state_ld = state.data_ptr(), state.stride(0)
+        a.action, a.probs_out = ids.data_ptr(), self.probs.data_ptr()
+        a.loss, a.error = self.loss.data_ptr(), self.error.data_ptr()
+        a.workspace, a.workspace_bytes = self.ws.data_ptr(), self.ws.numel()
+        self.args = a
 
 
 # ----------------------------------------------------------------------------- the Python API at world 1
-@pytest.fixture
-def one_rank_group(tmp_path):
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    dist.init_process_group("nccl", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1,
-                            device_id=torch.device(DEV))
-    yield
-    dist.destroy_process_group()
-
-
-def _bits(t):
-    return t.detach().contiguous().view(torch.int32).cpu()
-
-
 def _notebook_agent(source, items=1003, H=64, S=37):
     torch.manual_seed(9)
     beta_net = recnn_b200.nn.Beta(S, items).to(DEV)
@@ -312,7 +290,7 @@ def test_python_api_world1_equals_unsharded(one_rank_group, source):
             agent.step()
         assert losses[0] == losses[1], step
         assert torch.equal(plain_seen[-1], shard_seen[-1]), step
-        assert _bits(plain_beta.last_loss).tolist() == _bits(shard_beta.last_loss).tolist()
+        assert bits(plain_beta.last_loss).tolist() == bits(shard_beta.last_loss).tolist()
         pp, sp = plain.nets["policy_net"], shard.nets["policy_net"]
         for k in ("saved_log_probs", "correction", "lambda_k"):
             assert len(getattr(pp, k)) == len(getattr(sp, k))
@@ -326,7 +304,7 @@ def test_python_api_world1_equals_unsharded(one_rank_group, source):
     assert plain_beta.optim.steps_taken() == shard_beta.optim.steps_taken() == steps
     for x, y in ((plain_beta, shard_beta), (plain.nets["policy_net"], shard.nets["policy_net"]),
                  (plain.nets["value_net"], shard.nets["value_net"])):
-        assert torch.equal(_bits(param_arena(x)), _bits(param_arena(y)))
+        assert torch.equal(bits(param_arena(x)), bits(param_arena(y)))
     assert torch.equal(plain_beta.optim._m, shard_beta.optim._m) and torch.equal(plain_beta.optim._v, shard_beta.optim._v)
     # one-hot and item-id actions drive the sharded beta identically
     s = torch.randn(N, S, device=DEV)
@@ -448,18 +426,7 @@ def _vp_worker(rank, world, port, q):
 def test_multi_process_equals_unsharded(world):
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_vp_worker, args=(r, world, port, q)) for r in range(world)]
-    for pr in procs:
-        pr.start()
-    res = dict(q.get(timeout=300) for _ in range(world))
-    for pr in procs:
-        pr.join(timeout=60)
-        assert pr.exitcode == 0
+    res = dict(spawn(_vp_worker, world))
     rng, w, b, ids = _case_np(world)
     state = rng.normal(0, 1, (24, 37)).astype(np.float32)
     full = make_beta(w, b)

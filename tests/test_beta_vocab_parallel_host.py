@@ -16,6 +16,7 @@ from recnn_b200 import _lib
 from recnn_b200 import dist as D
 from recnn_b200.nn.arena import param_arena
 from tests import _beta_vocab_oracle as BV
+from tests._ranks import one_rank_cpu_group  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -90,14 +91,6 @@ def test_new_symbols_in_header_library_and_ctypes_table():
 
 
 # ----------------------------------------------------------------------------- refusals
-@pytest.fixture
-def one_rank_cpu_group(tmp_path):
-    import torch.distributed as dist
-    dist.init_process_group("gloo", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1)
-    yield
-    dist.destroy_process_group()
-
-
 def _agent(S=6, H=8, I=10):
     torch.manual_seed(0)
     return recnn_b200.nn.Reinforce(recnn_b200.nn.DiscreteActor(S, I, H), recnn_b200.nn.Critic(S, I, H))

@@ -1,7 +1,6 @@
 """DiscreteActor.topk / recnn_discrete_topk / the sharded pair on the GPU, against the float64 restatement in
-tests/_policy_topk_oracle.py, against the dense forward, and across chunkings, exclusions, ties and virtual ranks (the
-pattern of test_reinforce_vocab_parallel_gpu.py: W shards in one process, the all-gather stood in for by concatenating
-the records in rank order)."""
+tests/_policy_topk_oracle.py, against the dense forward, and across chunkings, exclusions, ties and virtual ranks (W
+copies of the sharded policy's public API in one process, tests/_ranks.py)."""
 from __future__ import annotations
 
 import gc
@@ -20,8 +19,8 @@ from recnn_b200.nn.arena import param_arena
 from oracle import reinforce_oracle as RO
 from tests import _policy_topk_oracle as TK
 from tests._discrete import make_policy
+from tests._ranks import chunked, one_rank_group, returned, run_ranks, shard, spawn  # noqa: F401
 from tests.test_reinforce_chunked_gpu import REORDER_BAR
-from tests.test_reinforce_vocab_parallel_gpu import Virtual
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -261,32 +260,14 @@ def test_million_items_memory_and_sampled_rows():
 
 
 # ----------------------------------------------------------------------------- virtual ranks
-def shard_topk(v, state, k, chunk=None, exclude=None, permute=None):
-    """Both calls on every virtual rank: (per-rank values, per-rank ids, per-rank error bits)."""
-    n = state.shape[0]
-    st = _lib.stream_ptr()
-    n_ex = 0 if exclude is None else exclude.shape[1]
-    recs = []
-    for r, m in enumerate(v.mods):
-        d = m.dims
-        c = d.num_items if chunk is None or chunk >= d.num_items else chunk
-        nbytes = L.recnn_discrete_topk_workspace_bytes(d, n, k, c)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
-        recs.append(torch.empty(L.recnn_vocab_topk_record_floats(n, k), device=DEV))
-        _lib.check(L.recnn_discrete_shard_topk(d, v.vs(r), param_arena(m).data_ptr(), state.data_ptr(), n, k,
-                                               _lib.ptr(exclude), n_ex, c, recs[r].data_ptr(), ws.data_ptr(), nbytes,
-                                               st))
-    gathered = torch.cat([recs[q] for q in (permute or range(v.world))])
-    vals, ids, flags = [], [], []
-    for r, m in enumerate(v.mods):
-        vals.append(torch.empty(n, k, device=DEV))
-        ids.append(torch.empty(n, k, dtype=torch.int64, device=DEV))
-        flag = torch.full((1,), 9, dtype=torch.int32, device=DEV)
-        _lib.check(L.recnn_discrete_shard_topk_finish(m.dims, v.vs(r), gathered.data_ptr(), n, k, _lib.ptr(exclude),
-                                                      n_ex, vals[r].data_ptr(), ids[r].data_ptr(), flag.data_ptr(), st))
-        flags.append(flag)
-    torch.cuda.synchronize()
-    return vals, ids, [int(f) for f in flags]
+def sharded_topk(full, world, state, k, chunk=None, exclude=None, order=None, dense=False):
+    """policy.topk on W virtual ranks sharded from ``full`` (tests/_ranks.py): each rank's (values, ids[, its column
+    block of policy(state)]) or exception."""
+    def rank(r):
+        pol = shard({"policy_net": full})[0]["policy_net"]
+        return pol.topk(state, k, exclude=exclude) + ((pol(state),) if dense else ())
+    with chunked(state.shape[0], chunk):
+        return run_ranks(world, rank, order=order)
 
 
 def _shard_tie_case(I, world, S=36, H=32, N=30):
@@ -302,72 +283,64 @@ def _shard_tie_case(I, world, S=36, H=32, N=30):
 def test_virtual_ranks(world):
     for S, H, I, N in [(52, 64, 1003, 40), (37, 32, 200, 17)]:      # 200 items over 8 ranks: 25 per block < k = 64
         p, state, edges = _shard_tie_case(I, world, S, H, N)
-        v = Virtual(p, S, H, world)
         full = make_policy(p, S, H, I)
         st = _t(state)
         z = TK.logits(p, state)
         for k in (10, 64):
             for chunk in (None, 128):
-                vals, ids, flags = shard_topk(v, st, k, chunk)
-                assert flags == [0] * world
-                for r in range(1, world):
-                    assert torch.equal(vals[r], vals[0]) and torch.equal(ids[r], ids[0])
-                check_against_oracle(vals[0], ids[0], z, k, what=("W", world, I, k, chunk), min_sure=0)
+                res = returned(sharded_topk(full, world, st, k, chunk, dense=chunk is None))
+                vals, ids = res[0][0], res[0][1]
+                for x in res[1:]:
+                    assert torch.equal(x[0], vals) and torch.equal(x[1], ids)
+                check_against_oracle(vals, ids, z, k, what=("W", world, I, k, chunk), min_sure=0)
                 want_i = TK.shard_topk(z, k, world)[1]
                 top = min(len(edges), k)
-                assert np.array_equal(ids[0][:, :top].cpu().numpy(), want_i[:, :top])
-                assert np.array_equal(ids[0][:, :top].cpu().numpy(), np.tile(edges[:top], (N, 1)))
+                assert np.array_equal(ids[:, :top].cpu().numpy(), want_i[:, :top])
+                assert np.array_equal(ids[:, :top].cpu().numpy(), np.tile(edges[:top], (N, 1)))
                 if world == 1:
-                    one_v, one_i, _ = call_topk(v.mods[0], st, k, chunk)
-                    assert torch.equal(vals[0], one_v) and torch.equal(ids[0], one_i)
+                    with chunked(N, chunk):
+                        one_v, one_i = full.topk(st, k)
+                    assert torch.equal(vals, one_v) and torch.equal(ids, one_i)
                 if chunk is None:
-                    blocks, _ = v.forward(st)
-                    dense = torch.cat(blocks, 1)
-                    assert torch.equal(vals[0], dense.gather(1, ids[0]))
+                    dense = torch.cat([x[2] for x in res], 1)
+                    assert torch.equal(vals, dense.gather(1, ids))
         if world > 1:
-            _, _, flags = shard_topk(v, st, 10, permute=[1, 0] + list(range(2, world)))
-            assert all(f & 2 for f in flags), flags
+            res = sharded_topk(full, world, st, 10, order={0: [1, 0] + list(range(2, world))})
+            assert all(isinstance(e, RuntimeError) and "disagree on the vocabulary shard plan" in str(e)
+                       for e in res), res
         del full
 
 
 def test_virtual_ranks_exclusion_on_shard_edges():
     S, H, I, N, world = 52, 64, 1003, 40, 3
     p, state, edges = _shard_tie_case(I, world, S, H, N)
-    v = Virtual(p, S, H, world)
+    full = make_policy(p, S, H, I)
     st = _t(state)
     z = TK.logits(p, state)
     ex = np.full((N, 4), -1)
     ex[:, 0] = edges[1]
     ex[:, 1] = edges[-1]
-    vals, ids, flags = shard_topk(v, st, 10, 128, _t(ex))
-    assert flags == [0] * world
+    res = returned(sharded_topk(full, world, st, 10, 128, _t(ex)))
+    vals, ids = res[0]
+    for x in res[1:]:
+        assert torch.equal(x[0], vals) and torch.equal(x[1], ids)
     want_v, want_i = TK.shard_topk(z, 10, world, ex)
-    assert np.array_equal(ids[0][:, :len(edges) - 2].cpu().numpy(), want_i[:, :len(edges) - 2])
-    check_against_oracle(vals[0], ids[0], z, 10, ex, what="W3 exclude", min_sure=0)
+    assert np.array_equal(ids[:, :len(edges) - 2].cpu().numpy(), want_i[:, :len(edges) - 2])
+    check_against_oracle(vals, ids, z, 10, ex, what="W3 exclude", min_sure=0)
     ex[2, 3] = I
-    _, _, flags = shard_topk(v, st, 10, 128, _t(ex))
-    assert flags == [1] * world
+    res = sharded_topk(full, world, st, 10, 128, _t(ex))
+    assert all(isinstance(e, IndexError) for e in res), res
 
 
 # ----------------------------------------------------------------------------- the Python API at world 1
-@pytest.fixture
-def one_rank_group(tmp_path):
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    dist.init_process_group("nccl", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1,
-                            device_id=torch.device(DEV))
-    yield
-    dist.destroy_process_group()
-
-
 def test_python_api_world1_equals_unsharded(one_rank_group, monkeypatch):
     S, H, I, N = 37, 32, 2000, 50
     torch.manual_seed(12)
     plain = recnn_b200.nn.DiscreteActor(S, I, H).to(DEV)
-    shard = recnn_b200.nn.DiscreteActor(S, I, H).to(DEV)
-    shard.load_state_dict(plain.state_dict())
-    D.enable_vocab_parallel(shard)
-    vp = shard.__dict__["_recnn_vp"]
+    sharded = recnn_b200.nn.DiscreteActor(S, I, H).to(DEV)
+    sharded.load_state_dict(plain.state_dict())
+    D.enable_vocab_parallel(sharded)
+    vp = sharded.__dict__["_recnn_vp"]
     try:
         st = torch.randn(N, S, device=DEV)
         ex = torch.randint(-1, I, (N, 7), device=DEV)
@@ -377,10 +350,10 @@ def test_python_api_world1_equals_unsharded(one_rank_group, monkeypatch):
                 monkeypatch.setattr(RF, "_chunk_items", lambda rows, items: min(chunk, items))
             for k, e in ((1, None), (17, ex), (64, ex)):
                 a = plain.topk(st, k, exclude=e)
-                b = shard.topk(st, k, exclude=e)
+                b = sharded.topk(st, k, exclude=e)
                 assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1]), (chunk, k)
         with pytest.raises(IndexError):
-            shard.topk(st, 3, exclude=torch.full((N, 1), I, device=DEV))
+            sharded.topk(st, 3, exclude=torch.full((N, 1), I, device=DEV))
     finally:
         vp.comm.close()
 
@@ -411,18 +384,7 @@ def _topk_worker(rank, world, port, q):
 def test_multi_process_equals_unsharded(world):
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_topk_worker, args=(r, world, port, q)) for r in range(world)]
-    for pr in procs:
-        pr.start()
-    res = {r: (v, i) for r, v, i in (q.get(timeout=300) for _ in range(world))}
-    for pr in procs:
-        pr.join(timeout=60)
-        assert pr.exitcode == 0
+    res = {r: (v, i) for r, v, i in spawn(_topk_worker, world)}
     S, H, I, N = 52, 64, 1003, 48
     p, state = make_case(S, H, I, N, 77)
     ex = np.arange(N * 3).reshape(N, 3) % I

@@ -1,8 +1,8 @@
 """The item-id REINFORCE critic sharded over the item vocabulary, on the GPU.
 
-As in test_reinforce_vocab_parallel_gpu.py, the maths is checked with VIRTUAL ranks on one device: the three C phases of
-W shards run in one process, the all-gather is stood in for by concatenating the ranks' records in rank order and the
-all-reduce of the [2, N, H] terms by an in-order fp32 sum.  The Python API is checked at world 1 through a one-rank
+As in test_reinforce_vocab_parallel_gpu.py, W > 1 runs as VIRTUAL ranks on one device (tests/_ranks.py): W copies of
+value_update on sharded nets in one process, the all-gather delivering the ranks' records in rank order and the
+all-reduce of the [2, N, H] terms an in-order fp32 sum.  The Python API is also checked at world 1 through a one-rank
 NCCL group against an unsharded twin, bit for bit; W > 1 processes need W GPUs."""
 from __future__ import annotations
 
@@ -18,12 +18,11 @@ from recnn_b200 import _lib
 from recnn_b200 import dist as D
 from recnn_b200.nn.arena import param_arena, grad_arena
 from recnn_b200.nn.update import reinforce as RF
-from oracle import recnn_oracle as O
-from oracle import reinforce_oracle as RO
+from recnn_b200.nn.update._engine import MASK_KEY
 from tests import _critic_vocab_oracle as CV
 from tests._cuda import load_net
-from tests._discrete import (PARAMS, critic_case as _case, critic_ranks as _ranks, make_policy,
-                             to_dev as _t)
+from tests._discrete import PARAMS, critic_case as _case, make_policy, to_dev as _t
+from tests._ranks import bits, chunked, exchange, one_rank_group, returned, run_ranks, shard, spawn  # noqa: F401
 from tests.test_reinforce_chunked_gpu import REORDER_BAR
 
 pytestmark = pytest.mark.gpu
@@ -34,38 +33,36 @@ L = _lib.lib()
 SHAPES = [(52, 64, 1003, 40, 128), (37, 32, 2000, 33, 256)]
 
 
-def run_phases(ranks, order=None):
-    """begin on every rank, the all-gather (records concatenated in ``order``), merge, the in-order fp32 sum of the
-    terms, end.  Returns the summed terms."""
-    st = _lib.stream_ptr()
-    n = ranks[0].n
-    recs = []
-    for rk in ranks:
-        recs.append(torch.empty(L.recnn_vocab_record_floats(n), device=DEV))
-        _lib.check(L.recnn_discrete_value_shard_begin(rk.args, rk.shard, recs[-1].data_ptr(), st))
-    gathered = torch.cat([recs[q] for q in (order or range(len(ranks)))])
-    terms = []
-    for rk in ranks:
-        terms.append(torch.empty(2 * n * rk.args.dims.hidden, device=DEV))
-        _lib.check(L.recnn_discrete_value_shard_merge(rk.args, rk.shard, gathered.data_ptr(), terms[-1].data_ptr(), st))
-    acc = terms[0].clone()
-    for t in terms[1:]:
-        acc += t
-    for rk in ranks:
-        _lib.check(L.recnn_discrete_value_shard_end(rk.args, rk.shard, acc.data_ptr(), st))
-    torch.cuda.synchronize()
-    return acc
+def _nets(pp, cp, tcp, S, H, I, train):
+    """The unsharded nets of a critic_case: the policy (also the target policy), the critic and its target."""
+    policy = make_policy(pp, S, H, I)
+    value = load_net(recnn_b200.nn.Critic(S, I, H), cp, DEV).train(train)
+    return {"policy_net": policy, "target_policy_net": policy, "value_net": value,
+            "target_value_net": load_net(recnn_b200.nn.Critic(S, I, H), tcp, DEV)}
 
 
-def _unsharded(pp, cp, tcp, S, H, I, chunk, batch, masks, lr=1e-2):
-    (rk,), _, _ = _ranks(pp, cp, tcp, S, H, I, 1, chunk, batch, masks, lr)
-    _lib.check(L.recnn_discrete_value_step(rk.args, _lib.stream_ptr()))
-    torch.cuda.synchronize()
-    return rk
+def value_step(nets, batch, masks):
+    """(loss, the stepped critic) of one value_update over item ids with SGD(lr 1e-2) and the given dropout masks."""
+    b = {k: _t(v) for k, v in batch.items()}
+    if masks is not None:
+        b[MASK_KEY] = [_t(m) for m in masks]
+    opt = recnn_b200.optim.SGD(nets["value_net"].parameters(), lr=1e-2)
+    loss = recnn_b200.nn.value_update(b, PARAMS, nets, {"value_optimizer": opt}, torch.device(DEV), {}, learn=True)
+    return float(loss), nets["value_net"]
 
 
-def _bits(t):
-    return t.detach().contiguous().view(torch.int32)
+def sharded_step(case, S, H, I, world, chunk, order=None, log=None):
+    """value_step on W virtual ranks sharded from the case's nets: each rank's (loss, critic) or exception."""
+    pp, cp, tcp, batch, masks = case
+    full = _nets(pp, cp, tcp, S, H, I, masks is not None)
+    with chunked(len(batch["action"]), chunk):
+        return run_ranks(world, lambda r: value_step(shard(full)[0], batch, masks), order=order, log=log)
+
+
+def unsharded_step(case, S, H, I, chunk):
+    pp, cp, tcp, batch, masks = case
+    with chunked(len(batch["action"]), chunk):
+        return value_step(_nets(pp, cp, tcp, S, H, I, masks is not None), batch, masks)
 
 
 def _blocks(m, S):
@@ -80,37 +77,39 @@ def _blocks(m, S):
 @pytest.mark.parametrize("world", [1, 2, 3, 8])
 @pytest.mark.parametrize("S,H,I,n,chunk", SHAPES)
 def test_virtual_ranks(S, H, I, n, chunk, world, train):
-    pp, cp, tcp, batch, masks = _case(S, H, I, n, S + I + world + int(train), world, train)
-    ranks, dev_batch, _ = _ranks(pp, cp, tcp, S, H, I, world, chunk, batch, masks)
-    one = _unsharded(pp, cp, tcp, S, H, I, chunk, batch, masks)
-    terms = run_phases(ranks)
+    case = _case(S, H, I, n, S + I + world + int(train), world, train)
+    pp, cp, tcp, batch, masks = case
+    log = []
+    res = returned(sharded_step(case, S, H, I, world, chunk, log=log))
+    loss1, one = unsharded_step(case, S, H, I, chunk)
     # the loss and every replicated block (gradient and stepped weights) have the same bits on every rank
-    assert all(rk.loss_bits() == ranks[0].loss_bits() for rk in ranks)
-    assert ranks[0].loss_bits()[1] == 0
-    rep0 = _blocks(ranks[0].value, S)[0]
-    for rk in ranks[1:]:
-        for x, y in zip(_blocks(rk.value, S)[0], rep0):
-            assert torch.equal(_bits(x), _bits(y))
+    losses = [x[0] for x in res]
+    assert len({np.float32(x).tobytes() for x in losses}) == 1, losses
+    rep0 = _blocks(res[0][1], S)[0]
+    for _, value in res[1:]:
+        for x, y in zip(_blocks(value, S)[0], rep0):
+            assert torch.equal(bits(x), bits(y))
     # the summed online action term is the unsharded gather bit for bit (exactly one rank contributes to each row)
-    add = terms[n * H:].view(n, H)
-    want_add = _t(cp["w1"])[:, S + dev_batch["action"]].T
-    assert torch.equal(_bits(add), _bits(want_add))
-    # against the unsharded CUDA step: loss and replicated blocks within the reordering bar, the action block too
-    loss, loss1 = float(ranks[0].losses[0]), float(one.losses[0])
+    assert [k for k, _ in log] == ["all_gather", "all_reduce"]
+    add = log[1][1][n * H:].view(n, H)
+    want_add = _t(cp["w1"])[:, S + _t(batch["action"])].T
+    assert torch.equal(bits(add), bits(want_add))
+    # against the unsharded step: loss and replicated blocks within the reordering bar, the action block too
+    loss = losses[0]
     assert loss == pytest.approx(loss1, rel=REORDER_BAR, abs=1e-7)
-    rep1, _, g1 = _blocks(one.value, S)
+    rep1, _, g1 = _blocks(one, S)
     for x, y in zip(rep0, rep1):
         assert float((x - y).abs().max()) <= REORDER_BAR * max(float(y.abs().max()), 1e-30)
-    gblock = torch.cat([_blocks(rk.value, S)[2] for rk in ranks], 1)
+    gblock = torch.cat([_blocks(value, S)[2] for _, value in res], 1)
     assert float((gblock - g1).abs().max()) <= REORDER_BAR * float(g1.abs().max())
-    wblock = torch.cat([_blocks(rk.value, S)[1] for rk in ranks], 1)
-    w1 = one.value.linear1.weight.detach()[:, S:]
+    wblock = torch.cat([_blocks(value, S)[1] for _, value in res], 1)
+    w1 = one.linear1.weight.detach()[:, S:]
     assert float((wblock - w1).abs().max()) <= REORDER_BAR * float(w1.abs().max())
     # against the float64 oracle at the item-id critic's bars
     want_loss, want, _ = CV.value_step({"value_net": cp, "target_value_net": tcp, "target_policy_net": pp}, batch, PARAMS,
                                        masks)
     assert loss == pytest.approx(want_loss, rel=2e-5, abs=1e-6)
-    got_gw1 = torch.cat([ranks[0].value.linear1.weight.grad[:, :S], gblock], 1).double().cpu().numpy()
+    got_gw1 = torch.cat([res[0][1].linear1.weight.grad[:, :S], gblock], 1).double().cpu().numpy()
     scale = np.abs(want["w1"]).max()
     assert np.abs(got_gw1 - want["w1"]).max() <= 1e-4 * scale
     unselected = torch.from_numpy(np.setdiff1d(np.arange(I), batch["action"])).to(DEV)
@@ -120,34 +119,21 @@ def test_virtual_ranks(S, H, I, n, chunk, world, train):
 @pytest.mark.parametrize("S,H,I,n,chunk", SHAPES)
 def test_world1_phases_are_bit_identical_to_the_step(S, H, I, n, chunk):
     for train in (False, True):
-        pp, cp, tcp, batch, masks = _case(S, H, I, n, 5 * S, 1, train)
-        ranks, _, _ = _ranks(pp, cp, tcp, S, H, I, 1, chunk, batch, masks)
-        one = _unsharded(pp, cp, tcp, S, H, I, chunk, batch, masks)
-        run_phases(ranks)
-        assert ranks[0].loss_bits() == one.loss_bits()
-        assert torch.equal(_bits(param_arena(ranks[0].value)), _bits(param_arena(one.value)))
-        assert torch.equal(_bits(grad_arena(ranks[0].value)), _bits(grad_arena(one.value)))
+        case = _case(S, H, I, n, 5 * S, 1, train)
+        (loss, value), = returned(sharded_step(case, S, H, I, 1, chunk))
+        loss1, one = unsharded_step(case, S, H, I, chunk)
+        assert np.float32(loss).tobytes() == np.float32(loss1).tobytes()
+        assert torch.equal(bits(param_arena(value)), bits(param_arena(one)))
+        assert torch.equal(bits(grad_arena(value)), bits(grad_arena(one)))
 
 
 def test_records_out_of_rank_order_are_flagged():
     S, H, I, n, chunk = SHAPES[0]
-    pp, cp, tcp, batch, masks = _case(S, H, I, n, 3, 3, False)
-    ranks, _, _ = _ranks(pp, cp, tcp, S, H, I, 3, chunk, batch, masks)
-    run_phases(ranks, order=[1, 0, 2])
-    assert all(rk.loss_bits()[1] & 2 for rk in ranks)
+    res = sharded_step(_case(S, H, I, n, 3, 3, False), S, H, I, 3, chunk, order={0: [1, 0, 2]})
+    assert all(isinstance(e, RuntimeError) and "disagree on the vocabulary shard plan" in str(e) for e in res), res
 
 
 # ----------------------------------------------------------------------------- the Python API at world 1
-@pytest.fixture
-def one_rank_group(tmp_path):
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    dist.init_process_group("nccl", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1,
-                            device_id=torch.device(DEV))
-    yield
-    dist.destroy_process_group()
-
-
 def _twins(S, H, I, variant):
     agents = []
     for _ in range(2):
@@ -178,9 +164,9 @@ def _ids_batch(rng, N, S, I):
 
 def _same_arenas(a, b):
     for k in a.nets:
-        assert torch.equal(_bits(param_arena(a.nets[k])), _bits(param_arena(b.nets[k]))), k
+        assert torch.equal(bits(param_arena(a.nets[k])), bits(param_arena(b.nets[k]))), k
     for k in ("policy_net", "value_net"):
-        assert torch.equal(_bits(grad_arena(a.nets[k])), _bits(grad_arena(b.nets[k]))), k
+        assert torch.equal(bits(grad_arena(a.nets[k])), bits(grad_arena(b.nets[k]))), k
 
 
 @pytest.mark.parametrize("variant", ["adam", "torch_sgd"])
@@ -323,6 +309,18 @@ def _run_agent(agent, dev):
     return outs
 
 
+def _agent_result(agent, dev):
+    """Two update() calls of a sharded agent: the losses, its replicated blocks and its critic's action block."""
+    outs = _run_agent(agent, dev)
+    vp = agent.nets["value_net"].__dict__["_recnn_vp"]
+    v = agent.nets["value_net"]
+    return {"outs": outs, "lo": vp.lo, "hi": vp.hi,
+            "rep": [p.detach().cpu().numpy() for p in list(v.parameters())[1:]]
+            + [v.linear1.weight.detach()[:, :52].cpu().numpy(),
+               agent.nets["policy_net"].linear1.weight.detach().cpu().numpy()],
+            "block": v.linear1.weight.detach()[:, 52:].cpu().numpy()}
+
+
 def _mp_worker(rank, world, port, q):
     import torch.distributed as dist
     os.environ["MASTER_ADDR"] = "127.0.0.1"
@@ -333,36 +331,16 @@ def _mp_worker(rank, world, port, q):
     try:
         agent = _agent(52, 64, 1003).to(dev)
         D.enable_vocab_parallel(agent)
-        outs = _run_agent(agent, dev)
-        vp = agent.nets["value_net"].__dict__["_recnn_vp"]
-        v = agent.nets["value_net"]
-        q.put((rank, {"outs": outs, "lo": vp.lo, "hi": vp.hi,
-                      "rep": [p.detach().cpu().numpy() for p in list(v.parameters())[1:]]
-                      + [v.linear1.weight.detach()[:, :52].cpu().numpy(),
-                         agent.nets["policy_net"].linear1.weight.detach().cpu().numpy()],
-                      "block": v.linear1.weight.detach()[:, 52:].cpu().numpy()}))
+        q.put((rank, _agent_result(agent, dev)))
         torch.cuda.synchronize()
-        vp.comm.close()
+        agent.nets["value_net"].__dict__["_recnn_vp"].comm.close()
     finally:
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("world", [2, 4, 8])
-def test_multi_process_equals_unsharded(world):
-    if torch.cuda.device_count() < world:
-        pytest.skip("needs %d GPUs" % world)
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_mp_worker, args=(r, world, port, q)) for r in range(world)]
-    for pr in procs:
-        pr.start()
-    res = dict(q.get(timeout=300) for _ in range(world))
-    for pr in procs:
-        pr.join(timeout=60)
-        assert pr.exitcode == 0
+def _check_against_unsharded(res, world):
+    """Every rank's losses and replicated blocks have the same bits; the losses and the critic's action blocks match
+    the unsharded agent's within the reordering bar."""
     full = _agent(52, 64, 1003).to(torch.device(DEV))
     want = _run_agent(full, torch.device(DEV))
     for r in range(world):
@@ -375,3 +353,23 @@ def test_multi_process_equals_unsharded(world):
     block = np.concatenate([res[r]["block"] for r in range(world)], 1)
     wref = full.nets["value_net"].linear1.weight.detach()[:, 52:].cpu().numpy()
     assert np.abs(block - wref).max() <= REORDER_BAR * np.abs(wref).max()
+
+
+@pytest.mark.parametrize("world", [2, 3])
+def test_virtual_ranks_run_reinforce_update(world):
+    """The multi-process test's agent on W virtual ranks: Reinforce.update() -> reinforce_update with the policy's
+    sharded draw, the all-reduced reward line, the sharded critic step and the sharded policy gradient."""
+    def rank(r):
+        ex = exchange()
+        agent = _agent(52, 64, 1003).to(torch.device(DEV))
+        lo, hi = D.vocab_shard(1003, r, world)
+        D.shard_in_place(agent.nets, D.VocabParallel(lo, hi, 1003, None, r, world, ex), None, agent.optimizers)
+        return _agent_result(agent, torch.device(DEV))
+    _check_against_unsharded(returned(run_ranks(world, rank)), world)
+
+
+@pytest.mark.parametrize("world", [2, 4, 8])
+def test_multi_process_equals_unsharded(world):
+    if torch.cuda.device_count() < world:
+        pytest.skip("needs %d GPUs" % world)
+    _check_against_unsharded(dict(spawn(_mp_worker, world)), world)

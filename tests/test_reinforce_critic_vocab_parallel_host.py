@@ -18,6 +18,7 @@ from recnn_b200 import _lib
 from recnn_b200 import dist as D
 from recnn_b200.nn.update import _ids
 from tests import _critic_vocab_oracle as CV
+from tests._ranks import one_rank_cpu_group  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WORLDS = [1, 2, 3, 8]
@@ -107,14 +108,6 @@ def test_an_id_outside_the_vocabulary_is_a_zero_term_on_every_rank(world):
 
 
 # ----------------------------------------------------------------------------- the agent-level plan and refusals
-@pytest.fixture
-def one_rank_cpu_group(tmp_path):
-    import torch.distributed as dist
-    dist.init_process_group("gloo", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1)
-    yield
-    dist.destroy_process_group()
-
-
 def _agent(S=6, H=8, I=10, critic_items=None):
     torch.manual_seed(0)
     policy = recnn_b200.nn.DiscreteActor(S, I, H)

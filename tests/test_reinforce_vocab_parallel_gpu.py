@@ -1,13 +1,12 @@
 """The vocabulary-parallel REINFORCE policy on the GPU.
 
 One GPU cannot run W > 1 ranks through the peer-memory protocol (every CTA of every rank must be resident at once; see
-test_comm_world1_gpu.py), so the maths is checked with VIRTUAL ranks on one device: the C phases of W shards run in one
-process, the all-gather is stood in for by concatenating the ranks' records in rank order (what recnn_comm_allgather
-delivers) and the layer-1 all-reduce by an in-order fp32 sum (the order allreduce_kernel sums in).  The transport itself
-is tested at world 1, and at W > 1 by the multi-process parametrisation, which needs W GPUs."""
+test_comm_world1_gpu.py), so W > 1 runs as VIRTUAL ranks on one device (tests/_ranks.py): W copies of the public API
+in one process, the all-gather delivering the ranks' records in rank order (what recnn_comm_allgather delivers) and the
+layer-1 all-reduce an in-order fp32 sum (the order allreduce_kernel sums in).  The transport itself is tested at world
+1, and at W > 1 by the multi-process parametrisation, which needs W GPUs."""
 from __future__ import annotations
 
-import ctypes
 import gc
 import os
 import subprocess
@@ -23,9 +22,9 @@ from recnn_b200 import dist as D
 from recnn_b200.nn.arena import param_arena, grad_arena
 from recnn_b200.utils.misc import DummyWriter
 from oracle import reinforce_oracle as RO
-from tests import _vocab_oracle as VO
+from tests._ranks import bits, chunked, one_rank_group, returned, run_ranks, shard, spawn  # noqa: F401
 from tests.test_comm_world1_gpu import World1Comm, _payload, CANARY
-from tests.test_reinforce_chunked_gpu import REORDER_BAR, make_policy, policy_grad, unpack
+from tests.test_reinforce_chunked_gpu import REORDER_BAR, make_policy, unpack
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -34,6 +33,9 @@ L = _lib.lib()
 # (S, H, items, rows, chunk): S % 4 == 0 (state read in place) and S % 4 != 0 (re-pitched image kept from the stats
 # phase); local slices chunked with a ragged last chunk (W = 1, 3) and narrower than one chunk (W = 8)
 SHAPES = [(52, 64, 1003, 40, 128), (37, 32, 2000, 33, 256)]
+METHODS = {RO.BASIC: recnn_b200.nn.ChooseREINFORCE.basic_reinforce,
+           RO.CORRECTED: recnn_b200.nn.ChooseREINFORCE.reinforce_with_correction,
+           RO.TOPK: recnn_b200.nn.ChooseREINFORCE.reinforce_with_TopK_correction}
 
 
 def _t(x, dtype=None):
@@ -41,136 +43,62 @@ def _t(x, dtype=None):
                                                                                                      device=DEV)
 
 
-class Virtual:
-    """W shards of one DiscreteActor as W modules on one device."""
-
-    def __init__(self, p, S, H, world):
-        self.items = p["w2"].shape[0]
-        self.world = world
-        self.shards = RO.shard_policy(p, world)
-        self.mods = [make_policy({"w1": p["w1"], "b1": p["b1"], "w2": sh["w2"], "b2": sh["b2"]}, S, H, len(sh["b2"]))
-                     for sh in self.shards]
-
-    def vs(self, r):
-        return _lib.VocabShard(self.shards[r]["offset"], self.items, r, self.world)
-
-    def grad(self, state, action, blp, ret, method, K, chunk, permute=None):
-        """Both phases on every rank: (losses, flags [W, 2], per-rank gradient dicts with the all-reduced layer 1)."""
-        n = state.shape[0]
-        st = _lib.stream_ptr()
-        recs, scratch, chunks = [], [], []
-        for r, m in enumerate(self.mods):
-            d = m.dims
-            c = chunk if chunk < d.num_items else d.num_items
-            chunks.append(c)
-            scratch.append(torch.empty(L.recnn_reinforce_scratch_floats(d, n, c), device=DEV))
-            recs.append(torch.empty(L.recnn_vocab_record_floats(n), device=DEV))
-            _lib.check(L.recnn_reinforce_shard_stats(d, self.vs(r), param_arena(m).data_ptr(), state.data_ptr(),
-                                                     action.data_ptr(), n, c, recs[r].data_ptr(),
-                                                     scratch[r].data_ptr(), st))
-        order = permute or list(range(self.world))
-        gathered = torch.cat([recs[q] for q in order])
-        grads, outs = [], []
-        for r, m in enumerate(self.mods):
-            g = torch.full_like(param_arena(m), float("nan"))
-            out = torch.zeros(3, device=DEV)
-            _lib.check(L.recnn_reinforce_shard_grad(m.dims, self.vs(r), param_arena(m).data_ptr(), g.data_ptr(),
-                                                    state.data_ptr(), action.data_ptr(), _lib.ptr(blp), ret.data_ptr(),
-                                                    n, method, K, chunks[r], gathered.data_ptr(), out.data_ptr(),
-                                                    scratch[r].data_ptr(), st))
-            grads.append(g)
-            outs.append(out)
-        layer1 = D.layer1_floats(self.mods[0].dims)
-        acc = grads[0][:layer1].clone()
-        for g in grads[1:]:
-            acc += g[:layer1]
-        for g in grads:
-            g[:layer1] = acc
-        torch.cuda.synchronize()
-        return ([float(o[0]) for o in outs], [o.view(torch.int32)[1:].tolist() for o in outs],
-                [unpack(g, m) for g, m in zip(grads, self.mods)])
-
-    def forward(self, state):
-        """(column blocks, gathered records) of the sharded forward."""
-        n = state.shape[0]
-        st = _lib.stream_ptr()
-        blocks, recs = [], []
-        for r, m in enumerate(self.mods):
-            d = m.dims
-            blocks.append(torch.empty(n, d.num_items, device=DEV))
-            recs.append(torch.empty(L.recnn_vocab_record_floats(n), device=DEV))
-            scratch = torch.empty(L.recnn_discrete_scratch_floats(d, n, 0), device=DEV)
-            _lib.check(L.recnn_discrete_shard_forward(d, self.vs(r), param_arena(m).data_ptr(), state.data_ptr(), n,
-                                                      blocks[r].data_ptr(), recs[r].data_ptr(), scratch.data_ptr(), st))
-        gathered = torch.cat(recs)
-        flag = torch.zeros(1, dtype=torch.int32, device=DEV)
-        for r, m in enumerate(self.mods):
-            _lib.check(L.recnn_discrete_shard_finish(m.dims, self.vs(r), gathered.data_ptr(), n, blocks[r].data_ptr(),
-                                                     flag.data_ptr(), st))
-        assert int(flag) == 0
-        return blocks, gathered
-
-    def _pick(self, draws, n):
-        action = torch.empty(n, dtype=torch.int64, device=DEV)
-        logp = torch.empty(n, device=DEV)
-        flag = torch.zeros(1, dtype=torch.int32, device=DEV)
-        _lib.check(L.recnn_discrete_shard_pick(self.world, torch.cat(draws).data_ptr(), n, action.data_ptr(),
-                                               logp.data_ptr(), flag.data_ptr(), _lib.stream_ptr()))
-        return action, logp, int(flag)
-
-    def sample(self, blocks, gathered, uniforms=None, seed=0, draw=1):
-        n = blocks[0].shape[0]
-        draws = []
-        for r, m in enumerate(self.mods):
-            draws.append(torch.empty(2 * n, device=DEV))
-            _lib.check(L.recnn_discrete_shard_sample(m.dims, self.vs(r), gathered.data_ptr(), blocks[r].data_ptr(), n,
-                                                     _lib.ptr(uniforms), seed, draw, draws[r].data_ptr(),
-                                                     _lib.stream_ptr()))
-        return self._pick(draws, n)
-
-    def log_prob(self, blocks, action):
-        n = blocks[0].shape[0]
-        draws, oob = [], torch.zeros(1, dtype=torch.int32, device=DEV)
-        for r, m in enumerate(self.mods):
-            draws.append(torch.empty(2 * n, device=DEV))
-            _lib.check(L.recnn_discrete_shard_log_prob(m.dims, self.vs(r), blocks[r].data_ptr(), n, action.data_ptr(),
-                                                       draws[r].data_ptr(), oob.data_ptr(), _lib.stream_ptr()))
-        a, lp, flag = self._pick(draws, n)
-        return lp, flag, int(oob)
+def _edges(I, world):
+    """Every shard's first item, last item and the item before it."""
+    return sorted({e for r in range(world) for lo, hi in [D.vocab_shard(I, r, world)] for e in (lo - 1, lo, hi - 1)
+                   if 0 <= e < I})
 
 
 def _case(S, H, I, R, seed, world):
+    """(parameters, state, action, beta log-probs, per-row returns): each row is one saved env step."""
     rng = np.random.default_rng(seed)
     p = RO.make_discrete_actor(rng, S, I, H)
     state = rng.normal(0, 1, (R, S)).astype(np.float32)
     blp = np.log(rng.uniform(1e-4, 5e-4, R)).astype(np.float32)
     ret = rng.normal(0, 1, R).astype(np.float32)
     action = rng.integers(0, I, R)
-    edges = sorted({e for sh in RO.shard_policy(p, world)
-                    for e in (sh["offset"] - 1, sh["offset"], sh["offset"] + len(sh["b2"]) - 1) if 0 <= e < I})
+    edges = _edges(I, world)
     action[:len(edges)] = edges[:R]
     return p, state, action, blp, ret
 
 
+def policy_loss(m, state, action, blp, ret, method, K=10):
+    """(loss, gradient dict) of the ChooseREINFORCE method on ``m`` with one saved env step per row and the given
+    per-row returns.  The gradient arena starts as NaN: the call must write every entry."""
+    m._saved = [{"state": state[i:i + 1], "action": action[i:i + 1],
+                 "beta_log_prob": None if method == RO.BASIC else blp[i:i + 1], "K": K} for i in range(len(state))]
+    grad_arena(m).fill_(float("nan"))
+    loss = METHODS[method](m, torch.from_numpy(ret))
+    return loss, {k: v.clone() for k, v in unpack(grad_arena(m), m).items()}
+
+
+def sharded_loss(full, world, *args, chunk=None, order=None):
+    """policy_loss on W virtual ranks sharded from ``full``, each rank's (loss, gradients) or exception."""
+    def rank(r):
+        return policy_loss(shard({"policy_net": full})[0]["policy_net"], *args)
+    with chunked(args[0].shape[0], chunk):
+        return run_ranks(world, rank, order=order)
+
+
 def run_virtual_sweep():
     """Every shape x W x method: loss and gradients against the float64 oracle (the chunked-gradient tests' bar) and
-    against the unsharded chunked CUDA call (reordering bar); the loss has the same bits on every rank."""
+    against the unsharded chunked policy update (reordering bar); the loss has the same bits on every rank."""
     for S, H, I, R, chunk in SHAPES:
         for world in (1, 2, 3, 8):
             p, state, action, blp, ret = _case(S, H, I, R, S + I + world, world)
-            v = Virtual(p, S, H, world)
             full = make_policy(p, S, H, I)
-            st, at, bt, rt = _t(state), _t(action), _t(blp), _t(ret)
+            st, at, bt = _t(state), _t(action), _t(blp)
             for method in (RO.BASIC, RO.CORRECTED, RO.TOPK):
-                beta = None if method == RO.BASIC else bt
-                losses, flags, grads = v.grad(st, at, beta, rt, method, 10, chunk)
-                assert flags == [[0, 0]] * world, flags
-                assert len({np.float32(x).tobytes() for x in losses}) == 1, losses
-                want_loss, want, _ = RO.reinforce_policy_grad(p, state, action, None if beta is None else blp, ret,
-                                                              method, 10)
-                one_loss, _, one = policy_grad(full, st, at, beta, rt, method, 10, chunk)
-                assert losses[0] == pytest.approx(want_loss, rel=2e-4, abs=1e-4 * (1 + abs(want_loss)))
-                assert losses[0] == pytest.approx(one_loss, rel=1e-5, abs=1e-6)
+                res = returned(sharded_loss(full, world, st, at, bt, ret, method, chunk=chunk))
+                losses, grads = [x[0] for x in res], [x[1] for x in res]
+                assert len({bits(x).item() for x in losses}) == 1, losses
+                want_loss, want, _ = RO.reinforce_policy_grad(p, state, action, None if method == RO.BASIC else blp,
+                                                              ret, method, 10)
+                with chunked(R, chunk):
+                    one_loss, one = policy_loss(full, st, at, bt, ret, method)
+                loss = float(losses[0])
+                assert loss == pytest.approx(want_loss, rel=2e-4, abs=1e-4 * (1 + abs(want_loss)))
+                assert loss == pytest.approx(float(one_loss), rel=1e-5, abs=1e-6)
                 got = {"w1": grads[0]["w1"], "b1": grads[0]["b1"],
                        "w2": torch.cat([g["w2"] for g in grads]), "b2": torch.cat([g["b2"] for g in grads])}
                 for k in got:
@@ -203,22 +131,22 @@ def test_virtual_ranks_on_the_cuda_core_back_end():
 @pytest.mark.parametrize("S,H,I,R,chunk", SHAPES)
 def test_world1_is_bit_identical_to_the_chunked_call(S, H, I, R, chunk):
     p, state, action, blp, ret = _case(S, H, I, R, 3 * S, 1)
-    v = Virtual(p, S, H, 1)
-    st, at, bt, rt = _t(state), _t(action), _t(blp), _t(ret)
+    full = make_policy(p, S, H, I)
+    st, at, bt = _t(state), _t(action), _t(blp)
     for method in (RO.BASIC, RO.TOPK):
-        beta = None if method == RO.BASIC else bt
-        losses, flags, grads = v.grad(st, at, beta, rt, method, 10, chunk)
-        loss, _, want = policy_grad(v.mods[0], st, at, beta, rt, method, 10, chunk)
-        assert np.float32(losses[0]).tobytes() == np.float32(loss).tobytes()
+        (loss, grads), = returned(sharded_loss(full, 1, st, at, bt, ret, method, chunk=chunk))
+        with chunked(R, chunk):
+            want_loss, want = policy_loss(full, st, at, bt, ret, method)
+        assert bits(loss).item() == bits(want_loss).item()
         for k in want:
-            assert torch.equal(grads[0][k], want[k]), k
+            assert torch.equal(grads[k], want[k]), k
 
 
 def test_gathered_records_out_of_rank_order_are_flagged():
     p, state, action, blp, ret = _case(52, 64, 1003, 40, 5, 3)
-    v = Virtual(p, 52, 64, 3)
-    _, flags, _ = v.grad(_t(state), _t(action), None, _t(ret), RO.BASIC, 1, 128, permute=[1, 0, 2])
-    assert all(f[1] == 1 for f in flags), flags
+    full = make_policy(p, 52, 64, 1003)
+    res = sharded_loss(full, 3, _t(state), _t(action), None, ret, RO.BASIC, chunk=128, order={0: [1, 0, 2]})
+    assert all(isinstance(e, RuntimeError) and "disagree on the vocabulary shard plan" in str(e) for e in res), res
 
 
 # ----------------------------------------------------------------------------- forward and draws
@@ -227,21 +155,38 @@ def _forward_case(world, n=300, S=52, H=64, I=1003, seed=0):
     p = RO.make_discrete_actor(rng, S, I, H)
     p["w2"] = (p["w2"] * 6).astype(np.float32)
     state = rng.normal(0, 1, (n, S)).astype(np.float32)
-    return p, state, Virtual(p, S, H, world), make_policy(p, S, H, I)
+    return p, state, make_policy(p, S, H, I)
+
+
+def sharded_draws(full, world, state, uniforms=None, ids=()):
+    """On W virtual ranks: (column block, sampled ids, their log-probs, [log-probs of each ``ids`` tensor]) from
+    policy._pi, policy._sample and policy._shard_log_prob, or the rank's exception."""
+    def rank(r):
+        pol = shard({"policy_net": full})[0]["policy_net"]
+        pol.uniform_source = None if uniforms is None else (lambda n: uniforms)
+        probs, gathered = pol._pi(state)
+        a, lp = pol._sample(probs, gathered)
+        return probs, a, lp, [pol._shard_log_prob(probs, x) for x in ids]
+    return run_ranks(world, rank)
 
 
 @pytest.mark.parametrize("world", [2, 3, 8])
 def test_forward_blocks_and_replayed_draws(world):
-    p, state, v, full = _forward_case(world)
+    p, state, full = _forward_case(world)
     st = _t(state)
-    blocks, gathered = v.forward(st)
-    probs = torch.cat(blocks, 1)
+    u = np.random.default_rng(world).random(state.shape[0]).astype(np.float32)
+    # the log-prob of given ids at every shard edge
+    edges = _edges(1003, world)
+    ids = np.random.default_rng(1).integers(0, 1003, state.shape[0])
+    ids[:len(edges)] = edges
+    res = returned(sharded_draws(full, world, st, _t(u), [_t(ids)]))
+    probs = torch.cat([x[0] for x in res], 1)
     want = full(st)
     assert float((probs - want).abs().max()) <= 1e-6 * float(want.abs().max())
     assert float((probs.double().sum(1) - 1).abs().max()) <= 1e-5
-    u = np.random.default_rng(world).random(state.shape[0]).astype(np.float32)
-    a, lp, flag = v.sample(blocks, gathered, uniforms=_t(u))
-    assert flag == 0
+    a, lp, (lp2,) = res[0][1:]
+    for x in res[1:]:
+        assert torch.equal(x[1], a) and torch.equal(x[2], lp) and torch.equal(x[3][0], lp2)
     full.uniform_source = lambda n: u
     ref_a, ref_lp = full._sample(want)
     _, _, margin = RO.categorical_sample(want.double().cpu().numpy(), u)
@@ -249,35 +194,25 @@ def test_forward_blocks_and_replayed_draws(world):
     assert int(keep.sum()) > 0.9 * state.shape[0]
     assert torch.equal(a[keep], ref_a[keep])
     assert float((lp[keep] - ref_lp[keep]).abs().max()) <= 1e-5
-    # the log-prob of given ids at every shard edge
-    edges = sorted({e for sh in v.shards for e in (sh["offset"] - 1, sh["offset"], sh["offset"] + len(sh["b2"]) - 1)
-                    if 0 <= e < 1003})
-    ids = np.random.default_rng(1).integers(0, 1003, state.shape[0])
-    ids[:len(edges)] = edges
-    lp2, flag2, oob = v.log_prob(blocks, _t(ids))
-    assert flag2 == 0 and oob == 0
     want_lp = RO.categorical_log_prob(want.double().cpu().numpy(), ids)
     assert np.abs(lp2.cpu().numpy() - want_lp).max() <= 1e-5
     ids[3] = 1003
-    _, flag3, oob3 = v.log_prob(blocks, _t(ids))
-    assert oob3 == 1 and flag3 == 1
+    res = sharded_draws(full, world, st, _t(u), [_t(ids)])
+    assert all(isinstance(e, IndexError) for e in res), res
 
 
 def test_world1_forward_and_draws_are_bit_identical():
-    p, state, v, full = _forward_case(1)
+    p, state, full = _forward_case(1)
     st = _t(state)
-    blocks, gathered = v.forward(st)
     want = full(st)
-    assert torch.equal(blocks[0], want)
     u = _t(np.random.default_rng(2).random(state.shape[0]).astype(np.float32))
     for uniforms in (u, None):
-        a, lp, flag = v.sample(blocks, gathered, uniforms=uniforms, seed=1234, draw=5)
-        ra = torch.empty_like(a)
-        rl = torch.empty_like(lp)
-        _lib.check(L.recnn_categorical_sample(want.data_ptr(), want.shape[0], want.shape[1], want.stride(0),
-                                              _lib.ptr(uniforms), 1234, 5, ra.data_ptr(), rl.data_ptr(),
-                                              _lib.stream_ptr()))
-        assert flag == 0
+        torch.manual_seed(1234)
+        (probs, a, lp, _), = returned(sharded_draws(full, 1, st, uniforms))
+        assert torch.equal(probs, want)
+        full.uniform_source = None if uniforms is None else (lambda n: uniforms)
+        full._draws = 0
+        ra, rl = full._sample(want)
         assert torch.equal(a, ra) and torch.equal(lp, rl)
 
 
@@ -285,12 +220,11 @@ def test_philox_draws_follow_the_softmax_at_w3():
     """One state repeated over 60,000 rows, 13 items over 3 ranks (5, 5, 3): the seeded Philox draws pass a
     chi-square test against the softmax."""
     from scipy.stats import chisquare
-    p, _, v, full = _forward_case(3, S=8, H=16, I=13, seed=40)
+    p, _, full = _forward_case(3, S=8, H=16, I=13, seed=40)
     rng = np.random.default_rng(9)
     state = np.repeat(rng.normal(0, 1, (1, 8)).astype(np.float32), 60_000, 0)
-    blocks, gathered = v.forward(_t(state))
-    a, _, flag = v.sample(blocks, gathered, seed=777, draw=3)
-    assert flag == 0
+    torch.manual_seed(777)
+    a = returned(sharded_draws(full, 3, _t(state)))[0][1]
     counts = np.bincount(a.cpu().numpy(), minlength=13)
     probs = full(_t(state[:1])).double().cpu().numpy()[0]
     probs /= probs.sum()
@@ -331,16 +265,6 @@ def test_allgather_moves_every_bit_pattern_and_interleaves_with_allreduce():
 
 
 # ----------------------------------------------------------------------------- the Python API at world 1
-@pytest.fixture
-def one_rank_group(tmp_path):
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    dist.init_process_group("nccl", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1,
-                            device_id=torch.device(DEV))
-    yield
-    dist.destroy_process_group()
-
-
 def _policy_pair(S, H, I, seed):
     torch.manual_seed(seed)
     a = recnn_b200.nn.DiscreteActor(S, I, H).to(DEV)
@@ -348,10 +272,6 @@ def _policy_pair(S, H, I, seed):
     b.load_state_dict(a.state_dict())
     D.enable_vocab_parallel(b)
     return a, b
-
-
-def _bits(t):
-    return t.detach().contiguous().view(torch.int32).cpu()
 
 
 @pytest.mark.parametrize("variant", ["basic_adam", "topk_torch_sgd"])
@@ -385,9 +305,9 @@ def test_python_api_world1_equals_unsharded(one_rank_group, variant):
                 for x, y in zip(getattr(plain, k), getattr(shard, k)):
                     assert torch.equal(x, y), k
         losses = [recnn_b200.nn.ChooseREINFORCE(method)(m, o) for m, o in zip((plain, shard), opts)]
-        assert _bits(losses[0]).tolist() == _bits(losses[1]).tolist()
-        assert torch.equal(_bits(param_arena(plain)), _bits(param_arena(shard))), update
-        assert torch.equal(_bits(grad_arena(plain)), _bits(grad_arena(shard))), update
+        assert bits(losses[0]).tolist() == bits(losses[1]).tolist()
+        assert torch.equal(bits(param_arena(plain)), bits(param_arena(shard))), update
+        assert torch.equal(bits(grad_arena(plain)), bits(grad_arena(shard))), update
     # error paths on the sharded policy
     shard._saved.append({"state": state, "action": torch.full((N,), I, dtype=torch.int64, device=DEV),
                          "beta_log_prob": None})
@@ -399,6 +319,30 @@ def test_python_api_world1_equals_unsharded(one_rank_group, variant):
     with pytest.raises(RuntimeError, match="ChooseREINFORCE"):
         recnn_b200.nn.reinforce_update({"state": state, "action": torch.zeros(N, I)}, {}, {"policy_net": shard}, {})
     vp.comm.close()
+
+
+def test_a_communicator_that_cannot_be_mapped_leaves_the_nets_unsharded(one_rank_group, monkeypatch):
+    """The communicator is made before the nets are broadcast or sharded.  At world 1 the plan is every item, so
+    sharding keeps the shapes but replaces every parameter's storage: the storage must be the same after the refusal."""
+    torch.manual_seed(3)
+    agent = recnn_b200.nn.Reinforce(recnn_b200.nn.DiscreteActor(52, 1003, 64),
+                                    recnn_b200.nn.Critic(52, 1003, 64)).to(torch.device(DEV))
+    beta = recnn_b200.nn.Beta(52, 1003).to(DEV)
+    nets = dict(agent.nets, beta=beta)
+    shapes = {k: [tuple(p.shape) for p in net.parameters()] for k, net in nets.items()}
+    storage = {k: [param_arena(net).data_ptr()] + [p.data_ptr() for p in net.parameters()] for k, net in nets.items()}
+    values = {k: bits(param_arena(net)) for k, net in nets.items()}
+
+    def unavailable(*args, **kwargs):
+        raise _lib.RecnnError("peer-memory communicator unavailable: no peer access")
+    monkeypatch.setattr(D, "PeerComm", unavailable)
+    with pytest.raises(_lib.RecnnError, match="unavailable"):
+        D.enable_vocab_parallel(agent, beta=beta)
+    for k, net in nets.items():
+        assert [tuple(p.shape) for p in net.parameters()] == shapes[k], k
+        assert [param_arena(net).data_ptr()] + [p.data_ptr() for p in net.parameters()] == storage[k], k
+        assert torch.equal(bits(param_arena(net)), values[k]), k
+        assert "_recnn_vp" not in net.__dict__, k
 
 
 # ----------------------------------------------------------------------------- one rank's share of config 5
@@ -486,18 +430,7 @@ def _vp_worker(rank, world, port, q):
 def test_multi_process_equals_unsharded(world):
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_vp_worker, args=(r, world, port, q)) for r in range(world)]
-    for pr in procs:
-        pr.start()
-    res = dict(q.get(timeout=300) for _ in range(world))
-    for pr in procs:
-        pr.join(timeout=60)
-        assert pr.exitcode == 0
+    res = dict(spawn(_vp_worker, world))
     S, H, I, R = 52, 64, 1003, 48
     p, state, action, blp, ret = _case(S, H, I, R, 77, world)
     full = make_policy(p, S, H, I)

@@ -14,6 +14,7 @@ import torch
 import recnn_b200
 from recnn_b200 import dist as D
 from recnn_b200.nn.arena import param_arena
+from tests._ranks import one_rank_group, spawn  # noqa: F401
 from tests.test_beta_vocab_parallel_gpu import _notebook_agent
 from tests.test_vocab_checkpoint_host import _full_state, _same
 
@@ -21,16 +22,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 S, H, ITEMS, N = 37, 64, 1003, 10              # the shapes _notebook_agent builds
 SOURCE = {"pi": "pi", "beta": "beta"}
-
-
-@pytest.fixture
-def one_rank_group(tmp_path):
-    import torch.distributed as dist
-    torch.cuda.set_device(0)
-    dist.init_process_group("nccl", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1,
-                            device_id=torch.device(DEV))
-    yield
-    dist.destroy_process_group()
 
 
 def _batch(step):
@@ -153,12 +144,10 @@ def test_virtual_ranks_on_one_device(one_rank_group, monkeypatch, world):
     ranks = []
     for r in range(world):
         lo, hi = D.vocab_shard(ITEMS, r, world)
-        agent = recnn_b200.nn.Reinforce(recnn_b200.nn.DiscreteActor(S, hi - lo, H).to(DEV),
-                                        recnn_b200.nn.Critic(S, hi - lo, H).to(DEV)).to(torch.device(DEV))
-        beta = recnn_b200.nn.Beta(S, hi - lo).to(DEV)
-        vp = D.VocabParallel(lo, hi, ITEMS, None, r, world, None)
-        for net in list(agent.nets.values()) + [beta]:
-            net.__dict__["_recnn_vp"] = vp
+        agent = recnn_b200.nn.Reinforce(recnn_b200.nn.DiscreteActor(S, ITEMS, H).to(DEV),
+                                        recnn_b200.nn.Critic(S, ITEMS, H).to(DEV)).to(torch.device(DEV))
+        beta = recnn_b200.nn.Beta(S, ITEMS).to(DEV)
+        D.shard_in_place(agent.nets, D.VocabParallel(lo, hi, ITEMS, None, r, world, None), beta, agent.optimizers)
         D.load_vocab_parallel_state(agent, full, beta=beta)
         assert torch.equal(beta.net[0].weight, plain_beta.net[0].weight[lo:hi])
         assert torch.equal(agent.nets["target_value_net"].linear1.weight[:, S:],
@@ -251,18 +240,7 @@ def _near(got, want, atol):
 def test_multi_process_gather_and_resume_at_another_world_size(tmp_path, world):
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
-    import socket
-    import torch.multiprocessing as mp
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_mp_worker, args=(r, world, port, str(tmp_path / "ckpt.pt"), q)) for r in range(world)]
-    for pr in procs:
-        pr.start()
-    ckpt, (losses, resumed) = q.get(timeout=600)
-    for pr in procs:
-        pr.join(timeout=120)
-        assert pr.exitcode == 0
+    (ckpt, (losses, resumed)), = spawn(_mp_worker, world, str(tmp_path / "ckpt.pt"), items=1, timeout=600)
     torch.cuda.set_device(0)
     plain, plain_beta = _trained(False)
     # Ranger / RAdam at lr 1e-5: a reordered gradient sum moves a weight by at most a few steps of 1e-5

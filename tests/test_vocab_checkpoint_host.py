@@ -12,17 +12,10 @@ import torch
 import recnn_b200
 from recnn_b200 import dist as D
 from recnn_b200.nn.arena import _views, param_arena
+from tests._ranks import one_rank_cpu_group  # noqa: F401
 
 S, H, ITEMS = 13, 10, 1003          # S % 4 != 0 and H % 4 != 0: every pitch pads; 1003 is not divisible by 2, 3 or 8
 KINDS = ["sgd", "adam", "ranger", "radam", "torch_adam"]
-
-
-@pytest.fixture
-def one_rank_cpu_group(tmp_path):
-    import torch.distributed as dist
-    dist.init_process_group("gloo", init_method="file://" + str(tmp_path / "pg"), rank=0, world_size=1)
-    yield
-    dist.destroy_process_group()
 
 
 def _optimizer(kind, net):
@@ -75,10 +68,8 @@ def _full_state(agent, beta):
 
 
 def _local(kind, lo, hi, rank, world):
-    agent, beta = _agent(kind, hi - lo)
-    vp = D.VocabParallel(lo, hi, ITEMS, None, rank, world, None)
-    for net in list(agent.nets.values()) + [beta]:
-        net.__dict__["_recnn_vp"] = vp
+    agent, beta = _agent(kind, ITEMS)
+    D.shard_in_place(agent.nets, D.VocabParallel(lo, hi, ITEMS, None, rank, world, None), beta, agent.optimizers)
     return agent, beta
 
 
