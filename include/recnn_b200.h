@@ -350,6 +350,13 @@ RECNN_API int recnn_categorical_sample(const float* probs, int64_t n_rows, int32
                                        const float* uniforms, uint64_t seed, int64_t draw, int64_t* action_out,
                                        float* log_prob_out, void* stream);
 /* Categorical(probs).log_prob(action) for given actions; *oob_flag (may be NULL) is set when an id is out of range */
+/* recnn_categorical_sample for the rows [row_offset, row_offset + n_rows) of a larger batch: the uniform of local row r
+ * is Philox(seed, draw, row_offset + r) (uniforms, when given, stay local: uniforms[r]).  A data-parallel rank holding
+ * global rows [lo, hi) thus draws what the single-GPU call over the whole batch draws for them; row_offset 0 is
+ * recnn_categorical_sample. */
+RECNN_API int recnn_categorical_sample_at(const float* probs, int64_t n_rows, int32_t num_items, int64_t ld,
+                                          const float* uniforms, uint64_t seed, int64_t draw, int64_t row_offset,
+                                          int64_t* action_out, float* log_prob_out, void* stream);
 RECNN_API int recnn_categorical_log_prob(const float* probs, int64_t n_rows, int32_t num_items, int64_t ld,
                                          const int64_t* action, float* log_prob_out, int32_t* oob_flag, void* stream);
 /* ChooseREINFORCE (recnn/nn/update/reinforce.py:10-65): the three policy losses */
@@ -559,6 +566,39 @@ RECNN_API int recnn_discrete_value_shard_merge(const recnn_discrete_value_args* 
 RECNN_API int recnn_discrete_value_shard_end(const recnn_discrete_value_args* args, const recnn_vocab_shard* v,
                                              const float* terms, void* stream);
 
+/* ---- REINFORCE: the item-id critic data-parallel over the rows of the batch --------------------------
+ * Every rank holds full replicas of both critics and the target policy and the rows [row_offset, row_offset + n_rows)
+ * of a batch of n_rows_global rows.  args is recnn_discrete_value_step's for the rank's rows.  Two phases on one stream,
+ * with two exchanges between them, replace the step:
+ *   dp_begin -> the action terms, the target critic, TD target and clamp, the online critic (dropout masks, when not
+ *               given, keyed by the GLOBAL row: the masks of the single-GPU step's rows), the MSE as this rank's partial
+ *               sum over 1 / n_rows_global and the backward down to dz1.  It writes two messages:
+ *      grad_msg (recnn_discrete_value_dp_grad_floats(d) = H (pad4(S) + H + 3) + 3 floats): the replicated part of the
+ *               gradient -- W1's state block [H, pad4(S)] (pads zero), b1, W2 [H, H], b2, W3, b3 -- then the loss
+ *               partial and 1.0 when an action id is outside [0, num_items).  Independent of num_items -> all-reduce
+ *               (recnn_comm_allreduce).
+ *      record   (recnn_discrete_value_dp_record_floats(d, record_rows), record_rows >= n_rows the same on every rank):
+ *               int32 header {row_offset, n_rows, n_rows_global, 0}, the ids as int32 (pad4(record_rows) words), then
+ *               dz1 [n_rows, H] -> all-gather (recnn_comm_allgather), rank order.
+ *   dp_end   -> checks the gathered headers (bit 2 unless they tile [0, n_rows_global) in order, each within record_rows,
+ *               all with this rank's n_rows_global); the reduced gradient and loss into value.grads and losses[0]; the
+ *               action block zeroed and every selected column the ascending-(id, global row) sum of the gathered dz1
+ *               rows; the built-in optimizer (RECNN_OPT_EXTERNAL: stop after the gradient), skipped on the device when
+ *               either error bit is set; ++rng_step, losses[4] and the host copy.
+ * Every rank computes the same bits.  At world 1 (row_offset 0, n_rows_global = n_rows) the pair computes exactly what
+ * recnn_discrete_value_step does.  The phases share args->workspace (recnn_discrete_value_dp_workspace_bytes), which
+ * must be left untouched between them. */
+RECNN_API int64_t recnn_discrete_value_dp_grad_floats(const recnn_dims* d);
+RECNN_API int64_t recnn_discrete_value_dp_record_floats(const recnn_dims* d, int64_t record_rows);
+RECNN_API int64_t recnn_discrete_value_dp_workspace_bytes(const recnn_dims* d, const recnn_discrete_dims* pd,
+                                                          int64_t n_rows, int64_t n_rows_global, int32_t chunk_items);
+RECNN_API int recnn_discrete_value_dp_begin(const recnn_discrete_value_args* args, int64_t row_offset,
+                                            int64_t n_rows_global, int64_t record_rows, float* grad_msg, float* record,
+                                            void* stream);
+RECNN_API int recnn_discrete_value_dp_end(const recnn_discrete_value_args* args, int64_t row_offset,
+                                          int64_t n_rows_global, int32_t world, int64_t record_rows,
+                                          const float* grad_msg, const float* gathered, void* stream);
+
 /* ---- REINFORCE with Top-K correction: the behaviour policy beta ------------------------------------
  * The reference ships beta in its Top-K notebook, not in the library (examples/2. REINFORCE TopK Off Policy
  * Correction/3. TopK Reinforce Off Policy Correction.ipynb, cell 3: class Beta), and DiscreteActor.pi_beta_sample
@@ -580,7 +620,9 @@ typedef struct recnn_beta_args {
   recnn_beta_dims dims;
   int64_t n_rows;
   int32_t chunk_items;
-  int32_t reserved;
+  int32_t n_rows_global;      /* 0: n_rows.  Else the rows of the whole batch when this call holds a data-parallel
+                               * rank's rows: the loss and the gradient are then this rank's partial sums of the mean
+                               * over n_rows_global rows (sum them over the ranks, then step the optimizer) */
   recnn_net net;              /* params, grads (required), opt_m / opt_v / opt_t for the built-in optimizer */
   recnn_optim optim;          /* RECNN_OPT_EXTERNAL: stop after the gradient (left in net.grads) */
   const float* state;         /* [n_rows, state_ld] */

@@ -89,7 +89,7 @@ class BetaDims(C.Structure):
 
 class BetaArgs(C.Structure):
     _fields_ = [
-        ("dims", BetaDims), ("n_rows", C.c_int64), ("chunk_items", C.c_int32), ("reserved", C.c_int32),
+        ("dims", BetaDims), ("n_rows", C.c_int64), ("chunk_items", C.c_int32), ("n_rows_global", C.c_int32),
         ("net", Net), ("optim", Optim),
         ("state", C.c_void_p), ("state_ld", C.c_int64), ("action", C.c_void_p), ("probs_out", C.c_void_p),
         ("loss", C.c_void_p), ("error", C.c_void_p),
@@ -98,7 +98,7 @@ class BetaArgs(C.Structure):
 
 
 _BETA_PROBE_FIELDS = ["dims", "n_rows", "net", "optim", "state", "action", "probs_out", "loss", "error",
-                      "workspace_bytes"]
+                      "workspace_bytes", "n_rows_global"]
 
 _PROBE_FIELDS =["dims", "n_rows", "table", "policy", "policy_optim", "gamma", "soft_tau", "masks", "seed",
                  "losses", "workspace_bytes", "comm"]
@@ -148,6 +148,8 @@ SIGNATURES = {
                                          C.c_void_p, C.c_void_p]),
     "recnn_categorical_sample": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_uint64,
                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_categorical_sample_at": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_uint64,
+                                              C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_categorical_log_prob": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
                                              C.c_void_p, C.c_void_p]),
     "recnn_reinforce_policy_grad": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -195,6 +197,14 @@ SIGNATURES = {
     "recnn_discrete_value_workspace_bytes": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                          C.c_int32]),
     "recnn_discrete_value_step": (C.c_int, [C.POINTER(DiscreteValueArgs), C.c_void_p]),
+    "recnn_discrete_value_dp_grad_floats": (C.c_int64, [C.POINTER(Dims)]),
+    "recnn_discrete_value_dp_record_floats": (C.c_int64, [C.POINTER(Dims), C.c_int64]),
+    "recnn_discrete_value_dp_workspace_bytes": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
+                                                            C.c_int64, C.c_int32]),
+    "recnn_discrete_value_dp_begin": (C.c_int, [C.POINTER(DiscreteValueArgs), C.c_int64, C.c_int64, C.c_int64,
+                                                C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_value_dp_end": (C.c_int, [C.POINTER(DiscreteValueArgs), C.c_int64, C.c_int64, C.c_int32,
+                                              C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_discrete_value_shard_begin": (C.c_int, [C.POINTER(DiscreteValueArgs), C.POINTER(VocabShard), C.c_void_p,
                                                    C.c_void_p]),
     "recnn_discrete_value_shard_merge": (C.c_int, [C.POINTER(DiscreteValueArgs), C.POINTER(VocabShard), C.c_void_p,

@@ -214,6 +214,7 @@ extern "C" int64_t recnn_offsetof_beta_args(int field) {
     case 7: return offsetof(recnn_beta_args, loss);
     case 8: return offsetof(recnn_beta_args, error);
     case 9: return offsetof(recnn_beta_args, workspace_bytes);
+    case 10: return offsetof(recnn_beta_args, n_rows_global);
     default: return -1;
   }
 }
@@ -224,6 +225,7 @@ static int beta_check(const recnn_beta_args* a, BetaWorkspace* w) {
   RECNN_REQUIRE(a != nullptr, "args");
   RECNN_REQUIRE(beta_dims_ok(&a->dims), "dims");
   RECNN_REQUIRE(a->n_rows > 0, "n_rows");
+  RECNN_REQUIRE(a->n_rows_global == 0 || a->n_rows_global >= a->n_rows, "n_rows_global is 0 or at least n_rows");
   const int S = a->dims.state_dim, I = a->dims.num_items, W = a->chunk_items;
   RECNN_REQUIRE(chunk_ok(I, W), "chunk_items must be num_items or a positive multiple of 128 below it");
   const int64_t widest = pad4(S) > W ? pad4(S) : W;
@@ -268,12 +270,13 @@ static int beta_grad_pass(const recnn_beta_args* a, const BetaWorkspace& w, int 
   float* G = a->net.grads;
   const long long* act = reinterpret_cast<const long long*>(a->action);
   const Seg xs = state_seg(S, a->state, a->state_ld, w.img);     // what pass 1 left
-  sum_rows_kernel<<<1, 1024, 0, st>>>(w.row_loss, n, (float)(1.0 / (double)n), a->loss);
+  const double n_mean = a->n_rows_global > 0 ? (double)a->n_rows_global : (double)n;   // the cross-entropy's mean
+  sum_rows_kernel<<<1, 1024, 0, st>>>(w.row_loss, n, (float)(1.0 / n_mean), a->loss);
   RECNN_CHECK_LAUNCH("sum_rows_kernel");
   for (int c0 = 0; c0 < I; c0 += W) {
     const int wc = I - c0 < W ? I - c0 : W;
     beta_dz_kernel<<<row_grid(n), kRowThreads, 0, st>>>(a->probs_out, I, n, wc, c0, lo, items, act, w.T, w.pe, w.pa,
-                                                        (float)(1.0 / (double)n), w.dz);
+                                                        (float)(1.0 / n_mean), w.dz);
     RECNN_CHECK_LAUNCH("beta_dz_kernel");
     RECNN_PROPAGATE(weight_grad(w.dz, wc, xs, kNoSeg, n, G + l.w + (int64_t)c0 * l.ldw, l.ldw, G + l.b + c0, w.partial,
                                 st));

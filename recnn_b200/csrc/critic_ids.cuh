@@ -406,20 +406,20 @@ static int dv_action_terms(const recnn_discrete_value_args* a, const DvWorkspace
   return RECNN_OK;
 }
 
-// misc.py:29-44 from the action terms Y and add on, in the reference's order: target critic -> TD target (clamped),
-// online critic, MSE, backward, optimizer.  lo: the global id of the arena's first action column (0 unsharded).
-static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, const float* Y, const float* add, int lo,
-                   cudaStream_t st) {
+// misc.py:29-39 from the action terms Y and add on, in the reference's order: target critic -> TD target (clamped),
+// online critic (dropout masks m0 / m1, or Philox by local row when they are null), MSE as a partial sum over
+// 1 / n_rows_global, and -- with learn -- the backward of layers 3, 2 and the state block of layer 1 into value.grads,
+// leaving dz1 [n_rows, H] in w.dz1 for the action block.
+static int dv_grads(const recnn_discrete_value_args* a, const DvWorkspace& w, const float* Y, const float* add,
+                    int64_t n_global, const uint8_t* m0, const uint8_t* m1, cudaStream_t st) {
   const recnn_dims& d = a->dims;
-  const int S = d.state_dim, I = d.action_dim, H = d.hidden;
+  const int S = d.state_dim, H = d.hidden;
   const int64_t n = a->n_rows;
   const NetLayout lc = critic_layout(d);
   const int ldS = pad4(S);
   const bool train = a->dropout != 0;
   const float gate = train ? 2.0f : 1.0f;
   Rng rng = {nullptr, a->seed, (const long long*)a->rng_step};
-  const long long* act = reinterpret_cast<const long long*>(a->action);
-  unsigned* oob = w.tickets + kTicketOob;
   const Seg ss = {w.S, S, ldS, 0}, ss2 = {w.S2, S, ldS, 0};
   const float* Pt = a->target_value.params;
   const float* P = a->value.params;
@@ -429,10 +429,10 @@ static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, con
   RECNN_PROPAGATE(hidden_layer(st1, kNoSeg, Pt + lc.w2, lc.ld2, Pt + lc.b2, H, n, false, nullptr, rng, 1, w.t2, st));
   // online critic on (state, one-hot(action)) (misc.py:37)
   const Seg sc1 = {w.c1, H, H, 0};
-  RECNN_PROPAGATE(hidden_layer(ss, kNoSeg, P + lc.w1, lc.ld1, P + lc.b1, H, n, train, train ? a->masks[0] : nullptr, rng,
-                               0, w.c1, st, add));
-  RECNN_PROPAGATE(hidden_layer(sc1, kNoSeg, P + lc.w2, lc.ld2, P + lc.b2, H, n, train, train ? a->masks[1] : nullptr, rng,
-                               1, w.c2, st));
+  RECNN_PROPAGATE(hidden_layer(ss, kNoSeg, P + lc.w1, lc.ld1, P + lc.b1, H, n, train, train ? m0 : nullptr, rng, 0, w.c1,
+                               st, add));
+  RECNN_PROPAGATE(hidden_layer(sc1, kNoSeg, P + lc.w2, lc.ld2, P + lc.b2, H, n, train, train ? m1 : nullptr, rng, 1, w.c2,
+                               st));
   // TD target and clamp (misc.py:30-35), MSE (:39), its gradient through the head
   float* G = a->value.grads;
   if (value_head_fusable(H)) {
@@ -442,7 +442,7 @@ static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, con
     v.th2 = w.t2; v.tw3 = Pt + lc.w3; v.tb3 = Pt + lc.b3;
     v.reward = a->reward; v.done = a->done;
     v.gamma = a->gamma; v.min_value = a->min_value; v.max_value = a->max_value;
-    v.y = w.y; v.n_rows = n; v.n_rows_global = n; v.hidden = H;
+    v.y = w.y; v.n_rows = n; v.n_rows_global = n_global; v.hidden = H;
     v.learn = a->learn ? 1 : 0; v.gate_scale = gate; v.dz2 = w.dz2;
     v.gw3 = a->learn ? G + lc.w3 : nullptr; v.gb3 = a->learn ? G + lc.b3 : nullptr;
     v.loss = a->losses;
@@ -453,7 +453,7 @@ static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, con
     HeadArgs h;
     memset(&h, 0, sizeof(h));
     h.w3 = Pt + lc.w3; h.b3 = Pt + lc.b3; h.h2 = w.t2;
-    h.n_rows = n; h.n_rows_global = n; h.hidden = H; h.mode = HEAD_TARGET_DDPG;
+    h.n_rows = n; h.n_rows_global = n_global; h.hidden = H; h.mode = HEAD_TARGET_DDPG;
     h.reward = a->reward; h.done = a->done; h.gamma = a->gamma; h.min_value = a->min_value; h.max_value = a->max_value;
     h.y = w.y; h.tmp = w.qtmp; h.dq = w.dq; h.block_partials = w.block_partials; h.ticket = w.tickets;
     RECNN_PROPAGATE(launch_critic_head(h, st));
@@ -467,31 +467,59 @@ static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, con
     }
   }
   if (a->learn) {
-    // layers 2 and 1 (state block) through the dense weight gradients, each reduced here; then the action block
+    // layers 2 and 1 (state block) through the dense weight gradients, each reduced here
     RECNN_PROPAGATE(weight_grad(w.dz2, H, sc1, kNoSeg, n, G + lc.w2, lc.ld2, G + lc.b2, w.partial, st));
     RECNN_PROPAGATE(backprop_hidden(w.dz2, H, P + lc.w2, lc.ld2, H, 0, H, n, w.c1, gate, w.dz1, st));
     RECNN_PROPAGATE(weight_grad(w.dz1, H, ss, kNoSeg, n, G + lc.w1, lc.ld1, G + lc.b1, w.partial, st));
-    RECNN_CHECK_CUDA(cudaMemset2DAsync(G + lc.w1 + S, (size_t)lc.ld1 * 4, 0, (size_t)I * 4, H, st));
-    const int64_t n2 = pow2_at_least(n);
-    action_keys_kernel<<<elem_grid(n2), 256, 0, st>>>(act, n, n2, lo, I, w.keys);
-    RECNN_CHECK_LAUNCH("action_keys_kernel");
-    for (int64_t k = 2; k <= n2; k <<= 1)
-      for (int64_t j = k >> 1; j > 0; j >>= 1) {
-        bitonic_step_kernel<<<elem_grid(n2), 256, 0, st>>>(w.keys, n2, j, k);
-        RECNN_CHECK_LAUNCH("bitonic_step_kernel");
-      }
-    const unsigned blocks = (unsigned)(n < (int64_t)kNumSMs * 16 ? n : (int64_t)kNumSMs * 16);
-    scatter_action_grad_kernel<<<blocks, H < 256 ? 128 : 256, 0, st>>>(w.keys, n, w.dz1, H, G + lc.w1 + S, lc.ld1);
-    RECNN_CHECK_LAUNCH("scatter_action_grad_kernel");
-    if (a->value_optim.kind != RECNN_OPT_EXTERNAL)
-      RECNN_PROPAGATE(launch_optimizer(a->value_optim, a->value, lc.count, nullptr, st, w.tickets + 3));
   }
-  // ++rng_step; losses[4] <- error bits (1: an action id outside [0, num_items): its row read a zero action column and
-  // its gradient column was skipped; 2: the gathered shard records disagree with the plan)
-  RECNN_PROPAGATE(launch_finish((long long*)a->rng_step, oob, w.tickets + kTicketDpMismatch, a->losses + 4, st));
+  return RECNN_OK;
+}
+
+// The action block of dW1 from dz1 [n, H] of the rows with ids act[n]: zeroed, then column j - lo <- the ascending-row
+// sum of the dz1 rows with id j, for the ids [lo, lo + action_dim) the arena holds (keys: pow2(n) words of scratch).
+static int dv_action_grad(const recnn_discrete_value_args* a, const long long* act, int64_t n, const float* dz1,
+                          unsigned long long* keys, int lo, cudaStream_t st) {
+  const recnn_dims& d = a->dims;
+  const int S = d.state_dim, I = d.action_dim, H = d.hidden;
+  const NetLayout lc = critic_layout(d);
+  float* G = a->value.grads;
+  RECNN_CHECK_CUDA(cudaMemset2DAsync(G + lc.w1 + S, (size_t)lc.ld1 * 4, 0, (size_t)I * 4, H, st));
+  const int64_t n2 = pow2_at_least(n);
+  action_keys_kernel<<<elem_grid(n2), 256, 0, st>>>(act, n, n2, lo, I, keys);
+  RECNN_CHECK_LAUNCH("action_keys_kernel");
+  for (int64_t k = 2; k <= n2; k <<= 1)
+    for (int64_t j = k >> 1; j > 0; j >>= 1) {
+      bitonic_step_kernel<<<elem_grid(n2), 256, 0, st>>>(keys, n2, j, k);
+      RECNN_CHECK_LAUNCH("bitonic_step_kernel");
+    }
+  const unsigned blocks = (unsigned)(n < (int64_t)kNumSMs * 16 ? n : (int64_t)kNumSMs * 16);
+  scatter_action_grad_kernel<<<blocks, H < 256 ? 128 : 256, 0, st>>>(keys, n, dz1, H, G + lc.w1 + S, lc.ld1);
+  RECNN_CHECK_LAUNCH("scatter_action_grad_kernel");
+  return RECNN_OK;
+}
+
+// The built-in optimizer (learn; skipped on the device while *skip is set, when given), ++rng_step and losses[4] <- the
+// error bits (1: an action id outside [0, num_items): its row read a zero action column and its gradient column was
+// skipped; 2: the gathered shard or row records disagree with the plan), then the host copy of the losses.
+static int dv_finish(const recnn_discrete_value_args* a, const DvWorkspace& w, const unsigned* skip, cudaStream_t st) {
+  if (a->learn && a->value_optim.kind != RECNN_OPT_EXTERNAL)
+    RECNN_PROPAGATE(launch_optimizer(a->value_optim, a->value, critic_layout(a->dims).count, nullptr, st,
+                                     w.tickets + 3, nullptr, skip));
+  RECNN_PROPAGATE(launch_finish((long long*)a->rng_step, w.tickets + kTicketOob, w.tickets + kTicketDpMismatch,
+                                a->losses + 4, st));
   if (a->losses_host)
     RECNN_CHECK_CUDA(cudaMemcpyAsync(a->losses_host, a->losses, 8 * sizeof(float), cudaMemcpyDeviceToHost, st));
   return RECNN_OK;
+}
+
+// misc.py:29-55 from the action terms on, over this call's rows.  lo: the global id of the arena's first action column
+// (0 unsharded).
+static int dv_tail(const recnn_discrete_value_args* a, const DvWorkspace& w, const float* Y, const float* add, int lo,
+                   cudaStream_t st) {
+  RECNN_PROPAGATE(dv_grads(a, w, Y, add, a->n_rows, a->masks[0], a->masks[1], st));
+  if (a->learn)
+    RECNN_PROPAGATE(dv_action_grad(a, reinterpret_cast<const long long*>(a->action), a->n_rows, w.dz1, w.keys, lo, st));
+  return dv_finish(a, w, nullptr, st);
 }
 
 // misc.py:10-55: the action terms, then the rest.  Everything on `stream`, no allocation, no synchronisation.
@@ -548,4 +576,224 @@ extern "C" int recnn_discrete_value_shard_end(const recnn_discrete_value_args* a
   RECNN_PROPAGATE(dv_shard_check(a, v, &w, &p));
   RECNN_REQUIRE(terms != nullptr, "terms");
   return dv_tail(a, w, terms, terms + a->n_rows * a->dims.hidden, p.lo, static_cast<cudaStream_t>(stream));
+}
+
+// ---- the row-sharded (data-parallel) critic: two phases around an all-reduce and an all-gather (see the header) -----
+namespace recnn {
+
+// Dropout keep-masks of rows [row_offset, row_offset + n) of the online critic's two hidden layers: the bits the
+// EPI_HIDDEN epilogue draws from Philox(seed, *step, layer) at idx = row * H + h, keyed by the GLOBAL row.  At offset 0
+// the masks equal the epilogue's own draws.
+__global__ void dp_masks_kernel(unsigned long long seed, const long long* __restrict__ step, long long row_offset,
+                                long long n, int H, uint8_t* __restrict__ m0, uint8_t* __restrict__ m1) {
+  const long long total = n * H;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long g = (unsigned long long)(row_offset * H + i);
+    m0[i] = (uint8_t)((philox_keep_bits32(seed, (unsigned long long)*step, 0, g >> 5) >> (g & 31)) & 1u);
+    m1[i] = (uint8_t)((philox_keep_bits32(seed, (unsigned long long)*step, 1, g >> 5) >> (g & 31)) & 1u);
+  }
+}
+
+// The tail of message 1 (loss partial, out-of-range flag as 0 / 1) and the record's header {row_offset, n_rows,
+// n_rows_global, 0} and ids as int32 bit patterns.
+__global__ void dp_begin_kernel(const float* __restrict__ loss, const unsigned* __restrict__ oob, float* __restrict__ tail,
+                                const long long* __restrict__ act, long long n, long long row_offset, long long n_global,
+                                float* __restrict__ record) {
+  int* hdr = reinterpret_cast<int*>(record);
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i0 == 0) {
+    tail[0] = *loss;
+    tail[1] = *oob ? 1.f : 0.f;
+    hdr[0] = (int)row_offset; hdr[1] = (int)n; hdr[2] = (int)n_global; hdr[3] = 0;
+  }
+  for (long long i = i0; i < n; i += (long long)gridDim.x * blockDim.x) hdr[4 + i] = (int)act[i];
+}
+
+// After the exchanges: error words from the reduced message (tail) and the gathered headers (bit 2 unless they tile
+// [0, n_global) in rank order, each within record_rows rows, all with this rank's n_global), the reduced loss into
+// losses[0] and the skip word of the optimizer.  One thread.
+__global__ void dp_check_kernel(const float* __restrict__ tail, const float* __restrict__ g, int world, long long stride,
+                                long long record_rows, long long n_global, unsigned* __restrict__ tickets,
+                                float* __restrict__ loss) {
+  long long expect = 0;
+  bool bad = false;
+  for (int q = 0; q < world; ++q) {
+    const int* h = reinterpret_cast<const int*>(g + (long long)q * stride);
+    if (h[0] != expect || h[1] <= 0 || h[1] > record_rows || h[2] != n_global) bad = true;
+    expect += h[1];
+  }
+  if (expect != n_global) bad = true;
+  const unsigned oob = tail[1] > 0.f ? 1u : 0u;
+  tickets[kTicketDpMismatch] = bad ? 1u : 0u;
+  tickets[kTicketOob] = oob;
+  tickets[5] = (bad || oob) ? 1u : 0u;
+  *loss = tail[0];
+}
+
+// The gathered records in row order: ids [n_global] (int64) and dz1 [n_global, H].  Skipped when the headers are bad.
+__global__ void dp_rows_kernel(const float* __restrict__ g, int world, long long stride, long long record_rows, int H,
+                               long long n_global, const unsigned* __restrict__ bad, long long* __restrict__ ids,
+                               float* __restrict__ dz1) {
+  if (*bad) return;
+  const int q = blockIdx.y;
+  const float* rec = g + (long long)q * stride;
+  const int* h = reinterpret_cast<const int*>(rec);
+  const long long off = h[0], n = h[1];
+  const float* rows = rec + 4 + (record_rows + 3) / 4 * 4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n * H; i += (long long)gridDim.x * blockDim.x) {
+    const long long m = i / H;
+    dz1[(off + m) * H + (i - m * H)] = rows[i];
+    if (i - m * H == 0) ids[off + m] = h[4 + m];
+  }
+}
+
+// The replicated part of the gradient arena <-> message 1: the state block of W1 [H, pad4(S)] (pads zero), b1, W2
+// [H, H], b2, W3 [H], b3; then the two tail words.
+struct DpGradBlock { int64_t arena, ld, rows, cols, msg_ld; };
+static int dp_grad_blocks(const recnn_dims& d, DpGradBlock* b) {
+  const NetLayout lc = critic_layout(d);
+  const int S = d.state_dim, H = d.hidden;
+  b[0] = {lc.w1, lc.ld1, H, S, pad4(S)};
+  b[1] = {lc.b1, H, 1, H, H};
+  b[2] = {lc.w2, lc.ld2, H, H, H};
+  b[3] = {lc.b2, H, 1, H, H};
+  b[4] = {lc.w3, lc.ld3, 1, H, H};
+  b[5] = {lc.b3, 1, 1, 1, 1};
+  return 6;
+}
+static int64_t dp_grad_floats(const recnn_dims& d) {
+  DpGradBlock b[6];
+  int64_t f = 0;
+  for (int i = 0, k = dp_grad_blocks(d, b); i < k; ++i) f += b[i].rows * b[i].msg_ld;
+  return f + 2;
+}
+static int dp_grad_copy(const recnn_dims& d, float* G, float* msg, bool pack, cudaStream_t st) {
+  DpGradBlock b[6];
+  int64_t off = 0;
+  for (int i = 0, k = dp_grad_blocks(d, b); i < k; ++i) {
+    float* arena = G + b[i].arena;
+    float* m = msg + off;
+    if (pack)
+      RECNN_CHECK_CUDA(cudaMemcpy2DAsync(m, (size_t)b[i].msg_ld * 4, arena, (size_t)b[i].ld * 4, (size_t)b[i].cols * 4,
+                                         b[i].rows, cudaMemcpyDeviceToDevice, st));
+    else
+      RECNN_CHECK_CUDA(cudaMemcpy2DAsync(arena, (size_t)b[i].ld * 4, m, (size_t)b[i].msg_ld * 4, (size_t)b[i].cols * 4,
+                                         b[i].rows, cudaMemcpyDeviceToDevice, st));
+    off += b[i].rows * b[i].msg_ld;
+  }
+  return RECNN_OK;
+}
+static int64_t dp_record_floats(int H, int64_t rows) { return 4 + round_up(rows, 4) + rows * H; }
+
+// Past dv_carve: the generated masks of the rank's rows and the row-ordered ids / dz1 / keys of all n_global rows.
+struct DpExtra {
+  uint8_t *m0, *m1;
+  long long* ids;
+  float* dz1;
+  unsigned long long* keys;
+  int64_t bytes;
+};
+static DpExtra dp_carve(const recnn_dims& d, const recnn_discrete_dims& pd, int64_t n, int64_t n_global, int chunk,
+                        void* base) {
+  const int64_t head = dv_carve(d, pd, n, chunk, nullptr).bytes;
+  DpExtra x;
+  Carve c(base ? static_cast<char*>(base) + head : nullptr);
+  x.m0 = c.take<uint8_t>(n * d.hidden);
+  x.m1 = c.take<uint8_t>(n * d.hidden);
+  x.ids = c.take<long long>(n_global);
+  x.dz1 = c.take(n_global * d.hidden);
+  x.keys = c.take<unsigned long long>(pow2_at_least(n_global));
+  x.bytes = head + c.bytes();
+  return x;
+}
+
+}  // namespace recnn
+
+extern "C" int64_t recnn_discrete_value_dp_grad_floats(const recnn_dims* d) {
+  if (!d || d->state_dim <= 0 || d->hidden <= 0) return 0;
+  return dp_grad_floats(*d);
+}
+
+extern "C" int64_t recnn_discrete_value_dp_record_floats(const recnn_dims* d, int64_t record_rows) {
+  if (!d || d->hidden <= 0 || record_rows <= 0) return 0;
+  return dp_record_floats(d->hidden, record_rows);
+}
+
+extern "C" int64_t recnn_discrete_value_dp_workspace_bytes(const recnn_dims* d, const recnn_discrete_dims* pd,
+                                                           int64_t n_rows, int64_t n_rows_global, int32_t chunk_items) {
+  if (!d || !pd || n_rows <= 0 || n_rows_global < n_rows || !dv_dims_ok(*d, *pd) || !chunk_ok(d->action_dim, chunk_items))
+    return 0;
+  return dp_carve(*d, *pd, n_rows, n_rows_global, chunk_items, nullptr).bytes;
+}
+
+static int dv_dp_check(const recnn_discrete_value_args* a, int64_t row_offset, int64_t n_global, int64_t record_rows,
+                       DvWorkspace* w, DpExtra* x) {
+  RECNN_PROPAGATE(dv_check(a, w));
+  RECNN_REQUIRE(row_offset >= 0 && n_global >= a->n_rows && row_offset + a->n_rows <= n_global,
+                "row_offset / n_rows_global: the rows [row_offset, row_offset + n_rows) must lie in [0, n_rows_global)");
+  RECNN_REQUIRE(n_global < (1ll << 31) / (a->dims.hidden + 1), "n_rows_global too large for int32 row ids");
+  RECNN_REQUIRE(record_rows >= a->n_rows, "record_rows < n_rows");
+  *x = dp_carve(a->dims, a->policy_dims, a->n_rows, n_global, a->chunk_items, a->workspace);
+  return check_workspace(x->bytes, a->workspace_bytes);
+}
+
+extern "C" int recnn_discrete_value_dp_begin(const recnn_discrete_value_args* a, int64_t row_offset,
+                                             int64_t n_rows_global, int64_t record_rows, float* grad_msg,
+                                             float* record, void* stream) {
+  DvWorkspace w;
+  DpExtra x;
+  RECNN_PROPAGATE(dv_dp_check(a, row_offset, n_rows_global, record_rows, &w, &x));
+  RECNN_REQUIRE(grad_msg && record, "grad_msg / record");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t n = a->n_rows;
+  const int H = a->dims.hidden;
+  RECNN_PROPAGATE(dv_action_terms(a, w, 0, a->dims.action_dim, true, st));
+  const uint8_t *m0 = a->masks[0], *m1 = a->masks[1];
+  if (a->dropout && !m0) {
+    dp_masks_kernel<<<elem_grid(n * H), 256, 0, st>>>(a->seed, (const long long*)a->rng_step, row_offset, n, H, x.m0,
+                                                      x.m1);
+    RECNN_CHECK_LAUNCH("dp_masks_kernel");
+    m0 = x.m0;
+    m1 = x.m1;
+  }
+  RECNN_PROPAGATE(dv_grads(a, w, w.Y, w.add, n_rows_global, m0, m1, st));
+  const int64_t gf = dp_grad_floats(a->dims);
+  if (a->learn) {
+    RECNN_CHECK_CUDA(cudaMemsetAsync(grad_msg, 0, (gf - 2) * sizeof(float), st));
+    RECNN_PROPAGATE(dp_grad_copy(a->dims, a->value.grads, grad_msg, true, st));
+    RECNN_CHECK_CUDA(cudaMemcpyAsync(record + 4 + round_up(record_rows, 4), w.dz1, n * H * sizeof(float),
+                                     cudaMemcpyDeviceToDevice, st));
+  } else {
+    RECNN_CHECK_CUDA(cudaMemsetAsync(grad_msg, 0, (gf - 2) * sizeof(float), st));
+  }
+  dp_begin_kernel<<<elem_grid(n), 256, 0, st>>>(a->losses, w.tickets + kTicketOob, grad_msg + gf - 2,
+                                                reinterpret_cast<const long long*>(a->action), n, row_offset,
+                                                n_rows_global, record);
+  RECNN_CHECK_LAUNCH("dp_begin_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_value_dp_end(const recnn_discrete_value_args* a, int64_t row_offset, int64_t n_rows_global,
+                                           int32_t world, int64_t record_rows, const float* grad_msg,
+                                           const float* gathered, void* stream) {
+  DvWorkspace w;
+  DpExtra x;
+  RECNN_PROPAGATE(dv_dp_check(a, row_offset, n_rows_global, record_rows, &w, &x));
+  RECNN_REQUIRE(grad_msg && gathered, "grad_msg / gathered");
+  RECNN_REQUIRE(world >= 1, "world");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int H = a->dims.hidden;
+  const int64_t gf = dp_grad_floats(a->dims), stride = dp_record_floats(H, record_rows);
+  dp_check_kernel<<<1, 1, 0, st>>>(grad_msg + gf - 2, gathered, world, stride, record_rows, n_rows_global, w.tickets,
+                                   a->losses);
+  RECNN_CHECK_LAUNCH("dp_check_kernel");
+  if (a->learn) {
+    RECNN_PROPAGATE(dp_grad_copy(a->dims, a->value.grads, const_cast<float*>(grad_msg), false, st));
+    const dim3 grid(elem_grid(record_rows * H), (unsigned)world);
+    dp_rows_kernel<<<grid, 256, 0, st>>>(gathered, world, stride, record_rows, H, n_rows_global,
+                                         w.tickets + kTicketDpMismatch, x.ids, x.dz1);
+    RECNN_CHECK_LAUNCH("dp_rows_kernel");
+    RECNN_PROPAGATE(dv_action_grad(a, x.ids, n_rows_global, x.dz1, x.keys, 0, st));
+  }
+  return dv_finish(a, w, w.tickets + 5, st);
 }

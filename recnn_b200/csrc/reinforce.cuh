@@ -152,7 +152,7 @@ __device__ int inverse_cdf_row(const float* row, int items, float target, CdfSha
 __global__ void __launch_bounds__(kRowThreads)
 categorical_sample_kernel(const float* __restrict__ probs, long long ld, long long n, int items,
                           const float* __restrict__ uniforms, unsigned long long seed, long long draw,
-                          long long* __restrict__ action, float* __restrict__ logp) {
+                          long long* __restrict__ action, float* __restrict__ logp, long long row_offset = 0) {
   __shared__ float red[32];
   __shared__ CdfShared sh;
   for (long long r = blockIdx.x; r < n; r += gridDim.x) {
@@ -160,7 +160,7 @@ categorical_sample_kernel(const float* __restrict__ probs, long long ld, long lo
     float t = 0.f;
     for (int j = threadIdx.x; j < items; j += blockDim.x) t += row[j];
     const float total = block_sum(t, red);
-    const float u = draw_uniform(uniforms, seed, draw, r);
+    const float u = uniforms ? uniforms[r] : draw_uniform(nullptr, seed, draw, row_offset + r);
     const int a = inverse_cdf_row(row, items, u * total, sh);
     if (threadIdx.x == 0) {
       action[r] = a;
@@ -880,6 +880,20 @@ extern "C" int recnn_categorical_sample(const float* probs, int64_t n_rows, int3
   if (n_rows <= 0) return RECNN_OK;
   categorical_sample_kernel<<<row_grid(n_rows), kRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       probs, ld, n_rows, num_items, uniforms, seed, draw, reinterpret_cast<long long*>(action_out), log_prob_out);
+  RECNN_CHECK_LAUNCH("categorical_sample_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_categorical_sample_at(const float* probs, int64_t n_rows, int32_t num_items, int64_t ld,
+                                           const float* uniforms, uint64_t seed, int64_t draw, int64_t row_offset,
+                                           int64_t* action_out, float* log_prob_out, void* stream) {
+  RECNN_REQUIRE(probs && action_out && log_prob_out, "null pointer");
+  RECNN_REQUIRE(num_items > 0 && ld >= num_items, "num_items / ld");
+  RECNN_REQUIRE(row_offset >= 0, "row_offset");
+  if (n_rows <= 0) return RECNN_OK;
+  categorical_sample_kernel<<<row_grid(n_rows), kRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      probs, ld, n_rows, num_items, uniforms, seed, draw, reinterpret_cast<long long*>(action_out), log_prob_out,
+      row_offset);
   RECNN_CHECK_LAUNCH("categorical_sample_kernel");
   return RECNN_OK;
 }

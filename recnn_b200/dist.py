@@ -88,12 +88,24 @@ def broadcast_nets(nets: dict, group=None, src: int = 0):
         dist.broadcast(param_arena(nets[name]), src=src, group=group)
 
 
-def enable_data_parallel(agent_or_nets, group=None, sync_weights=True):
+def enable_data_parallel(agent_or_nets, group=None, sync_weights=True, beta=None):
     """Turn on gradient all-reduce for an Algo (or a nets dict).  Must be called on every
-    rank after the nets are on their CUDA device."""
+    rank after the nets are on their CUDA device.
+
+    With a DiscreteActor policy (REINFORCE) the agent trains row-parallel instead (RowParallel below): the nets -- and
+    ``beta``, the Top-K behaviour policy -- are made identical to rank 0's, one peer communicator is built and
+    data_parallel_in_place attaches the plan.  Each rank then feeds its own rows of every batch
+    (``shard_rows(N, rank, world)``) with the same seed on every rank."""
     if not dist.is_initialized():
         raise RuntimeError("torch.distributed is not initialised")
     nets = agent_or_nets.nets if hasattr(agent_or_nets, "nets") else agent_or_nets
+    from .nn.arena import _is_beta, _is_discrete
+    policy = nets.get("policy_net") if isinstance(nets, dict) else None
+    if policy is not None and _is_discrete(policy) and not _is_beta(policy):
+        return _enable_row_parallel(agent_or_nets, group, sync_weights, beta)
+    if beta is not None:
+        raise TypeError("beta goes with a DiscreteActor policy (REINFORCE); this agent's policy is %s"
+                        % type(policy).__name__)
     world = dist.get_world_size(group)
     if sync_weights:
         broadcast_nets(nets, group)
@@ -156,16 +168,12 @@ def vocab_comm_floats(dims, world: int, rows: int) -> int:
     return max(layer1_floats(dims), world * int(_lib.lib().recnn_vocab_record_floats(rows)))
 
 
-class VocabParallel:
-    """What ``enable_vocab_parallel`` records on a policy: its block [lo, hi) of the ``num_items`` items, the process
-    group, rank, world size, and the peer communicator of the exchanges."""
+class _Exchanges:
+    """The exchanges of a plan over its communicator ``comm`` (a PeerComm, or a test's stand-in with the same two
+    calls): the process group, rank and world size, and the collective growth of the staging buffers."""
 
-    def __init__(self, lo, hi, num_items, group, rank, world, comm):
-        self.lo, self.hi, self.num_items = lo, hi, num_items
+    def __init__(self, group, rank, world, comm):
         self.group, self.rank, self.world, self.comm = group, rank, world, comm
-
-    def shard(self):
-        return _lib.VocabShard(self.lo, self.num_items, self.rank, self.world)
 
     def _fit(self, need, device):
         """Grow the communicator (collectively: every rank asks for the same size) to ``need`` floats."""
@@ -189,6 +197,110 @@ class VocabParallel:
         # a copied net (a target net) shares the online net's plan and communicator: there is one peer mapping per
         # process group, and every net of an agent exchanges over it in the same order on every rank
         return self
+
+
+class VocabParallel(_Exchanges):
+    """What ``enable_vocab_parallel`` records on a policy: its block [lo, hi) of the ``num_items`` items, the process
+    group, rank, world size, and the peer communicator of the exchanges."""
+
+    def __init__(self, lo, hi, num_items, group, rank, world, comm):
+        super().__init__(group, rank, world, comm)
+        self.lo, self.hi, self.num_items = lo, hi, num_items
+
+    def shard(self):
+        return _lib.VocabShard(self.lo, self.num_items, self.rank, self.world)
+
+
+class RowParallel(_Exchanges):
+    """What ``enable_data_parallel`` records on the nets of a REINFORCE agent: every rank holds full replicas of the
+    nets and of β and its own rows of each batch; the process group, rank, world size and the peer communicator of the
+    row exchanges.  The data-parallel counterpart of VocabParallel."""
+
+    def row_counts(self, n_local):
+        """Every rank's row count, in rank order (one all-gather; a collective).  Raises ValueError on every rank when
+        a rank has no rows."""
+        dev = torch.device("cuda", torch.cuda.current_device())
+        counts = self.all_gather(torch.tensor([int(n_local)], dtype=torch.int32, device=dev)).tolist()
+        if min(counts) <= 0:
+            raise ValueError("a data-parallel rank got no rows (rows per rank: %s): every rank needs at least one "
+                             "row of each batch" % counts)
+        return counts
+
+    def rows(self, n_local):
+        """(row_offset, n_rows_global) of this rank's ``n_local`` rows: the ranks' rows, in rank order, are the rows
+        of the whole batch (uneven shards included).  A collective."""
+        counts = self.row_counts(n_local)
+        return sum(counts[:self.rank]), sum(counts)
+
+
+def row_parallel_of(net):
+    """The RowParallel attached to ``net`` by enable_data_parallel, or None."""
+    return net.__dict__.get("_recnn_rows")
+
+
+def _row_parallel_refusal(nets, beta, optimizers):
+    """Why these nets (and β, and the agent's optimizers) cannot be made row-parallel, or None."""
+    for name, net in list(nets.items()) + ([("beta", beta)] if beta is not None else []):
+        label = name if name == "beta" else "nets[%r]" % name
+        if "_recnn_vp" in net.__dict__:
+            return RuntimeError("%s is vocabulary-parallel: data parallel and vocabulary parallel do not combine" % label)
+        if "_recnn_rows" in net.__dict__:
+            return RuntimeError("%s is already data-parallel" % label)
+    opts = [("optimizers[%r]" % k, o) for k, o in sorted((optimizers or {}).items()) if o is not None]
+    if beta is not None:
+        opts.append(("beta.optim", beta.optim))
+    for label, opt in opts:
+        err = _optimizer_state_error(label, opt)
+        if err:
+            return RuntimeError(err.replace("vocabulary parallelism", "data parallelism"))
+    return None
+
+
+def data_parallel_in_place(nets, plan, beta=None, optimizers=None):
+    """The local half of enable_data_parallel on a REINFORCE agent, with no exchange: attach the RowParallel ``plan``
+    to ``nets`` ({name: net}: the policy, target policy and both critics) and to ``beta``.  The nets stay full replicas
+    (their ``state_dict`` and checkpoints are the unsharded ones); they must hold identical weights on every rank.
+    ``optimizers`` ({key: optimizer}) must not hold state yet.  The counterpart of shard_in_place."""
+    err = _row_parallel_refusal(nets, beta, optimizers)
+    if err is not None:
+        raise err
+    for net in nets.values():
+        net.__dict__.pop("_recnn_engines", None)
+        net.__dict__.pop("_recnn_ids_steps", None)
+        net.__dict__["_recnn_rows"] = plan
+    if beta is not None:
+        beta.__dict__["_recnn_rows"] = plan
+
+
+def _enable_row_parallel(agent_or_nets, group, sync_weights, beta):
+    agent, nets = _vocab_nets(agent_or_nets, beta, "data parallel REINFORCE trains a DiscreteActor")
+    optimizers = getattr(agent, "optimizers", None)
+    err = _row_parallel_refusal(nets, beta, optimizers)
+    arena = param_arena(nets["policy_net"])
+    if err is None and not arena.is_cuda:
+        err = _lib.RecnnError("enable_data_parallel needs the nets on their CUDA device")
+    if err is None:
+        for name, net in list(nets.items()) + ([("beta", beta)] if beta is not None else []):
+            if param_arena(net).device != arena.device:
+                err = _lib.RecnnError("%s is on %s, the policy on %s" % (name, param_arena(net).device, arena.device))
+                break
+    # every rank learns every rank's refusal, so a refused call raises on all of them before any device work
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    everyone = [None] * world
+    dist.all_gather_object(everyone, None if err is None else (type(err).__name__, str(err)), group=group)
+    bad = [(q, e) for q, e in enumerate(everyone) if e is not None]
+    if err is not None:
+        raise err
+    if bad:
+        raise RuntimeError("rank %d refuses data parallel: %s: %s" % (bad[0][0], bad[0][1][0], bad[0][1][1]))
+    if sync_weights:
+        broadcast_nets(nets, group)
+        if beta is not None:
+            dist.broadcast(param_arena(beta), src=0, group=group)
+    sizes = [param_arena(m).numel() for m in nets.values()] + ([param_arena(beta).numel()] if beta is not None else [])
+    comm = PeerComm(group, arena.device, max(sizes))
+    data_parallel_in_place(nets, RowParallel(group, rank, world, comm), beta, optimizers)
+    return agent_or_nets
 
 
 def _item_axes(net):
@@ -363,6 +475,10 @@ def enable_vocab_parallel(policy_or_agent, group=None, beta=None):
     agent, nets = _vocab_nets(policy_or_agent, beta, "enable_vocab_parallel shards a DiscreteActor")
     lone = "value_net" not in nets
     policy = nets["policy_net"]
+    for name, net in list(nets.items()) + ([("beta", beta)] if beta is not None else []):
+        if "_recnn_rows" in net.__dict__:
+            raise RuntimeError("%s is data-parallel: data parallel and vocabulary parallel do not combine"
+                               % (name if name == "beta" else "nets[%r]" % name))
     for name, net in nets.items():
         if "_recnn_vp" in net.__dict__:
             raise RuntimeError("the policy is already vocabulary-parallel" if lone

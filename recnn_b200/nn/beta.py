@@ -10,7 +10,9 @@ built-in RAdam (torch_optimizer is not installable next to the notebook's code h
 
 ``recnn_b200.dist.enable_vocab_parallel(policy_or_agent, beta=beta_net)`` shards a Beta over the item vocabulary with
 the policy: each rank keeps rows [lo, hi) of ``net.0`` and ``forward`` returns the rank's column block [N, hi - lo] of
-the probabilities (recnn_beta_shard_* in include/recnn_b200.h).
+the probabilities (recnn_beta_shard_* in include/recnn_b200.h).  ``recnn_b200.dist.enable_data_parallel(agent,
+beta=beta_net)`` keeps a full replica on every rank instead: a call on the rank's rows steps on the cross-entropy mean
+over every rank's rows (the gradient all-reduced), so the replicas stay identical.
 """
 from __future__ import annotations
 
@@ -131,7 +133,10 @@ class Beta(nn.Module):
                 self._workspace = None
                 self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             a.workspace, a.workspace_bytes = self._workspace.data_ptr(), self._workspace.numel()
-            if vp is None:
+            rows = self.__dict__.get("_recnn_rows")
+            if rows is not None:
+                loss, error = self._row_parallel_grad(a, rows, n, dev, loss, error)
+            elif vp is None:
                 _lib.check(L.recnn_beta_step(a, _lib.stream_ptr(dev)))
             else:
                 gathered = self._sharded_step(a, vp, n, dev)
@@ -142,12 +147,26 @@ class Beta(nn.Module):
                                    "optimizer step was taken")
             if err != 0:
                 raise IndexError("action holds an item id outside [0, num_items): no optimizer step was taken")
+            if rows is not None and builtin:
+                _lib.check(L.recnn_optimizer_step(c_opt, net, param_arena(self).numel(), None, _lib.stream_ptr(dev)))
             if not builtin:
                 grad_arena(self)               # re-attach p.grad views if zero_grad(set_to_none) dropped them
                 opt.step()
         if vp is not None:
             self.__dict__["_recnn_block"] = (weakref.ref(probs), gathered)
         return probs
+
+    def _row_parallel_grad(self, a, rows, n, dev, loss, error):
+        """Data parallel: this rank's rows' share of the gradient of the cross-entropy mean over the global batch,
+        all-reduced with the loss partial and the error flag.  Returns (loss, error) -- the same bits on every rank;
+        the caller steps the optimizer on every rank or, on an error, on none."""
+        a.n_rows_global = rows.rows(n)[1]
+        a.optim = _lib.Optim(_lib.OPT_EXTERNAL, 0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0)
+        _lib.check(_lib.lib().recnn_beta_step(a, _lib.stream_ptr(dev)))
+        rows.all_reduce(grad_arena(self))
+        tail = torch.cat([loss.reshape(1), (error != 0).float()])
+        rows.all_reduce(tail)
+        return tail[0], (tail[1:] > 0).to(torch.int32)
 
     def _sharded_step(self, a, vp, n, dev):
         """begin -> all-gather -> rows -> all-gather -> end; returns the gathered records of the first exchange."""

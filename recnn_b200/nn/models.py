@@ -116,6 +116,9 @@ class DiscreteActor(nn.Module):
       ``uniform_source(n_rows) -> tensor[n_rows]`` when set: replayable draws for tests), not torch's global generator.
     * After ``recnn_b200.dist.enable_vocab_parallel`` each rank holds a block of linear2's rows, and ``forward`` /
       ``select_action`` return the rank's column block of the probabilities; draws and log-probs stay global.
+    * After ``recnn_b200.dist.enable_data_parallel`` each rank holds a full replica and its own rows: ``select_action``
+      / ``pi_beta_sample`` draw row r of the rank at the Philox counter of its global row; ``forward`` and ``topk``
+      stay local, with no exchange.
     """
 
     def __init__(self, input_dim, action_dim, hidden_size, init_w=0):
@@ -241,9 +244,17 @@ class DiscreteActor(nn.Module):
         del self._saved[:]
 
     # -- Categorical(probs).sample() / .log_prob() on the device ----------------------------------------------------
-    def _sample(self, probs, gathered=None):
+    def _row_offset(self, n):
+        """On a data-parallel policy (recnn_b200.dist.enable_data_parallel) the global row of this call's first row,
+        from the ranks' row counts (a collective); else None."""
+        plan = self.__dict__.get("_recnn_rows")
+        return None if plan is None else plan.rows(n)[0]
+
+    def _sample(self, probs, gathered=None, row_offset=None):
         """(action int64 [N], log_prob fp32 [N]) of one draw per row.  ``gathered``: the records of the sharded
-        forward that made ``probs`` (the rank's column block); the draw is then over the whole vocabulary."""
+        forward that made ``probs`` (the rank's column block); the draw is then over the whole vocabulary.
+        ``row_offset``: the global row of the first row (data parallel): row r draws the uniform of global row
+        row_offset + r, what the single-GPU call over the whole batch draws for it."""
         n, items = probs.shape
         dev = probs.device
         action = torch.empty(n, dtype=torch.int64, device=dev)
@@ -256,6 +267,11 @@ class DiscreteActor(nn.Module):
         self._draws += 1
         seed = int(torch.initial_seed()) & (2 ** 64 - 1)
         with torch.cuda.device(dev):
+            if gathered is None and row_offset is not None:
+                _lib.check(_lib.lib().recnn_categorical_sample_at(
+                    probs.data_ptr(), n, items, probs.stride(0), _lib.ptr(u), seed, self._draws, row_offset,
+                    action.data_ptr(), logp.data_ptr(), _lib.stream_ptr(dev)))
+                return action, logp
             if gathered is None:
                 _lib.check(_lib.lib().recnn_categorical_sample(
                     probs.data_ptr(), n, items, probs.stride(0), _lib.ptr(u), seed, self._draws, action.data_ptr(),
@@ -322,7 +338,7 @@ class DiscreteActor(nn.Module):
         # REINFORCE without correction: only pi is available, the action source is ignored (models.py:102-111)
         dev, (state,) = _device_check(self, state)
         pi_probs, gathered = self._pi(state)
-        pi_action, pi_log_prob = self._sample(pi_probs, gathered)
+        pi_action, pi_log_prob = self._sample(pi_probs, gathered, self._row_offset(state.shape[0]))
         self.saved_log_probs.append(pi_log_prob)
         self._saved.append({"state": state.clone(), "action": pi_action, "beta_log_prob": None})
         return pi_probs
@@ -361,9 +377,10 @@ class DiscreteActor(nn.Module):
         beta_gathered = self._beta_records(beta_out) if torch.is_tensor(beta_out) else None
         beta_probs = self._as_probs(beta_out, dev)
         pi_probs, gathered = self._pi(state)
+        row_offset = self._row_offset(state.shape[0])
         # the pi draw is made first, then the beta draw (models.py:133-136)
-        pi_draw = self._sample(pi_probs, gathered)
-        beta_draw = self._sample(beta_probs, beta_gathered)
+        pi_draw = self._sample(pi_probs, gathered, row_offset)
+        beta_draw = self._sample(beta_probs, beta_gathered, row_offset)
         available = {"pi": (pi_draw, pi_probs), "beta": (beta_draw, beta_probs)}
         (pi_action, pi_lp), src_pi = available[self.action_source["pi"]]
         (beta_action, beta_lp), src_beta = available[self.action_source["beta"]]

@@ -67,6 +67,7 @@ class StepEngine:
         self.group = None            # torch.distributed process group for data parallel
         self.world = 1
         self.comm = None             # recnn_b200.dist.PeerComm: in-kernel all-reduce over NVLink peer memory
+        self.plan = None             # recnn_b200.dist.RowParallel of a data-parallel REINFORCE critic (value_only)
         self.seed = int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF
         # value(1), value2, policy, ||actor grad||_1, error bits (int32), 3 spare  (include/recnn_b200.h: losses)
         self.losses = torch.zeros(8, dtype=torch.float32, device=self.device)
@@ -402,6 +403,9 @@ class StepEngine:
             return self._step(batch, params, nets, optimizer, learn, step, debug, policy_every_key)
 
     def _allreduce(self, t):
+        if self.plan is not None:
+            self.plan.all_reduce(t)
+            return
         import torch.distributed as dist
         dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
 
@@ -527,6 +531,8 @@ class StepEngine:
 def _value_only(self, batch, params, nets, optimizer, learn, debug):
     """recnn/nn/update/misc.py:10-55 on its own: critic step without the policy half."""
     with torch.cuda.device(self.device):
+        if self.plan is not None:
+            batch = dict(batch, n_rows_global=self.plan.rows(int(batch["state"].shape[0]))[1])
         st = self._stage_batch(batch)
         if self.discrete:
             # next_action = target_policy_net(next_state)   (misc.py:28 with a DiscreteActor: probabilities)
@@ -545,6 +551,8 @@ def _value_only(self, batch, params, nets, optimizer, learn, debug):
             else:
                 grad_arena(vn)
                 val_opts[0].step()
+        if self.plan is not None and self.world > 1:
+            self._allreduce(self.losses[:1])       # the ranks' partial sums of the mean: the same loss on every rank
         self._launch(a, _lib.PH_FINISH, want_debug)
         torch.cuda.current_stream(self.device).synchronize()
         if want_debug is not None:
@@ -567,5 +575,8 @@ def get_engine(algo, nets, device) -> StepEngine:
         dp = policy.__dict__.get("_recnn_dp")
         if dp is not None:
             eng.group, eng.world, eng.comm = dp
+        rows = policy.__dict__.get("_recnn_rows")
+        if rows is not None:
+            eng.plan, eng.world = rows, rows.world
         cache[key] = eng
     return eng

@@ -89,10 +89,11 @@ def critic_action_term(value_net, probs=None, policy=None, state=None, chunk_ite
     return out
 
 
-def critic_value_of_probs(value_net, state, probs):
+def critic_value_of_probs(value_net, state, probs, masks=None):
     """value_net(state, probs) [N, 1] through the chunked action term instead of a re-pitched [N, num_items] image
-    (same dropout convention as Critic.forward: fresh masks in train mode).  On a vocabulary-parallel critic ``probs``
-    is the rank's column block: the ranks' action terms are all-reduced, and the value is the same on every rank."""
+    (same dropout convention as Critic.forward: fresh masks in train mode, or ``masks``).  On a vocabulary-parallel
+    critic ``probs`` is the rank's column block: the ranks' action terms are all-reduced, and the value is the same on
+    every rank."""
     from ..models import _train_masks
     dev = _stream_device(value_net)
     state = state.detach().to(device=dev, dtype=torch.float32).contiguous()
@@ -102,7 +103,7 @@ def critic_value_of_probs(value_net, state, probs):
     vp = value_net.__dict__.get("_recnn_vp")
     if vp is not None and n > 0:
         vp.all_reduce(term)
-    m1, m2 = _train_masks(value_net, n, d.hidden, dev)
+    m1, m2 = masks if masks is not None else _train_masks(value_net, n, d.hidden, dev)
     out = torch.empty(n, 1, device=dev, dtype=torch.float32)
     if n == 0:
         return out
@@ -118,6 +119,11 @@ def critic_value_of_probs(value_net, state, probs):
 class IdsValueStep:
     """Host side of recnn_discrete_value_step for one set of nets: staging, arenas, the optimizer and the single
     synchronisation that reads the loss and the error bits back."""
+
+    _plan_error = "the ranks disagree on the vocabulary shard plan or on the number of rows"
+    _oob_error = ("batch['action'] holds an item id outside [0, num_items) (the update was applied with the offending "
+                  "rows' action term set to zero)")
+    _checked_step = False        # True: a torch optimizer steps only after the error bits were read
 
     def __init__(self, nets, device):
         self.device = torch.device(device)
@@ -198,26 +204,32 @@ class IdsValueStep:
             a.losses = self.losses.data_ptr()
             a.losses_host = self.losses_host.data_ptr()
             L = _lib.lib()
-            nbytes = L.recnn_discrete_value_workspace_bytes(d, pd, n, a.chunk_items)
+            nbytes = self._workspace_bytes(L, a)
             if self.workspace is None or self.workspace.numel() < nbytes:
                 self.workspace = None
                 self.workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             a.workspace = self.workspace.data_ptr()
             a.workspace_bytes = self.workspace.numel()
             self._launch(L, a, dev)
-            if learn and a.value_optim.kind == _lib.OPT_EXTERNAL and vo is not None:
+            external = learn and a.value_optim.kind == _lib.OPT_EXTERNAL and vo is not None
+            if external and not self._checked_step:
                 grad_arena(value)          # re-attach p.grad views if zero_grad(set_to_none) dropped them
                 vo.step()
             torch.cuda.current_stream(dev).synchronize()
             bits = int(self.losses_host.view(torch.int32)[4])
             if bits & 2:
-                raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+                raise RuntimeError(self._plan_error)
             if bits & 1:
-                raise IndexError("batch['action'] holds an item id outside [0, num_items) (the update was applied with "
-                                 "the offending rows' action term set to zero)")
+                raise IndexError(self._oob_error)
+            if external and self._checked_step:
+                grad_arena(value)
+                vo.step()
             if not learn:
                 debug["next_action"] = nets["target_policy_net"](next_state)       # the reference's debug contract
             return float(self.losses_host[0])
+
+    def _workspace_bytes(self, L, a):
+        return L.recnn_discrete_value_workspace_bytes(a.dims, a.policy_dims, a.n_rows, a.chunk_items)
 
     def _launch(self, L, a, dev):
         _lib.check(L.recnn_discrete_value_step(a, _lib.stream_ptr(dev)))
@@ -246,6 +258,39 @@ class ShardedIdsValueStep(IdsValueStep):
         _lib.check(L.recnn_discrete_value_shard_end(a, shard, terms.data_ptr(), st))
 
 
+class RowParallelIdsValueStep(IdsValueStep):
+    """IdsValueStep of a data-parallel agent (recnn_b200.dist.enable_data_parallel): full replicas, this rank's rows of
+    the batch.  The step is recnn_discrete_value_dp_begin / _end with an all-reduce of the replicated gradient and an
+    all-gather of the ranks' (ids, dz1) rows between them, so every rank takes the same optimizer step; on an error
+    bit no rank takes one."""
+
+    _plan_error = ("the ranks' row records do not tile the batch in rank order or disagree on its row count: no "
+                   "optimizer step was taken")
+    _oob_error = "batch['action'] holds an item id outside [0, num_items) on some rank: no optimizer step was taken"
+    _checked_step = True
+
+    def __init__(self, nets, device):
+        super().__init__(nets, device)
+        self.plan = nets["value_net"].__dict__["_recnn_rows"]
+
+    def _workspace_bytes(self, L, a):
+        counts = self.plan.row_counts(a.n_rows)
+        # (row_offset, n_rows_global, record rows: the same on every rank)
+        self.rows = (sum(counts[:self.plan.rank]), sum(counts), max(counts))
+        return L.recnn_discrete_value_dp_workspace_bytes(a.dims, a.policy_dims, a.n_rows, self.rows[1], a.chunk_items)
+
+    def _launch(self, L, a, dev):
+        off, n_global, cap = self.rows
+        st = _lib.stream_ptr(dev)
+        grad = torch.empty(L.recnn_discrete_value_dp_grad_floats(a.dims), device=dev, dtype=torch.float32)
+        record = torch.empty(L.recnn_discrete_value_dp_record_floats(a.dims, cap), device=dev, dtype=torch.float32)
+        _lib.check(L.recnn_discrete_value_dp_begin(a, off, n_global, cap, grad.data_ptr(), record.data_ptr(), st))
+        self.plan.all_reduce(grad)
+        gathered = self.plan.all_gather(record)
+        _lib.check(L.recnn_discrete_value_dp_end(a, off, n_global, self.plan.world, cap, grad.data_ptr(),
+                                                 gathered.data_ptr(), st))
+
+
 def vocab_parallel_of(nets, names=("value_net", "target_value_net", "target_policy_net")):
     """The VocabParallel the named nets share, or None when none is sharded; RuntimeError when only some are, or they
     were sharded apart."""
@@ -260,9 +305,12 @@ def vocab_parallel_of(nets, names=("value_net", "target_value_net", "target_poli
 
 def get_ids_step(nets, device) -> IdsValueStep:
     """Cached on the value net, like the step engines on the policy net."""
-    if nets["policy_net"].__dict__.get("_recnn_dp") is not None and nets["policy_net"].__dict__["_recnn_dp"][1] > 1:
-        raise ValueError("item-id actions run on one GPU: data parallel is not supported in this mode")
-    cls = IdsValueStep if vocab_parallel_of(nets) is None else ShardedIdsValueStep
+    if vocab_parallel_of(nets) is not None:
+        cls = ShardedIdsValueStep
+    elif "_recnn_rows" in nets["value_net"].__dict__:
+        cls = RowParallelIdsValueStep
+    else:
+        cls = IdsValueStep
     value = nets["value_net"]
     cache = value.__dict__.setdefault("_recnn_ids_steps", {})
     dev = torch.device(device)

@@ -69,11 +69,21 @@ def _policy_loss(policy, returns, method):
         raise ValueError("select_action was called with different K since the last policy update: %s" % sorted(ks))
     K = ks.pop() if ks else 1
     vp = policy.__dict__.get("_recnn_vp")
+    rows = policy.__dict__.get("_recnn_rows")
     with torch.cuda.device(dev):
         if vp is None:
             _lib.check(L.recnn_reinforce_policy_grad_chunked(
                 d, flat.data_ptr(), grads.data_ptr(), state.data_ptr(), action.data_ptr(), _lib.ptr(beta_lp),
                 ret_rows.data_ptr(), n, method, K, chunk, out.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
+            if rows is not None:
+                # data parallel: the loss is a sum over rows, so the ranks' gradients and losses add up to the whole
+                # batch's; the out-of-range flag travels with the loss
+                rows.all_reduce(grads)
+                tail = torch.cat([out[:1], (out.view(torch.int32)[1:2] != 0).float()])
+                rows.all_reduce(tail)
+                if float(tail[1]) > 0:
+                    raise IndexError("saved action index out of range for the policy's output layer (on some rank)")
+                return tail[0].clone()
         else:
             # vocabulary-parallel: row statistics of the local items, all-gather, local dW2 / db2 and this rank's
             # share of the layer-1 gradient, all-reduce of the layer-1 block
@@ -148,6 +158,29 @@ class ChooseREINFORCE:
         return policy_loss
 
 
+def _row_masks(critic, plan, n, dev):
+    """The critic's two dropout keep-masks (train mode; else None) for this rank's ``n`` rows: rows [lo, lo + n) of
+    the masks the single-GPU call draws for the whole batch, so every row's mask follows its global row."""
+    if not critic.training:
+        return None
+    lo, n_global = plan.rows(n)
+    H = critic.linear1.out_features
+    keep = (torch.rand(2, n_global, H, device=dev) >= 0.5).to(torch.uint8)
+    return keep[0, lo:lo + n], keep[1, lo:lo + n]
+
+
+def _global_mean(plan, reward):
+    """The mean of the whole batch's rewards [N_global, 1] from this rank's rows [n, 1]: every rank gathers every
+    rank's rows (padded to the longest shard) and takes the mean of the same row-ordered vector, so all ranks hold the
+    same bits -- and the single-GPU value whenever the rows' rewards are."""
+    counts = plan.row_counts(reward.shape[0])
+    cap = max(counts)
+    buf = torch.zeros(cap, device=reward.device, dtype=torch.float32)
+    buf[:reward.shape[0]] = reward.reshape(-1)
+    everyone = plan.all_gather(buf).view(plan.world, cap)
+    return torch.cat([everyone[q, :c] for q, c in enumerate(counts)]).reshape(-1, 1).mean()
+
+
 def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"), debug=None,
                      writer=DummyWriter(), learn=True, step=-1):
     """Same signature, side effects and return value as the reference (reinforce.py:68-129): returns the losses dict
@@ -155,10 +188,20 @@ def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"),
 
     With nets sharded over the item vocabulary (recnn_b200.dist.enable_vocab_parallel on the agent) the batch action
     must be item ids: the reward line feeds the critic the policy's column block (action terms all-reduced) and the
-    critic step runs vocabulary-parallel.  Every rank must make the call with the same batch."""
+    critic step runs vocabulary-parallel.  Every rank must make the call with the same batch.
+
+    With a data-parallel agent (recnn_b200.dist.enable_data_parallel) every rank makes the call with its own rows of
+    the batch: draws, the reward line's dropout masks and the item-id critic's masks follow the global row, the reward
+    mean is the whole batch's, the critic and policy gradients are exchanged, and the returned losses are the same on
+    every rank."""
     # Due to its mechanics, reinforce doesn't support testing (reinforce.py:80-81)
     learn = True
     policy = nets["policy_net"]
+    plan = policy.__dict__.get("_recnn_rows")
+    if plan is not None and any(nets.get(k) is None or nets[k].__dict__.get("_recnn_rows") is not plan
+                                for k in ("value_net", "target_value_net", "target_policy_net")):
+        raise RuntimeError("a data-parallel policy trains with its critics and target policy data-parallel with it: "
+                           "recnn_b200.dist.enable_data_parallel on the agent")
     vp = policy.__dict__.get("_recnn_vp")
     if vp is not None:
         critics = [nets.get(k) for k in ("value_net", "target_value_net", "target_policy_net")]
@@ -185,11 +228,13 @@ def reinforce_update(batch, params, nets, optimizer, device=torch.device("cpu"),
         mx = predicted_probs.max(dim=1).values
         writer.add_histogram("predicted_probs_max_mean", mx.mean(), step)
         writer.add_histogram("predicted_probs_max_std", mx.std(), step)
+    rows = policy.__dict__.get("_recnn_rows")
+    masks = None if rows is None else _row_masks(nets["value_net"], rows, state.shape[0], dev)
     if ids:
-        reward = _ids.critic_value_of_probs(nets["value_net"], state, predicted_probs).detach()
+        reward = _ids.critic_value_of_probs(nets["value_net"], state, predicted_probs, masks=masks).detach()
     else:
-        reward = nets["value_net"](state, predicted_probs).detach()
-    policy.rewards.append(reward.mean())
+        reward = nets["value_net"](state, predicted_probs, masks=masks).detach()
+    policy.rewards.append(reward.mean() if rows is None else _global_mean(rows, reward))
 
     value_loss = value_update(batch, params, nets, optimizer, writer=writer, device=dev, debug=debug, learn=True, step=step)
 
