@@ -121,6 +121,15 @@ RECNN_API int recnn_window_gather_ids(const int64_t* hist_items, const float* hi
                             const int64_t* window_ids, int frame, int64_t n_rows,
                             int64_t* items, float* ratings, float* done, int64_t* users_out,
                             int* err_flag, void* stream);
+/* The serving state of each user: out fp32 [n, F*D + F] row u = the state after the last F interactions of user
+ * position users[u] (F embedding rows of the table, then the F ratings: batch_tensor_embeddings' column order), bit for
+ * bit the next_state of that user's last window.  A user with exactly F interactions has no window but has this state.
+ * *err_flag |= 1 for a position outside [0, n_users), 2 for a history shorter than F, 4 for a history item outside the
+ * table; such rows are zero-filled where they could not be read. */
+RECNN_API int recnn_user_states(const float* table, int64_t n_items, int32_t dim, const int64_t* hist_items,
+                                const float* hist_ratings, const int64_t* hist_offsets, int64_t n_users,
+                                const int64_t* users, int64_t n, int32_t frame, float* out, int32_t* err_flag,
+                                void* stream);
 
 /* ------------------------------------------------------------------ networks */
 
@@ -328,6 +337,23 @@ RECNN_API int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32
                                   int64_t n_items, const float* norms, int32_t metric, int32_t k,
                                   int64_t* ids_out, float* dist_out, void* workspace, int64_t workspace_bytes,
                                   void* stream);
+/* Item-set tables (the exclusion of the *_sets calls): set_ids int64 [n_set_ids], set_offsets int64 [n_sets + 1];
+ * set s is set_ids[set_offsets[s] : set_offsets[s + 1]], ascending (duplicates allowed).  row_set int64 [n_rows] maps
+ * each row of the call to the set it excludes, -1 for none, so rows can share a set (e.g. all rows of one user); NULL
+ * maps row r to set r and needs n_sets == n_rows.  Only the sets the rows reference are read and checked, on the
+ * device: *error_flag <- bits: 1 = a set id outside [0, num_items); 4 = a row_set outside [-1, n_sets), set offsets
+ * outside [0, n_set_ids] or decreasing, or a descending pair inside a set.  A malformed table is never read out of
+ * bounds; the results are then meaningless.  Sets of up to 4,096 ids are searched in shared memory, longer ones in
+ * global memory, and only for a candidate that would enter a row's list.
+ *
+ * recnn_retrieve_topk with exclusion: the ids of row q's set are never returned.  A row with fewer than k eligible
+ * items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  Every row_set -1: recnn_retrieve_topk's bits.
+ * Same workspace. */
+RECNN_API int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                       int64_t n_items, const float* norms, int32_t metric, int32_t k,
+                                       const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                       int64_t n_sets, const int64_t* row_set, int64_t* ids_out, float* dist_out,
+                                       int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- REINFORCE with (Top-K) off-policy correction: the policy side (SURVEY 8f-2) ------------------
  * DiscreteActor (recnn/nn/models.py:76-99): probs = softmax(W2 relu(W1 s + b1) + b2), one output per item.
@@ -482,6 +508,21 @@ RECNN_API int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, con
                                                const float* gathered, int64_t n_rows, int32_t k,
                                                const int64_t* exclude, int32_t n_exclude, float* values_out,
                                                int64_t* ids_out, int32_t* error_flag, void* stream);
+/* recnn_discrete_topk and recnn_discrete_shard_topk with an item-set table (see recnn_retrieve_topk_sets) in place of
+ * the dense list: set ids are global, so every rank passes the same table and excludes within its own block; the pair
+ * shard_topk_sets + shard_topk_finish (n_exclude 0) equals recnn_discrete_topk_sets at world 1.  *error_flag <- bits
+ * 1 and 4 as above, the same on every rank.  Same workspace: it does not grow with the table. */
+RECNN_API int recnn_discrete_topk_sets(const recnn_discrete_dims* d, const float* params, const float* state,
+                                       int64_t n_rows, int32_t k, const int64_t* set_ids, int64_t n_set_ids,
+                                       const int64_t* set_offsets, int64_t n_sets, const int64_t* row_set,
+                                       int32_t chunk_items, float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                       void* workspace, int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_topk_sets(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                             const float* params, const float* state, int64_t n_rows, int32_t k,
+                                             const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                             int64_t n_sets, const int64_t* row_set, int32_t chunk_items,
+                                             float* record, int32_t* error_flag, void* workspace,
+                                             int64_t workspace_bytes, void* stream);
 
 /* ---- REINFORCE: the critic side with item-id actions ---------------------------------------------
  * The REINFORCE critic is a Critic(S, num_items, H) (recnn/nn/update/reinforce.py:92-102): layer 1 is W1 [H, S + num_items]

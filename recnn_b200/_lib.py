@@ -119,6 +119,8 @@ SIGNATURES = {
     "recnn_window_gather_ids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                           C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p]),
+    "recnn_user_states": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                     C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_actor_param_count": (C.c_int64, [C.POINTER(Dims)]),
     "recnn_critic_param_count": (C.c_int64, [C.POINTER(Dims)]),
     "recnn_net_layout": (C.c_int, [C.POINTER(Dims), C.c_int, C.POINTER(C.c_int64)]),
@@ -142,6 +144,10 @@ SIGNATURES = {
     "recnn_retrieve_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64, C.c_int32]),
     "recnn_retrieve_topk": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_retrieve_topk_sets": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
+                                           C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                           C.c_void_p]),
     "recnn_discrete_layout": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(C.c_int64)]),
     "recnn_discrete_scratch_floats": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32]),
     "recnn_discrete_forward": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
@@ -186,6 +192,13 @@ SIGNATURES = {
     "recnn_discrete_shard_topk_finish": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
                                                    C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_discrete_topk_sets": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_discrete_shard_topk_sets": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                 C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
+                                                 C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_int64, C.c_void_p]),
     "recnn_critic_action_term_scratch_floats": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                             C.c_int32]),
     "recnn_critic_action_term_chunked": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.POINTER(DiscreteDims), C.c_void_p,

@@ -138,3 +138,63 @@ extern "C" int recnn_window_gather_ids(const int64_t* hist_items, const float* h
                                      n_rows, frame, n_rows, items, ratings, done, users, err_flag,
                                      static_cast<cudaStream_t>(stream));
 }
+
+// ---- Serving state: the state after each user's whole history ------------------------------------------------------
+// Row u of out [n, F*D + F] is the next_state of user users[u]'s last window, in batch_tensor_embeddings' column order
+// (F embedding rows, then F ratings) -- the history's last F items and ratings.  A user with exactly F interactions has
+// no window but has this state.  One warp per (row, slot): pure copies, bit-exact.  *err |= 1 for a user position
+// outside [0, n_users), 2 for a history shorter than F, 4 for an item outside the table (the row is then zero-filled
+// where it could not be read).
+namespace recnn {
+__global__ void __launch_bounds__(256)
+user_state_kernel(const float* __restrict__ table, long long n_items, int dim, const long long* __restrict__ hist_items,
+                  const float* __restrict__ hist_ratings, const long long* __restrict__ hist_offsets,
+                  long long n_users, const long long* __restrict__ users, long long n, int frame,
+                  float* __restrict__ out, int* __restrict__ err) {
+  const long long warp = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  const long long units = n * (frame + 1);               // F embedding rows and one ratings tail per row
+  if (warp >= units) return;
+  const long long r = warp / (frame + 1);
+  const int j = (int)(warp - r * (frame + 1));
+  const long long ld = (long long)frame * dim + frame;
+  float* row = out + r * ld;
+  const long long u = users[r];
+  int bad = 0;
+  long long src = 0;
+  if (u < 0 || u >= n_users) bad = 1;
+  else {
+    const long long end = hist_offsets[u + 1];
+    if (end - hist_offsets[u] < frame) bad = 2;
+    src = end - frame;
+  }
+  if (j == frame) {                                      // the ratings tail
+    for (int t = lane; t < frame; t += 32) row[(long long)frame * dim + t] = bad ? 0.f : hist_ratings[src + t];
+    if (bad && lane == 0) atomicOr(err, bad);
+    return;
+  }
+  long long id = bad ? -1 : hist_items[src + j];
+  if (!bad && (id < 0 || id >= n_items)) {
+    if (lane == 0) atomicOr(err, 4);
+    id = -1;
+  }
+  float* dst = row + (long long)j * dim;
+  for (int c = lane; c < dim; c += 32) dst[c] = id < 0 ? 0.f : __ldg(table + id * dim + c);
+}
+}  // namespace recnn
+
+extern "C" int recnn_user_states(const float* table, int64_t n_items, int32_t dim, const int64_t* hist_items,
+                                 const float* hist_ratings, const int64_t* hist_offsets, int64_t n_users,
+                                 const int64_t* users, int64_t n, int32_t frame, float* out, int32_t* err_flag,
+                                 void* stream) {
+  RECNN_REQUIRE(table && hist_items && hist_ratings && hist_offsets && out && err_flag && (users || n == 0),
+                "null pointer");
+  RECNN_REQUIRE(n_items > 0 && dim > 0 && n_users > 0 && n >= 0 && frame > 0, "sizes");
+  if (n == 0) return RECNN_OK;
+  const int64_t blocks = recnn::ceil_div(n * (frame + 1), 8);
+  recnn::user_state_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      table, n_items, dim, (const long long*)hist_items, hist_ratings, (const long long*)hist_offsets, n_users,
+      (const long long*)users, n, frame, out, err_flag);
+  RECNN_CHECK_LAUNCH("user_state_kernel");
+  return RECNN_OK;
+}

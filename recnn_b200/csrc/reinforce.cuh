@@ -611,7 +611,7 @@ static int reinforce_grad_pass(const recnn_discrete_dims& d, const float* params
 // logits fold into (run_max, run_sum) through logit_stats_kernel, and its best k candidates merge into a running list
 // of k (key = -logit, global id) per row, sorted best first (ties: smaller id).  Finish: pi = exp(z - M) / S, the
 // expression of softmax_rows_kernel.
-constexpr int kMaxExclude = 256;
+constexpr int kMaxExclude = 256;     // E of the dense [n, E] form
 constexpr int kTopkSplitCap = 31;     // the running list takes lane 0 of the merge warp
 
 // -logit, with NaN and -inf logits ranked after every finite one (and still before an empty slot, by id)
@@ -624,24 +624,24 @@ __global__ void cand_fill_kernel(Cand* __restrict__ c, long long count) {
 
 // grid (splits, rows): the best k of columns [lo, hi) of one row of a chunk's logits z [n, w] (ids id0 + j) that beat
 // the row's running k-th best, ascending, into part [n, splits, k] (empty slots: {FLT_MAX, kNoId}).  A candidate is
-// checked against the row's excluded ids only once it beats its thread's list and the running k-th.
-template <int KMAX>
+// tested against the row's excluded set (global ids, topk.cuh) only once it beats its thread's list and the running k-th
+// (SETS; without, nothing is staged).
+template <int KMAX, bool SETS>
 __global__ void __launch_bounds__(kTopkThreads)
-policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int id0, int k,
-                          const long long* __restrict__ exclude, int n_ex, const Cand* __restrict__ run,
-                          Cand* __restrict__ part) {
+policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int id0, int k, ItemSets ex, int stage_cap,
+                          const Cand* __restrict__ run, Cand* __restrict__ part) {
   __shared__ float s_key[32];
   __shared__ int s_id[32], s_owner[32];
-  __shared__ int s_ex[kMaxExclude];
+  extern __shared__ int s_set[];
   const int sp = blockIdx.x, splits = gridDim.x;
   const int per = (w + splits - 1) / splits;
   const int lo = sp * per, hi = min(w, lo + per);
   for (long long r = blockIdx.y; r < n; r += gridDim.y) {
-    for (int e = threadIdx.x; e < n_ex; e += blockDim.x) {
-      const long long x = exclude[r * n_ex + e];
-      s_ex[e] = (x >= 0 && x < kNoId) ? (int)x : -1;       // padding and out-of-range ids match no item
+    SetView set = {nullptr, 0, true};
+    if (SETS) {
+      set = set_stage(ex, r, s_set, stage_cap);
+      __syncthreads();
     }
-    __syncthreads();
     const Cand bar = run[r * k + k - 1];
     float keys[KMAX];
     int ids[KMAX];
@@ -650,11 +650,9 @@ policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int i
     for (int j = lo + threadIdx.x; j < hi; j += blockDim.x) {
       const float key = logit_key(row[j]);
       const int id = id0 + j;
-      if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && better(key, id, bar.key, bar.id)) {
-        bool ex = false;
-        for (int e = 0; e < n_ex; ++e) ex |= s_ex[e] == id;
-        if (!ex) list_insert(keys, ids, key, id);
-      }
+      if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && better(key, id, bar.key, bar.id) &&
+          (!SETS || set.n == 0 || !set_has(set, s_set, id)))
+        list_insert(keys, ids, key, id);
     }
     // merge the CTA's sorted lists: rounds of arg-min over the heads, until k or every list is empty
     Cand* out = part + (r * splits + sp) * k;
@@ -669,7 +667,7 @@ policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int i
       if (threadIdx.x == 0) out[i] = Cand{wk, wi};
     }
     for (int j = i + threadIdx.x; j < k; j += blockDim.x) out[j] = Cand{FLT_MAX, kNoId};
-    __syncthreads();                                        // s_ex is refilled for the next row
+    __syncthreads();                                        // s_set is refilled for the next row
   }
 }
 
@@ -775,6 +773,7 @@ struct TopkWorkspace {
   DiscreteScratch s;           // img, h and z ([n, chunk]) for discrete_hidden / discrete_logits
   float *run_max, *run_sum;
   Cand *list[2], *part;        // two running lists [n, k] (ping-pong), the chunk's partial lists [n, splits, k]
+  long long* sorted;           // the dense form's [n, E <= kMaxExclude] ids, each row ascending
   int64_t bytes;
 };
 static TopkWorkspace topk_carve(const recnn_discrete_dims& d, int64_t n, int k, int chunk, void* base) {
@@ -789,6 +788,7 @@ static TopkWorkspace topk_carve(const recnn_discrete_dims& d, int64_t n, int k, 
   w.list[0] = c.take<Cand>(n * k);
   w.list[1] = c.take<Cand>(n * k);
   w.part = c.take<Cand>(n * topk_splits(n, chunk, kTopkSplitCap) * k);     // the widest chunk has the most splits
+  w.sorted = c.take<long long>(n * kMaxExclude);
   w.bytes = c.bytes();
   return w;
 }
@@ -796,9 +796,13 @@ static TopkWorkspace topk_carve(const recnn_discrete_dims& d, int64_t n, int k, 
 // The hidden layer, then every chunk: logits, row statistics into (run_max, run_sum), selection and merge.  Candidate
 // ids are id0 + the local item.  Returns the final lists.
 static int policy_topk_pass(const recnn_discrete_dims& d, const float* params, const float* state, int64_t n, int k,
-                            const long long* exclude, int n_ex, int chunk, int id0, const TopkWorkspace& w,
-                            float* run_max, float* run_sum, const Cand** lists, cudaStream_t st) {
+                            const ItemSets& ex, int chunk, int id0, const TopkWorkspace& w, float* run_max,
+                            float* run_sum, const Cand** lists, cudaStream_t st) {
   const int I = d.num_items;
+  // the dense form stages its E ids, a table up to kSetStage
+  const int cap = !ex.ids ? 0 : (ex.offsets ? kSetStage : ex.stride), stage = cap * (int)sizeof(int);
+  auto select = k <= 16 ? (cap ? policy_topk_select_kernel<16, true> : policy_topk_select_kernel<16, false>)
+                        : (cap ? policy_topk_select_kernel<64, true> : policy_topk_select_kernel<64, false>);
   RECNN_PROPAGATE(discrete_hidden(d, params, state, n, w.s, st, nullptr));
   cand_fill_kernel<<<(unsigned)ceil_div(n * k, 256), 256, 0, st>>>(w.list[0], n * k);
   RECNN_CHECK_LAUNCH("cand_fill_kernel");
@@ -811,12 +815,7 @@ static int policy_topk_pass(const recnn_discrete_dims& d, const float* params, c
     RECNN_CHECK_LAUNCH("logit_stats_kernel");
     const int splits = topk_splits(n, cw, kTopkSplitCap);
     const dim3 grid((unsigned)splits, (unsigned)(n < 65535 ? n : 65535));
-    if (k <= 16)
-      policy_topk_select_kernel<16><<<grid, kTopkThreads, 0, st>>>(w.s.z, n, cw, id0 + c0, k, exclude, n_ex,
-                                                                   w.list[cur], w.part);
-    else
-      policy_topk_select_kernel<64><<<grid, kTopkThreads, 0, st>>>(w.s.z, n, cw, id0 + c0, k, exclude, n_ex,
-                                                                   w.list[cur], w.part);
+    select<<<grid, kTopkThreads, stage, st>>>(w.s.z, n, cw, id0 + c0, k, ex, cap, w.list[cur], w.part);
     RECNN_CHECK_LAUNCH("policy_topk_select_kernel");
     policy_topk_merge_kernel<<<(unsigned)ceil_div(n, 4), 128, 0, st>>>(w.list[cur], w.part, splits, k, n,
                                                                        w.list[cur ^ 1]);
@@ -831,6 +830,17 @@ static int exclude_check(const long long* exclude, int64_t n, int n_ex, int64_t 
   if (n_ex == 0) return RECNN_OK;
   exclude_check_kernel<<<(unsigned)ceil_div(n * n_ex, 256), 256, 0, st>>>(exclude, n * n_ex, items, flag);
   RECNN_CHECK_LAUNCH("exclude_check_kernel");
+  return RECNN_OK;
+}
+
+// The dense [n, n_ex] form as a table: each row sorted into the workspace, row r excluding segment r
+static int dense_sets(const long long* exclude, int64_t n, int n_ex, const TopkWorkspace& w, ItemSets* out,
+                      cudaStream_t st) {
+  *out = ItemSets{nullptr, nullptr, nullptr, 0, 0, 0};
+  if (n_ex == 0) return RECNN_OK;
+  exclude_sort_kernel<<<(unsigned)n, pow2_threads(n_ex), 0, st>>>(exclude, n_ex, w.sorted);
+  RECNN_CHECK_LAUNCH("exclude_sort_kernel");
+  *out = ItemSets{w.sorted, nullptr, nullptr, n * n_ex, n, n_ex};
   return RECNN_OK;
 }
 
@@ -1114,6 +1124,19 @@ static int topk_check(const recnn_discrete_dims* d, const float* params, const f
   return check_workspace(topk_carve(*d, n_rows, k, chunk_items, nullptr).bytes, workspace_bytes);
 }
 
+// the passes and the finish of an unsharded call
+static int topk_local(const recnn_discrete_dims& d, const float* params, const float* state, int64_t n_rows, int k,
+                      const ItemSets& sets, int chunk_items, float* values_out, int64_t* ids_out,
+                      const TopkWorkspace& w, cudaStream_t st) {
+  const Cand* lists;
+  RECNN_PROPAGATE(policy_topk_pass(d, params, state, n_rows, k, sets, chunk_items, 0, w, w.run_max, w.run_sum, &lists,
+                                   st));
+  policy_topk_finish_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(
+      lists, n_rows, k, w.run_max, w.run_sum, values_out, reinterpret_cast<long long*>(ids_out));
+  RECNN_CHECK_LAUNCH("policy_topk_finish_kernel");
+  return RECNN_OK;
+}
+
 extern "C" int recnn_discrete_topk(const recnn_discrete_dims* d, const float* params, const float* state,
                                    int64_t n_rows, int32_t k, const int64_t* exclude, int32_t n_exclude,
                                    int32_t chunk_items, float* values_out, int64_t* ids_out, int32_t* error_flag,
@@ -1126,17 +1149,42 @@ extern "C" int recnn_discrete_topk(const recnn_discrete_dims* d, const float* pa
   const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
   RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
   RECNN_PROPAGATE(exclude_check(ex, n_rows, n_exclude, d->num_items, error_flag, st));
-  const Cand* lists;
-  RECNN_PROPAGATE(policy_topk_pass(*d, params, state, n_rows, k, ex, n_exclude, chunk_items, 0, w, w.run_max,
-                                   w.run_sum, &lists, st));
-  policy_topk_finish_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(
-      lists, n_rows, k, w.run_max, w.run_sum, values_out, reinterpret_cast<long long*>(ids_out));
-  RECNN_CHECK_LAUNCH("policy_topk_finish_kernel");
-  return RECNN_OK;
+  ItemSets sets;
+  RECNN_PROPAGATE(dense_sets(ex, n_rows, n_exclude, w, &sets, st));
+  return topk_local(*d, params, state, n_rows, k, sets, chunk_items, values_out, ids_out, w, st);
+}
+
+extern "C" int recnn_discrete_topk_sets(const recnn_discrete_dims* d, const float* params, const float* state,
+                                        int64_t n_rows, int32_t k, const int64_t* set_ids, int64_t n_set_ids,
+                                        const int64_t* set_offsets, int64_t n_sets, const int64_t* row_set,
+                                        int32_t chunk_items, float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                        void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(values_out && ids_out, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, nullptr, 0, chunk_items, workspace, workspace_bytes));
+  RECNN_REQUIRE(k <= d->num_items, "k <= num_items");
+  ItemSets sets;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_rows, error_flag, &sets));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(item_sets_check(sets, n_rows, d->num_items, error_flag, st));
+  return topk_local(*d, params, state, n_rows, k, sets, chunk_items, values_out, ids_out, w, st);
 }
 
 extern "C" int64_t recnn_vocab_topk_record_floats(int64_t n_rows, int32_t k) {
   return n_rows > 0 && k >= 1 && k <= 64 ? topk_record_floats(n_rows, k) : 0;
+}
+
+// the passes over the rank's block and its record
+static int topk_shard_local(const recnn_discrete_dims& d, const ShardPlan& p, const float* params, const float* state,
+                            int64_t n_rows, int k, const ItemSets& sets, int chunk_items, float* record,
+                            const TopkWorkspace& w, cudaStream_t st) {
+  const Cand* lists;
+  RECNN_PROPAGATE(policy_topk_pass(d, params, state, n_rows, k, sets, chunk_items, p.lo, w,
+                                   shard_plane(record, n_rows, 0), shard_plane(record, n_rows, 1), &lists, st));
+  policy_topk_record_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(lists, n_rows, k, p, record);
+  RECNN_CHECK_LAUNCH("policy_topk_record_kernel");
+  return RECNN_OK;
 }
 
 extern "C" int recnn_discrete_shard_topk(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
@@ -1150,13 +1198,29 @@ extern "C" int recnn_discrete_shard_topk(const recnn_discrete_dims* d, const rec
   RECNN_REQUIRE(k <= p.items, "k <= num_items (the whole vocabulary)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
-  const Cand* lists;
-  RECNN_PROPAGATE(policy_topk_pass(*d, params, state, n_rows, k, reinterpret_cast<const long long*>(exclude),
-                                   n_exclude, chunk_items, p.lo, w, shard_plane(record, n_rows, 0),
-                                   shard_plane(record, n_rows, 1), &lists, st));
-  policy_topk_record_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(lists, n_rows, k, p, record);
-  RECNN_CHECK_LAUNCH("policy_topk_record_kernel");
-  return RECNN_OK;
+  ItemSets sets;
+  RECNN_PROPAGATE(dense_sets(reinterpret_cast<const long long*>(exclude), n_rows, n_exclude, w, &sets, st));
+  return topk_shard_local(*d, p, params, state, n_rows, k, sets, chunk_items, record, w, st);
+}
+
+extern "C" int recnn_discrete_shard_topk_sets(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                              const float* params, const float* state, int64_t n_rows, int32_t k,
+                                              const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                              int64_t n_sets, const int64_t* row_set, int32_t chunk_items,
+                                              float* record, int32_t* error_flag, void* workspace,
+                                              int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(record, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, nullptr, 0, chunk_items, workspace, workspace_bytes));
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(k <= p.items, "k <= num_items (the whole vocabulary)");
+  ItemSets sets;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_rows, error_flag, &sets));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(item_sets_check(sets, n_rows, p.items, error_flag, st));   // global ids: every rank agrees
+  return topk_shard_local(*d, p, params, state, n_rows, k, sets, chunk_items, record, w, st);
 }
 
 extern "C" int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,

@@ -37,17 +37,25 @@ item_norms_kernel(const float* __restrict__ table, long long n_items, int dim, i
   if (lane == 0) out[row] = metric == RECNN_METRIC_COS ? 1.0f / fmaxf(sqrtf(s), 1e-30f) : s;
 }
 
-// grid (splits, n_queries).  scores [n_queries, ld]; writes k candidates per (query, split), ascending.
-template <int KMAX>
+// grid (splits, n_queries).  scores [n_queries, ld]; writes k candidates per (query, split), ascending.  Query q is
+// row row0 + q of the call; with SETS its excluded set (ex) is tested only for a candidate that enters the thread's
+// list (without, the kernel is the plain search, nothing staged).
+template <int KMAX, bool SETS>
 __global__ void __launch_bounds__(kTopkThreads)
 topk_partial_kernel(const float* __restrict__ scores, long long ld, long long n_items, const float* __restrict__ norms,
-                    int metric, int k, Cand* __restrict__ part) {
+                    int metric, int k, ItemSets ex, long long row0, int stage_cap, Cand* __restrict__ part) {
   __shared__ float s_key[32];
   __shared__ int s_id[32], s_owner[32];
+  extern __shared__ int s_set[];
   const int q = blockIdx.y, sp = blockIdx.x, splits = gridDim.x;
   const long long per = (n_items + splits - 1) / splits;
   const long long lo = sp * per, hi = min(n_items, lo + per);
   const float* row = scores + (long long)q * ld;
+  SetView set = {nullptr, 0, true};
+  if (SETS) {
+    set = set_stage(ex, row0 + q, s_set, stage_cap);
+    __syncthreads();
+  }
   float keys[KMAX];
   int ids[KMAX];
   list_clear(keys, ids);
@@ -57,7 +65,8 @@ topk_partial_kernel(const float* __restrict__ scores, long long ld, long long n_
               : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s;
     if (!(key == key)) key = FLT_MAX;                 // NaN scores rank last
     int id = (int)j;
-    if (better(key, id, keys[KMAX - 1], ids[KMAX - 1])) list_insert(keys, ids, key, id);
+    if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && (!SETS || set.n == 0 || !set_has(set, s_set, id)))
+      list_insert(keys, ids, key, id);
   }
   // merge the 256 sorted lists: k rounds of arg-min over the heads
   int head = 0;
@@ -96,6 +105,7 @@ topk_merge_kernel(const Cand* __restrict__ part, int splits, int k, long long n_
       if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);                 // squared L2 distance
       else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);  // cosine similarity
       else d = -key;                                                           // inner product
+      if (id == kNoId) d = metric == RECNN_METRIC_L2 ? FLT_MAX : -FLT_MAX;       // fewer than k eligible items
       ids_out[q * k + r] = id == kNoId ? -1 : (int64_t)id;
       dist_out[q * k + r] = d;
     }
@@ -147,9 +157,10 @@ extern "C" int64_t recnn_retrieve_workspace_bytes(int64_t n_queries, int64_t n_i
   return retrieve_carve(n_queries, n_items, k, nullptr).bytes;
 }
 
-extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
-                                   int64_t n_items, const float* norms, int32_t metric, int32_t k, int64_t* ids_out,
-                                   float* dist_out, void* workspace, int64_t workspace_bytes, void* stream) {
+// the search behind both entry points; ex.ids NULL: no exclusion
+static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
+                    const float* norms, int32_t metric, int32_t k, const ItemSets& ex, int64_t* ids_out,
+                    float* dist_out, void* workspace, int64_t workspace_bytes, cudaStream_t st) {
   RECNN_REQUIRE(queries && table && ids_out && dist_out && workspace, "null pointer");
   RECNN_REQUIRE(n_queries >= 0 && n_items > 0 && dim > 0, "sizes");
   RECNN_REQUIRE(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_IP || metric == RECNN_METRIC_COS, "metric");
@@ -159,10 +170,10 @@ extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int3
   if (n_queries == 0) return RECNN_OK;
   const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, k, workspace);
   RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t ld = w.ld, slab = w.slab;
   float* scores = w.scores;
   Cand* part = w.part;
+  const int stage = set_stage_bytes(ex);
   const bool tc_ok = dim % 4 == 0 && (reinterpret_cast<uintptr_t>(queries) & 15) == 0 &&
                      (reinterpret_cast<uintptr_t>(table) & 15) == 0;
   for (int64_t q0 = 0; q0 < n_queries; q0 += slab) {
@@ -185,14 +196,36 @@ extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int3
     }
     const int splits = topk_splits(nq, n_items, 32);
     dim3 grid((unsigned)splits, (unsigned)nq);
-    if (k <= 16)
-      topk_partial_kernel<16><<<grid, kTopkThreads, 0, st>>>(scores, ld, n_items, norms, metric, k, part);
-    else
-      topk_partial_kernel<64><<<grid, kTopkThreads, 0, st>>>(scores, ld, n_items, norms, metric, k, part);
+    auto kernel = k <= 16 ? (stage ? topk_partial_kernel<16, true> : topk_partial_kernel<16, false>)
+                          : (stage ? topk_partial_kernel<64, true> : topk_partial_kernel<64, false>);
+    kernel<<<grid, kTopkThreads, stage, st>>>(scores, ld, n_items, norms, metric, k, ex, q0, stage / (int)sizeof(int),
+                                              part);
     RECNN_CHECK_LAUNCH("topk_partial_kernel");
     topk_merge_kernel<<<(unsigned)ceil_div(nq, 4), 128, 0, st>>>(part, splits, k, nq, metric, Q, dim, ids_out + q0 * k,
                                                                   dist_out + q0 * k);
     RECNN_CHECK_LAUNCH("topk_merge_kernel");
   }
   return RECNN_OK;
+}
+
+extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                   int64_t n_items, const float* norms, int32_t metric, int32_t k, int64_t* ids_out,
+                                   float* dist_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  const ItemSets none = {nullptr, nullptr, nullptr, 0, 0, 0};
+  return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, none, ids_out, dist_out, workspace,
+                  workspace_bytes, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                        int64_t n_items, const float* norms, int32_t metric, int32_t k,
+                                        const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                        int64_t n_sets, const int64_t* row_set, int64_t* ids_out, float* dist_out,
+                                        int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream) {
+  ItemSets ex;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_queries, error_flag, &ex));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  if (n_queries > 0) RECNN_PROPAGATE(item_sets_check(ex, n_queries, n_items, error_flag, st));
+  return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, ex, ids_out, dist_out, workspace,
+                  workspace_bytes, st);
 }

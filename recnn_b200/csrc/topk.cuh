@@ -5,6 +5,7 @@
 #pragma once
 
 #include <float.h>
+#include <limits.h>
 
 #include "common.cuh"
 
@@ -99,6 +100,154 @@ __device__ __forceinline__ void list_at(const float (&keys)[KMAX], const int (&i
   k = FLT_MAX; id = kNoId;
 #pragma unroll
   for (int i = 0; i < KMAX; ++i) if (i == head) { k = keys[i]; id = ids[i]; }
+}
+
+// ---- Item-set exclusion: the ids a row must never return ----------------------------------------------------------
+// A table of segments: segment s is ids[offsets[s] : offsets[s + 1]], ascending (duplicates allowed); row r of a call
+// excludes segment row_set[r] (-1: nothing).  Many rows can share one segment, e.g. every window of one user.  Two
+// defaults describe the dense [n_rows, E] form: offsets NULL (segment s is ids[s * stride, (s + 1) * stride)) and
+// row_set NULL (row r -> segment r).  ids NULL: no exclusion.
+struct ItemSets {
+  const long long* ids;
+  const long long* offsets;
+  const long long* row_set;
+  long long total, n_sets;
+  int stride;
+};
+
+// Segments of up to kSetStage ids are staged in shared memory as int32 (16 KB: the select kernels are register bound
+// at 256 threads, so the stage never costs a CTA per SM), longer ones are searched in global memory.
+constexpr int kSetStage = 4096;
+
+// [lo, hi) of row r's segment; empty for -1 and, defensively, for anything out of range (the call's check kernel
+// reports those, and no read here leaves the table)
+__device__ __forceinline__ void set_segment(const ItemSets& s, long long r, long long& lo, long long& hi) {
+  lo = hi = 0;
+  if (!s.ids) return;
+  const long long seg = s.row_set ? s.row_set[r] : r;
+  if (seg < 0 || seg >= s.n_sets) return;
+  long long a = s.offsets ? s.offsets[seg] : seg * s.stride, b = s.offsets ? s.offsets[seg + 1] : a + s.stride;
+  a = a < 0 ? 0 : (a > s.total ? s.total : a);
+  b = b < a ? a : (b > s.total ? s.total : b);
+  lo = a; hi = b;
+}
+
+// a staged id: monotone in the int64 id (sorted stays sorted), and no candidate id (0 <= id < kNoId) is lost
+__device__ __forceinline__ int set_stage_id(long long x) { return x < 0 ? -1 : (x >= kNoId ? kNoId : (int)x); }
+
+// The CTA's view of one row's segment.  set_stage is called by every thread, then __syncthreads before set_has.
+struct SetView {
+  const long long* g;   // the segment in global memory, when it is not staged
+  long long n;
+  bool staged;
+};
+__device__ __forceinline__ SetView set_stage(const ItemSets& s, long long r, int* s_ids, int cap) {
+  long long lo, hi;
+  set_segment(s, r, lo, hi);
+  SetView v = {s.ids ? s.ids + lo : nullptr, hi - lo, hi - lo <= cap};
+  if (v.staged)
+    for (long long e = threadIdx.x; e < v.n; e += blockDim.x) s_ids[e] = set_stage_id(v.g[e]);
+  return v;
+}
+
+// id in the segment: binary search (lower bound) in shared or global memory
+__device__ __forceinline__ bool set_has(const SetView& v, const int* s_ids, int id) {
+  long long lo = 0, hi = v.n;
+  if (v.staged) {
+    while (lo < hi) {
+      const long long mid = (lo + hi) >> 1;
+      if (s_ids[mid] < id) lo = mid + 1; else hi = mid;
+    }
+    return lo < v.n && s_ids[lo] == id;
+  }
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (__ldg(v.g + mid) < id) lo = mid + 1; else hi = mid;
+  }
+  return lo < v.n && __ldg(v.g + lo) == id;
+}
+
+// One warp per row of the call: *flag |= 4 for a row_set outside [-1, n_sets), offsets out of [0, total] or
+// decreasing, or a descending pair in the row's segment; |= 1 for an id outside [0, items).  Only the segments the rows
+// reference are read.
+static __global__ void __launch_bounds__(128)
+item_sets_check_kernel(ItemSets s, long long n_rows, long long items, int* flag) {
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n_rows) return;
+  const long long seg = s.row_set ? s.row_set[r] : r;
+  if (seg < -1 || seg >= s.n_sets) {
+    if (lane == 0) atomicOr(flag, 4);
+    return;
+  }
+  if (seg < 0) return;
+  const long long a = s.offsets ? s.offsets[seg] : seg * s.stride, b = s.offsets ? s.offsets[seg + 1] : a + s.stride;
+  if (a < 0 || b < a || b > s.total) {
+    if (lane == 0) atomicOr(flag, 4);
+    return;
+  }
+  int bits = 0;
+  for (long long e = a + lane; e < b; e += 32) {
+    const long long x = s.ids[e];
+    if (x < 0 || x >= items) bits |= 1;
+    if (e > a && s.ids[e - 1] > x) bits |= 4;
+  }
+  bits = __reduce_or_sync(0xffffffffu, bits);
+  if (lane == 0 && bits) atomicOr(flag, bits);
+}
+
+// One CTA per row of a dense [n_rows, n_ex] list (n_ex <= blockDim.x, a power of two): the row sorted ascending into
+// out, so that the dense form is searched like a table segment
+static __global__ void __launch_bounds__(256)
+exclude_sort_kernel(const long long* __restrict__ ex, int n_ex, long long* __restrict__ out) {
+  __shared__ long long s[256];
+  const long long r = blockIdx.x;
+  const int t = threadIdx.x, n = blockDim.x;
+  s[t] = t < n_ex ? ex[r * n_ex + t] : LLONG_MAX;
+  __syncthreads();
+  for (int size = 2; size <= n; size <<= 1) {            // bitonic sort of n keys, one per thread
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      const int p = t ^ stride;
+      if (p > t) {
+        const long long a = s[t], b = s[p];
+        const bool up = (t & size) == 0;
+        if ((a > b) == up) { s[t] = b; s[p] = a; }
+      }
+      __syncthreads();
+    }
+  }
+  if (t < n_ex) out[r * n_ex + t] = s[t];
+}
+
+static inline int pow2_threads(int n) {
+  int t = 32;
+  while (t < n) t <<= 1;
+  return t;
+}
+
+// the shared-memory stage of a select kernel: none without exclusion
+static inline int set_stage_bytes(const ItemSets& s) { return s.ids ? kSetStage * (int)sizeof(int) : 0; }
+
+// The host checks of a table passed to a *_sets entry point (its contents are checked on the device); row_set NULL
+// maps row r to segment r and then needs n_sets == n_rows.
+static inline int item_sets_args(const int64_t* ids, int64_t total, const int64_t* offsets, int64_t n_sets,
+                                 const int64_t* row_set, int64_t n_rows, const int32_t* error_flag, ItemSets* out) {
+  RECNN_REQUIRE(error_flag && offsets && (ids || total == 0), "null pointer");
+  RECNN_REQUIRE(total >= 0 && n_sets >= 0, "n_set_ids >= 0, n_sets >= 0");
+  RECNN_REQUIRE(row_set || n_sets == n_rows, "without row_set, row r excludes set r: n_sets == n_rows");
+  out->ids = reinterpret_cast<const long long*>(ids);
+  out->offsets = reinterpret_cast<const long long*>(offsets);
+  out->row_set = reinterpret_cast<const long long*>(row_set);
+  out->total = total;
+  out->n_sets = n_sets;
+  out->stride = 0;                                         // ids NULL (an empty table): every segment is empty
+  return RECNN_OK;
+}
+
+static inline int item_sets_check(const ItemSets& s, int64_t n_rows, int64_t items, int* flag, cudaStream_t st) {
+  item_sets_check_kernel<<<(unsigned)ceil_div(n_rows, 4), 128, 0, st>>>(s, n_rows, items, flag);
+  RECNN_CHECK_LAUNCH("item_sets_check_kernel");
+  return RECNN_OK;
 }
 
 }  // namespace recnn

@@ -9,7 +9,9 @@ already resident in HBM for the update step: ``search`` is one exact
 top-k, both in librecnn_b200.so (recnn_retrieve_topk).  No server, no CPU path.
 
 ``ItemIndex(table, metric).search(vecs, topk)`` returns a ``SearchResult`` with
-the reference's accessors ``.id(device)`` / ``.dist(device)``.
+the reference's accessors ``.id(device)`` / ``.dist(device)``; ``exclude=`` an
+``ItemSets`` (recnn_b200/data/item_sets.py) keeps each query's set out of its
+results (recnn_retrieve_topk_sets).
 ``MilvusConnection(env, ...)`` keeps the reference's constructor shape for code
 written against recnn.data.db_con.
 """
@@ -62,8 +64,13 @@ class ItemIndex:
                                                        self.norms.data_ptr(), _lib.stream_ptr(self.device)))
         self._ws = None
 
-    def search(self, search_vecs, topk=10, search_param=None):
-        """search_vecs: [n, dim] (tensor / array on any device).  Returns SearchResult on the index's device."""
+    def search(self, search_vecs, topk=10, search_param=None, exclude=None, exclude_rows=None):
+        """search_vecs: [n, dim] (tensor / array on any device).  Returns SearchResult on the index's device.
+        ``exclude``: an ``ItemSets`` of item ids never returned (e.g. ``DeviceFrameFeed.seen_items()``), with
+        ``exclude_rows`` int64 [n] naming each query's set (-1: none; default query r -> set r).  A query with fewer
+        than topk eligible items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  An excluded id outside
+        [0, n_items) raises IndexError, a malformed table ValueError."""
+        from .item_sets import ItemSets, row_map
         q = torch.as_tensor(search_vecs)
         if q.dim() == 1:
             q = q.unsqueeze(0)
@@ -72,8 +79,15 @@ class ItemIndex:
         topk = int(topk)
         if not 1 <= topk <= min(64, self.n_items):
             raise ValueError("topk must be in [1, min(64, n_items)]")
-        q = q.detach().to(device=self.device, dtype=torch.float32).contiguous()
         n = int(q.shape[0])
+        sets = rows = None
+        if exclude is not None:
+            if not isinstance(exclude, ItemSets):
+                raise ValueError("exclude must be a recnn_b200.data.ItemSets (got %s)" % type(exclude).__name__)
+            sets, rows = row_map(exclude, exclude_rows, n)
+        elif exclude_rows is not None:
+            raise ValueError("exclude_rows maps queries to the sets of an ItemSets exclude")
+        q = q.detach().to(device=self.device, dtype=torch.float32).contiguous()
         ids = torch.empty(n, topk, dtype=torch.int64, device=self.device)
         dist = torch.empty(n, topk, dtype=torch.float32, device=self.device)
         if n == 0:
@@ -82,10 +96,26 @@ class ItemIndex:
         need = L.recnn_retrieve_workspace_bytes(n, self.n_items, topk)
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        args = (q.data_ptr(), n, self.dim, self.table.data_ptr(), self.n_items, _lib.ptr(self.norms), self.metric, topk)
         with torch.cuda.device(self.device):
-            _lib.check(L.recnn_retrieve_topk(q.data_ptr(), n, self.dim, self.table.data_ptr(), self.n_items,
-                                             _lib.ptr(self.norms), self.metric, topk, ids.data_ptr(), dist.data_ptr(),
-                                             self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr(self.device)))
+            if sets is None:
+                _lib.check(L.recnn_retrieve_topk(*args, ids.data_ptr(), dist.data_ptr(), self._ws.data_ptr(),
+                                                 self._ws.numel(), _lib.stream_ptr(self.device)))
+                return SearchResult(ids, dist)
+            sets = sets.to(self.device)
+            rows = None if rows is None else rows.to(self.device).contiguous()
+            flag = torch.empty(1, dtype=torch.int32, device=self.device)
+            _lib.check(L.recnn_retrieve_topk_sets(*args, sets.ids.data_ptr() if sets.ids.numel() else None,
+                                                  sets.ids.numel(), sets.offsets.data_ptr(), len(sets),
+                                                  _lib.ptr(rows), ids.data_ptr(), dist.data_ptr(), flag.data_ptr(),
+                                                  self._ws.data_ptr(), self._ws.numel(),
+                                                  _lib.stream_ptr(self.device)))
+        bits = int(flag.item())
+        if bits & 1:
+            raise IndexError("an excluded item id is out of range for the index's %d items" % self.n_items)
+        if bits & 4:
+            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
         return SearchResult(ids, dist)
 
 

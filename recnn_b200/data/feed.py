@@ -134,6 +134,7 @@ class DeviceFrameFeed:
         self.hist_offsets = up(csr.offsets)
         self.win_offsets = up(csr.win_offsets)
         self._err = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._seen = None
         self.kernels = 0
 
     # ------------------------------------------------------------------ helpers
@@ -244,3 +245,35 @@ class DeviceFrameFeed:
                 action.data_ptr(), reward.data_ptr(), None, _lib.stream_ptr(self.device)))
         return {"state": state, "action": action, "reward": reward, "next_state": next_state,
                 "done": frame_batch["done"], "meta": frame_batch.get("meta", {})}
+
+    # ------------------------------------------------------------------ serving
+    def user_states(self, user_positions):
+        """fp32 [U, F*D + F]: the state after each user's whole history (its last F items and ratings), the state a
+        recommendation for that user is served from -- bit for bit the ``next_state`` of the user's last window, in
+        ``batch_tensor_embeddings``' column order.  A user with exactly F interactions has no window but has this
+        state; fewer than F raises ValueError.  One kernel (recnn_user_states)."""
+        pos = self.csr.check_positions(user_positions)
+        n = int(pos.size)
+        dim = self.table.shape[1]
+        out = torch.empty(n, self.frame_size * dim + self.frame_size, device=self.device)
+        if n == 0:
+            return out
+        users = torch.from_numpy(pos).to(self.device)
+        err = torch.zeros(1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().recnn_user_states(
+                self.table.data_ptr(), self.table.shape[0], dim, self.hist_items.data_ptr(),
+                self.hist_ratings.data_ptr(), self.hist_offsets.data_ptr(), self.csr.n_users, users.data_ptr(), n,
+                self.frame_size, out.data_ptr(), err.data_ptr(), _lib.stream_ptr(self.device)))
+        if int(err.item()) != 0:
+            raise IndexError("user_states: a user position or history item outside the resident histories")
+        return out
+
+    def seen_items(self):
+        """``ItemSets`` with one set per user position of the CSR: the distinct items of that user's history,
+        ascending.  Built on the device once and cached.  ``policy.topk(feed.user_states(pos), k,
+        exclude=feed.seen_items(), exclude_rows=pos)`` recommends only items the users have not rated."""
+        if self._seen is None:
+            from .item_sets import ItemSets
+            self._seen = ItemSets(self.hist_items, self.hist_offsets, unique=True)
+        return self._seen

@@ -174,15 +174,19 @@ class DiscreteActor(nn.Module):
             raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
         return out, gathered
 
-    def topk(self, state, k, exclude=None):
+    def topk(self, state, k, exclude=None, exclude_rows=None):
         """``(values, indices)`` as ``torch.topk(self(state), k)`` without forming the [N, num_items] probabilities:
         the k items of highest logit per row (equal logits: the smaller id first), values fp32 [N, k] = pi(a|s),
         indices int64 [N, k] global item ids, on a vocabulary-parallel policy too (one all-gather of k candidates per
-        row and rank).  ``exclude``: optional integer [N, E] (E <= 256) of ids never returned -- e.g. the frame's
-        items -- that stay in the softmax's normaliser (values are not renormalised); negative ids are padding, an
-        id >= num_items raises IndexError.  A row with fewer than k eligible items ends in id -1, value 0.
-        1 <= k <= min(64, num_items).  Inference only: nothing saved for the policy update is touched."""
+        row and rank).  ``exclude``: ids never returned, which stay in the softmax's normaliser (values are not
+        renormalised) -- either an integer tensor [N, E] (E <= 256, e.g. the frame's items; negative ids are padding)
+        or a ``recnn_b200.data.ItemSets`` table of any length (e.g. ``DeviceFrameFeed.seen_items()``: everything the
+        user has rated), with ``exclude_rows`` int64 [N] naming each row's set (-1: none; default row r -> set r).
+        An excluded id outside [0, num_items) raises IndexError, a malformed table ValueError.  A row with fewer than
+        k eligible items ends in id -1, value 0.  1 <= k <= min(64, num_items).  Inference only: nothing saved for
+        the policy update is touched."""
         from .update.reinforce import _chunk_items
+        from ..data.item_sets import ItemSets, row_map
         vp = self.__dict__.get("_recnn_vp")
         d = self.dims
         items = d.num_items if vp is None else vp.num_items
@@ -192,11 +196,17 @@ class DiscreteActor(nn.Module):
             raise ValueError("state must be a [N, %d] tensor" % d.state_dim)
         n = state.shape[0]
         n_ex = 0
-        if exclude is not None:
+        sets = rows = None
+        if isinstance(exclude, ItemSets):
+            sets, rows = row_map(exclude, exclude_rows, n)
+        elif exclude_rows is not None:
+            raise ValueError("exclude_rows maps rows to the sets of an ItemSets exclude")
+        elif exclude is not None:
             if (not torch.is_tensor(exclude) or exclude.dim() != 2 or exclude.shape[0] != n
                     or exclude.shape[1] > 256 or exclude.dtype.is_floating_point or exclude.dtype == torch.bool):
-                raise ValueError("exclude must be an integer tensor [N, E] with N = %d rows and E <= 256 (got %s)"
-                                 % (n, tuple(exclude.shape) if torch.is_tensor(exclude) else type(exclude).__name__))
+                raise ValueError("exclude must be an ItemSets or an integer tensor [N, E] with N = %d rows and E <= 256 "
+                                 "(got %s)" % (n, tuple(exclude.shape) if torch.is_tensor(exclude)
+                                               else type(exclude).__name__))
             n_ex = exclude.shape[1]
         dev = self.linear1.weight.device
         if dev.type != "cuda":
@@ -207,33 +217,51 @@ class DiscreteActor(nn.Module):
             return values, ids
         _, (state,) = _device_check(self, state)
         ex = None if n_ex == 0 else exclude.detach().to(device=dev, dtype=torch.int64).contiguous()
+        if sets is not None:
+            sets = sets.to(dev)
+            rows = None if rows is None else rows.to(dev).contiguous()
+            table = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
+                     len(sets), _lib.ptr(rows))
         L = _lib.lib()
         flat = param_arena(self)
         chunk = _chunk_items(n, d.num_items)
         nbytes = L.recnn_discrete_topk_workspace_bytes(d, n, k, chunk)
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        flag = torch.empty(1, dtype=torch.int32, device=dev)
+        flag = torch.zeros(2, dtype=torch.int32, device=dev)       # the call's bits, the table check's (sharded)
         with torch.cuda.device(dev):
-            if vp is None:
+            if vp is None and sets is None:
                 _lib.check(L.recnn_discrete_topk(d, flat.data_ptr(), state.data_ptr(), n, k, _lib.ptr(ex), n_ex, chunk,
                                                  values.data_ptr(), ids.data_ptr(), flag.data_ptr(), ws.data_ptr(),
                                                  nbytes, _lib.stream_ptr(dev)))
+            elif vp is None:
+                _lib.check(L.recnn_discrete_topk_sets(d, flat.data_ptr(), state.data_ptr(), n, k, *table, chunk,
+                                                      values.data_ptr(), ids.data_ptr(), flag.data_ptr(),
+                                                      ws.data_ptr(), nbytes, _lib.stream_ptr(dev)))
             else:
                 shard = vp.shard()
                 rec = torch.empty(L.recnn_vocab_topk_record_floats(n, k), device=dev, dtype=torch.float32)
-                _lib.check(L.recnn_discrete_shard_topk(d, shard, flat.data_ptr(), state.data_ptr(), n, k, _lib.ptr(ex),
-                                                       n_ex, chunk, rec.data_ptr(), ws.data_ptr(), nbytes,
-                                                       _lib.stream_ptr(dev)))
+                if sets is None:
+                    _lib.check(L.recnn_discrete_shard_topk(d, shard, flat.data_ptr(), state.data_ptr(), n, k,
+                                                           _lib.ptr(ex), n_ex, chunk, rec.data_ptr(), ws.data_ptr(),
+                                                           nbytes, _lib.stream_ptr(dev)))
+                else:
+                    _lib.check(L.recnn_discrete_shard_topk_sets(d, shard, flat.data_ptr(), state.data_ptr(), n, k,
+                                                                *table, chunk, rec.data_ptr(), flag[1:].data_ptr(),
+                                                                ws.data_ptr(), nbytes, _lib.stream_ptr(dev)))
                 del ws
                 gathered = vp.all_gather(rec)
                 _lib.check(L.recnn_discrete_shard_topk_finish(d, shard, gathered.data_ptr(), n, k, _lib.ptr(ex), n_ex,
                                                               values.data_ptr(), ids.data_ptr(), flag.data_ptr(),
                                                               _lib.stream_ptr(dev)))
-        bits = int(flag.item())
+        f = flag.tolist()
+        bits = f[0] | f[1]
         if bits & 2:
             raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
         if bits & 1:
             raise IndexError("an excluded item id is out of range for the policy's %d items" % items)
+        if bits & 4:
+            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
         return values, ids
 
     def gc(self):
