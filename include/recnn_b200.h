@@ -354,6 +354,23 @@ RECNN_API int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries, 
                                        const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
                                        int64_t n_sets, const int64_t* row_set, int64_t* ids_out, float* dist_out,
                                        int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
+/* Offline evaluation: the exact rank of each query's target item, rank_out int64 [n_queries] = the number of items j
+ * that recnn_retrieve_topk(_sets) over the same queries would put before target[q]: j != target, j not in the row's set
+ * (the target itself is never excluded) and j's key beats the target's (ties: the smaller id).  The target's key is read
+ * from the same score bits the search ranks (same slabs, same GEMM), so for a target not in its set, target[q] is at
+ * position rank_out[q] of the search's ids when rank_out[q] < k and absent otherwise, at any k.  One GEMM and one count
+ * kernel per slab.  *error_flag <- bits: 1 = a target (rank -1) or a set id outside [0, n_items); 4 = a malformed table
+ * (as recnn_retrieve_topk_sets).  workspace_bytes >= recnn_retrieve_rank_workspace_bytes: one slab of scores. */
+RECNN_API int64_t recnn_retrieve_rank_workspace_bytes(int64_t n_queries, int64_t n_items);
+RECNN_API int recnn_retrieve_rank(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                  int64_t n_items, const float* norms, int32_t metric, const int64_t* target,
+                                  int64_t* rank_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                                  void* stream);
+RECNN_API int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                       int64_t n_items, const float* norms, int32_t metric, const int64_t* target,
+                                       const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                       int64_t n_sets, const int64_t* row_set, int64_t* rank_out,
+                                       int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- REINFORCE with (Top-K) off-policy correction: the policy side (SURVEY 8f-2) ------------------
  * DiscreteActor (recnn/nn/models.py:76-99): probs = softmax(W2 relu(W1 s + b1) + b2), one output per item.
@@ -523,6 +540,57 @@ RECNN_API int recnn_discrete_shard_topk_sets(const recnn_discrete_dims* d, const
                                              int64_t n_sets, const int64_t* row_set, int32_t chunk_items,
                                              float* record, int32_t* error_flag, void* workspace,
                                              int64_t workspace_bytes, void* stream);
+/* Offline evaluation: the exact rank of each row's target item under the policy, rank_out int64 [n_rows] = the number
+ * of items j that recnn_discrete_topk(_sets) with the same chunk_items would put before target[r]: j != target, j not in
+ * the row's set (the target itself is never excluded) and logit_j > logit_t, equal logits to the smaller id, NaN and
+ * -inf logits last.  log_prob_out fp32 [n_rows] = log pi(target | state) = z_t - M - log S.  Pass 1 is the policy
+ * gradient's stats pass with action = target; pass 2 recomputes the chunks, last chunk first (one GEMM in all with one
+ * chunk), and counts the beating ids of each.  The logits are topk's own bits, so for a target not in its set, target[r]
+ * is at position rank_out[r] of topk's ids when rank_out[r] < k and absent otherwise, at any k.  Deterministic (integer
+ * atomics).  *error_flag <- bits: 1 = a target (rank -1, log-prob 0) or a set id outside [0, num_items); 4 = a
+ * malformed table (as recnn_retrieve_topk_sets).  workspace_bytes >= recnn_discrete_rank_workspace_bytes: the state
+ * image, the hidden layer, one [n_rows, chunk_items] logits block and four [n_rows] planes. */
+RECNN_API int64_t recnn_discrete_rank_workspace_bytes(const recnn_discrete_dims* d, int64_t n_rows,
+                                                      int32_t chunk_items);   /* 0 when chunk_items is refused */
+RECNN_API int recnn_discrete_rank(const recnn_discrete_dims* d, const float* params, const float* state,
+                                  const int64_t* target, int64_t n_rows, int32_t chunk_items, int64_t* rank_out,
+                                  float* log_prob_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                                  void* stream);
+RECNN_API int recnn_discrete_rank_sets(const recnn_discrete_dims* d, const float* params, const float* state,
+                                       const int64_t* target, int64_t n_rows, const int64_t* set_ids,
+                                       int64_t n_set_ids, const int64_t* set_offsets, int64_t n_sets,
+                                       const int64_t* row_set, int32_t chunk_items, int64_t* rank_out,
+                                       float* log_prob_out, int32_t* error_flag, void* workspace,
+                                       int64_t workspace_bytes, void* stream);
+/* The same on a vocabulary-sharded policy (d: the LOCAL dims; target: global ids), around two all-gathers.
+ * shard_rank_stats runs pass 1 over the rank's block on the rank workspace and writes the stats record of
+ * recnn_reinforce_shard_stats (recnn_vocab_record_floats(n_rows): header, local max, local sum of exp, the target's
+ * logit from its owner).  After recnn_comm_allgather of those records, shard_rank(_sets) runs pass 2 over the block with
+ * global ids, on the same workspace untouched since, and writes a count record of recnn_vocab_rank_record_floats(n_rows)
+ * floats: the header, then n_rows int32 counts; the _sets form checks the table (bits 1 and 4, the same on every rank).
+ * After the all-gather of the count records, shard_rank_finish sums the counts in rank order and merges M, S and the
+ * target's logit in rank order (recnn_discrete_shard_finish's merge): every rank writes the same bits, and at world 1 the
+ * phases compute what recnn_discrete_rank(_sets) does.  Its *error_flag <- bits: 1 = a target outside [0, num_items);
+ * 2 = the headers of either record set do not tile the vocabulary in rank order with this rank's block. */
+RECNN_API int64_t recnn_vocab_rank_record_floats(int64_t n_rows);
+RECNN_API int recnn_discrete_shard_rank_stats(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                              const float* params, const float* state, const int64_t* target,
+                                              int64_t n_rows, int32_t chunk_items, float* record, void* workspace,
+                                              int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_rank(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                        const int64_t* target, int64_t n_rows, int32_t chunk_items,
+                                        const float* gathered, float* record, void* workspace,
+                                        int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_rank_sets(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                             const float* params, const int64_t* target, int64_t n_rows,
+                                             const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                             int64_t n_sets, const int64_t* row_set, int32_t chunk_items,
+                                             const float* gathered, float* record, int32_t* error_flag,
+                                             void* workspace, int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_rank_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                               const float* gathered_stats, const float* gathered_counts,
+                                               const int64_t* target, int64_t n_rows, int64_t* rank_out,
+                                               float* log_prob_out, int32_t* error_flag, void* stream);
 
 /* ---- REINFORCE: the critic side with item-id actions ---------------------------------------------
  * The REINFORCE critic is a Critic(S, num_items, H) (recnn/nn/update/reinforce.py:92-102): layer 1 is W1 [H, S + num_items]

@@ -148,6 +148,12 @@ SIGNATURES = {
                                            C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                            C.c_void_p]),
+    "recnn_retrieve_rank_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int64]),
+    "recnn_retrieve_rank": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_retrieve_rank_sets": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
+                                           C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "recnn_discrete_layout": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(C.c_int64)]),
     "recnn_discrete_scratch_floats": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32]),
     "recnn_discrete_forward": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
@@ -199,7 +205,28 @@ SIGNATURES = {
                                                  C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
                                                  C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_int64, C.c_void_p]),
-    "recnn_critic_action_term_scratch_floats": (C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
+    "recnn_discrete_rank_workspace_bytes": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32]),
+    "recnn_discrete_rank": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                      C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                      C.c_void_p]),
+    "recnn_discrete_rank_sets": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_vocab_rank_record_floats": (C.c_int64, [C.c_int64]),
+    "recnn_discrete_shard_rank_stats": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
+                                                  C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_discrete_shard_rank": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                            C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                            C.c_void_p]),
+    "recnn_discrete_shard_rank_sets": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                 C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                 C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_discrete_shard_rank_finish": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]),
+    "recnn_critic_action_term_scratch_floats":(C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                             C.c_int32]),
     "recnn_critic_action_term_chunked": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.POINTER(DiscreteDims), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p,

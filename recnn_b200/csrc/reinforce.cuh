@@ -844,6 +844,142 @@ static int dense_sets(const long long* exclude, int64_t n, int n_ex, const TopkW
   return RECNN_OK;
 }
 
+// ---- The exact rank of each row's target item (offline evaluation): the number of eligible items j that the row's
+// top-k would put before t, i.e. j != t, j not excluded and better(logit_key(z_j), j, logit_key(z_t), t).  Pass 1 is
+// the policy gradient's stats pass with action = target (max, sum of exp and the target's logit za); pass 2 walks the
+// chunks again, last chunk first (its logits are still in z), and counts the beating ids of each chunk with integer
+// atomics (deterministic).  Both passes make the logits with the discrete_logits calls of topk's chunking, so the
+// counts compare topk's own bits.
+
+// grid (splits, rows): counts[r] += the ids id0 + j of columns [lo, hi) of z's row r that beat the target, minus the
+// excluded ones (SETS).  za: the target's logit; a target outside [0, items) counts nothing.
+template <bool SETS>
+__global__ void __launch_bounds__(kTopkThreads)
+policy_rank_count_kernel(const float* __restrict__ z, long long n, int w, int id0, int items,
+                         const long long* __restrict__ target, const float* __restrict__ za, ItemSets ex,
+                         int* __restrict__ counts) {
+  __shared__ long long s_range[3];
+  const int sp = blockIdx.x, splits = gridDim.x;
+  const int per = (w + splits - 1) / splits;
+  const int lo = sp * per, hi = min(w, lo + per);
+  for (long long r = blockIdx.y; r < n; r += gridDim.y) {
+    const long long t = target[r];
+    if (t < 0 || t >= items) continue;                        // the same decision in every thread
+    const float kt = logit_key(za[r]);
+    const float* row = z + r * w;
+    int c = 0;
+    for (int j = lo + threadIdx.x; j < hi; j += blockDim.x) {
+      const int id = id0 + j;
+      c += id != (int)t && better(logit_key(row[j]), id, kt, (int)t);
+    }
+    if (SETS)
+      c -= excluded_beaters(ex, r, (long long)id0 + lo, (long long)id0 + hi, kt, (int)t,
+                            [&](long long x) { return logit_key(row[x - id0]); }, s_range);
+    c = __reduce_add_sync(0xffffffffu, c);
+    if ((threadIdx.x & 31) == 0 && c != 0) atomicAdd(counts + r, c);
+  }
+}
+
+// log pi(t | s) from the row's max M, sum of exp S and the target's logit
+__device__ __forceinline__ float target_log_prob(float za, float M, float S) { return (za - M) - logf(S); }
+
+// one thread per row: rank (-1 for a target outside [0, items)) and log pi(t | s)
+__global__ void policy_rank_finish_kernel(const int* __restrict__ counts, const float* __restrict__ za,
+                                          const float* __restrict__ run_max, const float* __restrict__ run_sum,
+                                          const long long* __restrict__ target, long long n, int items,
+                                          long long* __restrict__ rank, float* __restrict__ logp) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const bool ok = target[r] >= 0 && target[r] < items;
+  rank[r] = ok ? counts[r] : -1;
+  logp[r] = ok ? target_log_prob(za[r], run_max[r], run_sum[r]) : 0.f;
+}
+
+struct RankWorkspace {
+  DiscreteScratch s;           // img, h, z ([n, chunk]), run_max, run_sum and za for the passes
+  int* counts;                 // [n] (the unsharded call)
+  int64_t bytes;
+};
+static RankWorkspace rank_carve(const recnn_discrete_dims& d, int64_t n, int chunk, void* base) {
+  RankWorkspace w;
+  Carve c(base);
+  memset(&w.s, 0, sizeof(w.s));
+  w.s.img = c.take(n * pad4(d.state_dim));
+  w.s.h = c.take(n * d.hidden);
+  w.s.z = c.take(n * (int64_t)chunk);
+  w.s.run_max = c.take(n);
+  w.s.run_sum = c.take(n);
+  w.s.za = c.take(n);
+  w.counts = c.take<int>(n);
+  w.bytes = c.bytes();
+  return w;
+}
+
+// Pass 2 over the arena's items (global ids id0 + the local item, the last chunk's logits already in s.z): counts +=
+// the beating ids of every chunk.  items: the whole vocabulary.
+static int rank_count_pass(const recnn_discrete_dims& d, const float* params, int64_t n, const DiscreteScratch& s,
+                           int chunk, int id0, int items, const long long* target, const float* za, const ItemSets& ex,
+                           int* counts, cudaStream_t st) {
+  const int I = d.num_items;
+  const int n_chunks = (int)ceil_div(I, chunk);
+  auto count = ex.ids ? policy_rank_count_kernel<true> : policy_rank_count_kernel<false>;
+  for (int c = n_chunks - 1; c >= 0; --c) {
+    const int c0 = c * chunk, w = I - c0 < chunk ? I - c0 : chunk;
+    if (c != n_chunks - 1) RECNN_PROPAGATE(discrete_logits(d, params, n, s, c0, w, s.z, st));
+    const dim3 grid((unsigned)topk_splits(n, w, 32), (unsigned)(n < 65535 ? n : 65535));
+    count<<<grid, kTopkThreads, 0, st>>>(s.z, n, w, id0 + c0, items, target, za, ex, counts);
+    RECNN_CHECK_LAUNCH("policy_rank_count_kernel");
+  }
+  return RECNN_OK;
+}
+
+// A rank's count record (vocabulary-parallel rank): the header {lo, hi, num_items, n_rows}, then n int32 counts of the
+// rank's block.
+__host__ __device__ __forceinline__ int64_t rank_record_floats(int64_t n) { return kShardHeader + n; }
+
+__global__ void rank_record_init_kernel(float* __restrict__ rec, long long n, ShardPlan p) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) reinterpret_cast<int*>(shard_plane(rec, n, 0))[i] = 0;
+  if (i == 0) shard_header_write(rec, p, n);
+}
+
+// gathered stats records -> za[r], the target's logit: the rank-order sum of shard_merge_row (every plane but the
+// owner's holds 0)
+__global__ void shard_target_logit_kernel(const float* __restrict__ g, long long n, int W, float* __restrict__ za) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const long long stride = shard_record_floats(n);
+  float z = 0.f;
+  for (int q = 0; q < W; ++q) z += shard_plane(g, n, 2, q, stride)[r];
+  za[r] = z;
+}
+
+// gathered stats and count records -> every rank's (rank, log pi): M, S and za merged in rank order (shard_merge_row),
+// the counts summed in rank order.  *flag |= 2 when either set of headers does not tile the vocabulary with this rank's
+// block, |= 1 for a target outside [0, items).
+__global__ void shard_rank_finish_kernel(const float* __restrict__ gs, const float* __restrict__ gc, long long n,
+                                         ShardPlan p, const long long* __restrict__ target, long long* __restrict__ rank,
+                                         float* __restrict__ logp, int* flag) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r == 0 && (shard_plan_bad(gs, shard_record_floats(n), p, n) || shard_plan_bad(gc, rank_record_floats(n), p, n)))
+    atomicOr(flag, 2);
+  if (r >= n) return;
+  const long long t = target[r];
+  if (t < 0 || t >= p.items) {
+    atomicOr(flag, 1);
+    rank[r] = -1;
+    logp[r] = 0.f;
+    return;
+  }
+  float M, S, za;
+  shard_merge_row(gs, p.world, n, r, M, S, za);
+  long long c = 0;
+  for (int q = 0; q < p.world; ++q)
+    c += reinterpret_cast<const int*>(shard_plane(gc, n, 0, q, rank_record_floats(n)))[r];
+  rank[r] = c;
+  logp[r] = target_log_prob(za, M, S);
+}
+
 }  // namespace recnn
 
 using namespace recnn;
@@ -1239,5 +1375,159 @@ extern "C" int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, co
   policy_topk_shard_finish_kernel<<<(unsigned)ceil_div(n_rows, 4), 128, 0, st>>>(
       gathered, n_rows, k, p, values_out, reinterpret_cast<long long*>(ids_out), error_flag);
   RECNN_CHECK_LAUNCH("policy_topk_shard_finish_kernel");
+  return RECNN_OK;
+}
+
+// ---- the exact rank of each row's target ---------------------------------------------------------------------
+extern "C" int64_t recnn_discrete_rank_workspace_bytes(const recnn_discrete_dims* d, int64_t n_rows,
+                                                       int32_t chunk_items) {
+  if (!discrete_dims_ok(d) || n_rows <= 0 || !chunk_ok(d->num_items, chunk_items)) return 0;
+  return rank_carve(*d, n_rows, chunk_items, nullptr).bytes;
+}
+
+// the checks of every rank entry point that runs a pass
+static int rank_check(const recnn_discrete_dims* d, const float* params, const int64_t* target, int64_t n_rows,
+                      int32_t chunk_items, const int32_t* error_flag, void* workspace, int64_t workspace_bytes) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && target && error_flag && workspace, "null pointer / dims");
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  return check_workspace(rank_carve(*d, n_rows, chunk_items, nullptr).bytes, workspace_bytes);
+}
+
+// both passes and the finish of an unsharded call
+static int rank_local(const recnn_discrete_dims& d, const float* params, const float* state, const long long* target,
+                      int64_t n, const ItemSets& sets, int chunk, int64_t* rank_out, float* log_prob_out, int* flag,
+                      const RankWorkspace& w, cudaStream_t st) {
+  const DiscreteScratch& s = w.s;
+  RECNN_CHECK_CUDA(cudaMemsetAsync(w.counts, 0, n * sizeof(int), st));
+  RECNN_PROPAGATE(rank_target_check(target, n, d.num_items, flag, st));
+  RECNN_PROPAGATE(discrete_hidden(d, params, state, n, s, st, nullptr));
+  RECNN_PROPAGATE(reinforce_stats_pass(d, params, n, s, chunk, target, 0, s.run_max, s.run_sum, s.za, st));
+  RECNN_PROPAGATE(rank_count_pass(d, params, n, s, chunk, 0, d.num_items, target, s.za, sets, w.counts, st));
+  policy_rank_finish_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(
+      w.counts, s.za, s.run_max, s.run_sum, target, n, d.num_items, reinterpret_cast<long long*>(rank_out),
+      log_prob_out);
+  RECNN_CHECK_LAUNCH("policy_rank_finish_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_rank(const recnn_discrete_dims* d, const float* params, const float* state,
+                                   const int64_t* target, int64_t n_rows, int32_t chunk_items, int64_t* rank_out,
+                                   float* log_prob_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                                   void* stream) {
+  RECNN_REQUIRE(state && rank_out && log_prob_out, "null pointer");
+  RECNN_PROPAGATE(rank_check(d, params, target, n_rows, chunk_items, error_flag, workspace, workspace_bytes));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const RankWorkspace w = rank_carve(*d, n_rows, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  const ItemSets none = {nullptr, nullptr, nullptr, 0, 0, 0};
+  return rank_local(*d, params, state, reinterpret_cast<const long long*>(target), n_rows, none, chunk_items, rank_out,
+                    log_prob_out, error_flag, w, st);
+}
+
+extern "C" int recnn_discrete_rank_sets(const recnn_discrete_dims* d, const float* params, const float* state,
+                                        const int64_t* target, int64_t n_rows, const int64_t* set_ids,
+                                        int64_t n_set_ids, const int64_t* set_offsets, int64_t n_sets,
+                                        const int64_t* row_set, int32_t chunk_items, int64_t* rank_out,
+                                        float* log_prob_out, int32_t* error_flag, void* workspace,
+                                        int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(state && rank_out && log_prob_out, "null pointer");
+  RECNN_PROPAGATE(rank_check(d, params, target, n_rows, chunk_items, error_flag, workspace, workspace_bytes));
+  ItemSets sets;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_rows, error_flag, &sets));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const RankWorkspace w = rank_carve(*d, n_rows, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(item_sets_check(sets, n_rows, d->num_items, error_flag, st));
+  return rank_local(*d, params, state, reinterpret_cast<const long long*>(target), n_rows, sets, chunk_items, rank_out,
+                    log_prob_out, error_flag, w, st);
+}
+
+extern "C" int64_t recnn_vocab_rank_record_floats(int64_t n_rows) { return n_rows > 0 ? rank_record_floats(n_rows) : 0; }
+
+extern "C" int recnn_discrete_shard_rank_stats(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                               const float* params, const float* state, const int64_t* target,
+                                               int64_t n_rows, int32_t chunk_items, float* record, void* workspace,
+                                               int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && state && target && record && workspace, "null pointer / dims");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_PROPAGATE(check_workspace(rank_carve(*d, n_rows, chunk_items, nullptr).bytes, workspace_bytes));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const RankWorkspace w = rank_carve(*d, n_rows, chunk_items, workspace);
+  RECNN_PROPAGATE(discrete_hidden(*d, params, state, n_rows, w.s, st, nullptr));
+  RECNN_PROPAGATE(shard_record_init(p, record, n_rows, st));
+  return reinforce_stats_pass(*d, params, n_rows, w.s, chunk_items, reinterpret_cast<const long long*>(target), p.lo,
+                              shard_plane(record, n_rows, 0), shard_plane(record, n_rows, 1),
+                              shard_plane(record, n_rows, 2), st);
+}
+
+// the count pass over the rank's block from the gathered stats records, into the rank's count record
+static int shard_rank_local(const recnn_discrete_dims& d, const ShardPlan& p, const float* params,
+                            const long long* target, int64_t n, const ItemSets& sets, int chunk, const float* gathered,
+                            float* record, const RankWorkspace& w, cudaStream_t st) {
+  shard_target_logit_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(gathered, n, p.world, w.s.za);
+  RECNN_CHECK_LAUNCH("shard_target_logit_kernel");
+  rank_record_init_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(record, n, p);
+  RECNN_CHECK_LAUNCH("rank_record_init_kernel");
+  return rank_count_pass(d, params, n, w.s, chunk, p.lo, p.items, target, w.s.za, sets,
+                         reinterpret_cast<int*>(shard_plane(record, n, 0)), st);
+}
+
+extern "C" int recnn_discrete_shard_rank(const recnn_discrete_dims* d, const recnn_vocab_shard* v, const float* params,
+                                         const int64_t* target, int64_t n_rows, int32_t chunk_items,
+                                         const float* gathered, float* record, void* workspace,
+                                         int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && target && gathered && record && workspace, "null pointer / dims");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_PROPAGATE(check_workspace(rank_carve(*d, n_rows, chunk_items, nullptr).bytes, workspace_bytes));
+  const RankWorkspace w = rank_carve(*d, n_rows, chunk_items, workspace);
+  const ItemSets none = {nullptr, nullptr, nullptr, 0, 0, 0};
+  return shard_rank_local(*d, p, params, reinterpret_cast<const long long*>(target), n_rows, none, chunk_items,
+                          gathered, record, w, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int recnn_discrete_shard_rank_sets(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                              const float* params, const int64_t* target, int64_t n_rows,
+                                              const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                              int64_t n_sets, const int64_t* row_set, int32_t chunk_items,
+                                              const float* gathered, float* record, int32_t* error_flag,
+                                              void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && params && target && gathered && record && workspace, "null pointer / dims");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  RECNN_PROPAGATE(check_workspace(rank_carve(*d, n_rows, chunk_items, nullptr).bytes, workspace_bytes));
+  ItemSets sets;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_rows, error_flag, &sets));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const RankWorkspace w = rank_carve(*d, n_rows, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(item_sets_check(sets, n_rows, p.items, error_flag, st));   // global ids: every rank agrees
+  return shard_rank_local(*d, p, params, reinterpret_cast<const long long*>(target), n_rows, sets, chunk_items,
+                          gathered, record, w, st);
+}
+
+extern "C" int recnn_discrete_shard_rank_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                const float* gathered_stats, const float* gathered_counts,
+                                                const int64_t* target, int64_t n_rows, int64_t* rank_out,
+                                                float* log_prob_out, int32_t* error_flag, void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && gathered_stats && gathered_counts && target && rank_out && log_prob_out &&
+                    error_flag, "null pointer / dims");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  shard_rank_finish_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
+      gathered_stats, gathered_counts, n_rows, p, reinterpret_cast<const long long*>(target),
+      reinterpret_cast<long long*>(rank_out), log_prob_out, error_flag);
+  RECNN_CHECK_LAUNCH("shard_rank_finish_kernel");
   return RECNN_OK;
 }

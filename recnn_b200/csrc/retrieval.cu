@@ -37,6 +37,14 @@ item_norms_kernel(const float* __restrict__ table, long long n_items, int dim, i
   if (lane == 0) out[row] = metric == RECNN_METRIC_COS ? 1.0f / fmaxf(sqrtf(s), 1e-30f) : s;
 }
 
+// the key of item j from its score: smaller is better; NaN scores rank last
+__device__ __forceinline__ float score_key(float s, const float* __restrict__ norms, long long j, int metric) {
+  float key = metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
+            : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s;
+  if (!(key == key)) key = FLT_MAX;
+  return key;
+}
+
 // grid (splits, n_queries).  scores [n_queries, ld]; writes k candidates per (query, split), ascending.  Query q is
 // row row0 + q of the call; with SETS its excluded set (ex) is tested only for a candidate that enters the thread's
 // list (without, the kernel is the plain search, nothing staged).
@@ -60,10 +68,7 @@ topk_partial_kernel(const float* __restrict__ scores, long long ld, long long n_
   int ids[KMAX];
   list_clear(keys, ids);
   for (long long j = lo + threadIdx.x; j < hi; j += blockDim.x) {
-    const float s = __ldcs(row + j);
-    float key = metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
-              : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s;
-    if (!(key == key)) key = FLT_MAX;                 // NaN scores rank last
+    const float key = score_key(__ldcs(row + j), norms, j, metric);
     int id = (int)j;
     if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && (!SETS || set.n == 0 || !set_has(set, s_set, id)))
       list_insert(keys, ids, key, id);
@@ -112,6 +117,43 @@ topk_merge_kernel(const Cand* __restrict__ part, int splits, int k, long long n_
   }
 }
 
+// grid (splits, n_queries): rank[row0 + q] += the items of columns [lo, hi) that beat the query's target by
+// score_key (ties: the smaller id), minus the excluded ones (SETS).  The target's key is read from the same scores row,
+// so every comparison is between the bits the search ranks.  A target outside [0, n_items) counts nothing.
+template <bool SETS>
+__global__ void __launch_bounds__(kTopkThreads)
+rank_count_kernel(const float* __restrict__ scores, long long ld, long long n_items, const float* __restrict__ norms,
+                  int metric, const long long* __restrict__ target, ItemSets ex, long long row0,
+                  long long* __restrict__ rank) {
+  __shared__ long long s_range[3];
+  const int q = blockIdx.y, sp = blockIdx.x, splits = gridDim.x;
+  const long long per = (n_items + splits - 1) / splits;
+  const long long lo = sp * per, hi = min(n_items, lo + per);
+  const long long t = target[row0 + q];
+  if (t < 0 || t >= n_items) return;
+  const float* row = scores + (long long)q * ld;
+  const float kt = score_key(row[t], norms, t, metric);
+  int c = 0;
+  for (long long j = lo + threadIdx.x; j < hi; j += blockDim.x)
+    c += j != t && better(score_key(__ldcs(row + j), norms, j, metric), (int)j, kt, (int)t);
+  if (SETS)
+    c -= excluded_beaters(ex, row0 + q, lo, hi, kt, (int)t,
+                          [&](long long x) { return score_key(row[x], norms, x, metric); }, s_range);
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c != 0)
+    atomicAdd(reinterpret_cast<unsigned long long*>(rank + row0 + q), (unsigned long long)(long long)c);
+}
+
+// rank[q] <- 0, or -1 and *flag |= 1 for a target outside [0, n_items)
+__global__ void rank_init_kernel(const long long* __restrict__ target, long long n, long long n_items,
+                                 long long* __restrict__ rank, int* flag) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= n) return;
+  const bool ok = target[q] >= 0 && target[q] < n_items;
+  rank[q] = ok ? 0 : -1;
+  if (!ok) atomicOr(flag, 1);
+}
+
 static int64_t slab_rows(int64_t n_items) {
   // a slab of scores should stay L2-resident between the GEMM that writes it and the top-k pass that reads it:
   // 32 MB of the H100's 50 MB L2, leaving room for the item table, its norms and the top-k partials
@@ -157,32 +199,21 @@ extern "C" int64_t recnn_retrieve_workspace_bytes(int64_t n_queries, int64_t n_i
   return retrieve_carve(n_queries, n_items, k, nullptr).bytes;
 }
 
-// the search behind both entry points; ex.ids NULL: no exclusion
-static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
-                    const float* norms, int32_t metric, int32_t k, const ItemSets& ex, int64_t* ids_out,
-                    float* dist_out, void* workspace, int64_t workspace_bytes, cudaStream_t st) {
-  RECNN_REQUIRE(queries && table && ids_out && dist_out && workspace, "null pointer");
-  RECNN_REQUIRE(n_queries >= 0 && n_items > 0 && dim > 0, "sizes");
-  RECNN_REQUIRE(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_IP || metric == RECNN_METRIC_COS, "metric");
-  RECNN_REQUIRE(metric == RECNN_METRIC_IP || norms != nullptr, "L2 / COS need recnn_item_norms");
-  RECNN_REQUIRE(k >= 1 && k <= 64 && k <= n_items, "1 <= k <= min(64, n_items)");
-  RECNN_REQUIRE(n_items < (1ll << 31), "n_items must fit int32");
-  if (n_queries == 0) return RECNN_OK;
-  const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, k, workspace);
-  RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
-  const int64_t ld = w.ld, slab = w.slab;
-  float* scores = w.scores;
-  Cand* part = w.part;
-  const int stage = set_stage_bytes(ex);
+// The slab loop of every retrieval call: for each slab of up to w.slab query rows, scores[q, j] = <query q0 + q,
+// item j> into w.scores (the tensor-core GEMM when the operands allow it, else the CUDA-core one: one choice per call),
+// then after(q0, nq) reads the slab.  A search and a rank over the same queries see the same score bits.
+template <class After>
+static int retrieve_slabs(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
+                          const RetrieveWorkspace& w, cudaStream_t st, After after) {
   const bool tc_ok = dim % 4 == 0 && (reinterpret_cast<uintptr_t>(queries) & 15) == 0 &&
                      (reinterpret_cast<uintptr_t>(table) & 15) == 0;
-  for (int64_t q0 = 0; q0 < n_queries; q0 += slab) {
-    const int64_t nq = n_queries - q0 < slab ? n_queries - q0 : slab;
+  for (int64_t q0 = 0; q0 < n_queries; q0 += w.slab) {
+    const int64_t nq = n_queries - q0 < w.slab ? n_queries - q0 : w.slab;
     const float* Q = queries + q0 * dim;
     Epilogue e;
     memset(&e, 0, sizeof(e));
-    e.out = scores;
-    e.ldo = ld;
+    e.out = w.scores;
+    e.ldo = w.ld;
     if (tc_ok) {
       tc::Operand a0 = {Q, dim, 0, 0}, a1 = {nullptr, 0, 0, 0}, b = {table, dim, n_items, dim};
       tc::Problem p;
@@ -194,18 +225,68 @@ static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const 
       RECNN_PROPAGATE((launch_gemm_simt<true, true, EPI_STORE>(mat(Q, dim), mat(table, dim), (int)nq, (int)n_items, dim,
                                                                 1, e, st)));
     }
-    const int splits = topk_splits(nq, n_items, 32);
-    dim3 grid((unsigned)splits, (unsigned)nq);
-    auto kernel = k <= 16 ? (stage ? topk_partial_kernel<16, true> : topk_partial_kernel<16, false>)
-                          : (stage ? topk_partial_kernel<64, true> : topk_partial_kernel<64, false>);
-    kernel<<<grid, kTopkThreads, stage, st>>>(scores, ld, n_items, norms, metric, k, ex, q0, stage / (int)sizeof(int),
-                                              part);
-    RECNN_CHECK_LAUNCH("topk_partial_kernel");
-    topk_merge_kernel<<<(unsigned)ceil_div(nq, 4), 128, 0, st>>>(part, splits, k, nq, metric, Q, dim, ids_out + q0 * k,
-                                                                  dist_out + q0 * k);
-    RECNN_CHECK_LAUNCH("topk_merge_kernel");
+    RECNN_PROPAGATE(after(q0, nq));
   }
   return RECNN_OK;
+}
+
+// the argument checks of every retrieval call
+static int retrieve_check(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
+                          const float* norms, int32_t metric, const void* workspace) {
+  RECNN_REQUIRE(queries && table && workspace, "null pointer");
+  RECNN_REQUIRE(n_queries >= 0 && n_items > 0 && dim > 0, "sizes");
+  RECNN_REQUIRE(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_IP || metric == RECNN_METRIC_COS, "metric");
+  RECNN_REQUIRE(metric == RECNN_METRIC_IP || norms != nullptr, "L2 / COS need recnn_item_norms");
+  RECNN_REQUIRE(n_items < (1ll << 31), "n_items must fit int32");
+  return RECNN_OK;
+}
+
+// the search behind both entry points; ex.ids NULL: no exclusion
+static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
+                    const float* norms, int32_t metric, int32_t k, const ItemSets& ex, int64_t* ids_out,
+                    float* dist_out, void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+  RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
+  RECNN_REQUIRE(ids_out && dist_out, "null pointer");
+  RECNN_REQUIRE(k >= 1 && k <= 64 && k <= n_items, "1 <= k <= min(64, n_items)");
+  if (n_queries == 0) return RECNN_OK;
+  const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, k, workspace);
+  RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
+  const int stage = set_stage_bytes(ex);
+  auto kernel = k <= 16 ? (stage ? topk_partial_kernel<16, true> : topk_partial_kernel<16, false>)
+                        : (stage ? topk_partial_kernel<64, true> : topk_partial_kernel<64, false>);
+  return retrieve_slabs(queries, n_queries, dim, table, n_items, w, st, [&](int64_t q0, int64_t nq) {
+    const float* Q = queries + q0 * dim;
+    const int splits = topk_splits(nq, n_items, 32);
+    dim3 grid((unsigned)splits, (unsigned)nq);
+    kernel<<<grid, kTopkThreads, stage, st>>>(w.scores, w.ld, n_items, norms, metric, k, ex, q0,
+                                              stage / (int)sizeof(int), w.part);
+    RECNN_CHECK_LAUNCH("topk_partial_kernel");
+    topk_merge_kernel<<<(unsigned)ceil_div(nq, 4), 128, 0, st>>>(w.part, splits, k, nq, metric, Q, dim,
+                                                                  ids_out + q0 * k, dist_out + q0 * k);
+    RECNN_CHECK_LAUNCH("topk_merge_kernel");
+    return RECNN_OK;
+  });
+}
+
+// the rank behind both entry points: the slab's GEMM, then one count kernel per slab
+static int retrieve_rank(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
+                         const float* norms, int32_t metric, const int64_t* target, const ItemSets& ex,
+                         int64_t* rank_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                         cudaStream_t st) {
+  if (n_queries == 0) return RECNN_OK;
+  const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, 0, workspace);
+  RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
+  const long long* tgt = reinterpret_cast<const long long*>(target);
+  long long* rank = reinterpret_cast<long long*>(rank_out);
+  rank_init_kernel<<<(unsigned)ceil_div(n_queries, 256), 256, 0, st>>>(tgt, n_queries, n_items, rank, error_flag);
+  RECNN_CHECK_LAUNCH("rank_init_kernel");
+  auto kernel = ex.ids ? rank_count_kernel<true> : rank_count_kernel<false>;
+  return retrieve_slabs(queries, n_queries, dim, table, n_items, w, st, [&](int64_t q0, int64_t nq) {
+    dim3 grid((unsigned)topk_splits(nq, n_items, 32), (unsigned)nq);
+    kernel<<<grid, kTopkThreads, 0, st>>>(w.scores, w.ld, n_items, norms, metric, tgt, ex, q0, rank);
+    RECNN_CHECK_LAUNCH("rank_count_kernel");
+    return RECNN_OK;
+  });
 }
 
 extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
@@ -228,4 +309,38 @@ extern "C" int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries,
   if (n_queries > 0) RECNN_PROPAGATE(item_sets_check(ex, n_queries, n_items, error_flag, st));
   return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, ex, ids_out, dist_out, workspace,
                   workspace_bytes, st);
+}
+
+extern "C" int64_t recnn_retrieve_rank_workspace_bytes(int64_t n_queries, int64_t n_items) {
+  if (n_queries <= 0 || n_items <= 0) return 0;
+  return retrieve_carve(n_queries, n_items, 0, nullptr).bytes;
+}
+
+extern "C" int recnn_retrieve_rank(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                   int64_t n_items, const float* norms, int32_t metric, const int64_t* target,
+                                   int64_t* rank_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                                   void* stream) {
+  RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
+  RECNN_REQUIRE(target && rank_out && error_flag, "null pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  const ItemSets none = {nullptr, nullptr, nullptr, 0, 0, 0};
+  return retrieve_rank(queries, n_queries, dim, table, n_items, norms, metric, target, none, rank_out, error_flag,
+                       workspace, workspace_bytes, st);
+}
+
+extern "C" int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                                        int64_t n_items, const float* norms, int32_t metric, const int64_t* target,
+                                        const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                        int64_t n_sets, const int64_t* row_set, int64_t* rank_out,
+                                        int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
+  RECNN_REQUIRE(target && rank_out, "null pointer");
+  ItemSets ex;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_queries, error_flag, &ex));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  if (n_queries > 0) RECNN_PROPAGATE(item_sets_check(ex, n_queries, n_items, error_flag, st));
+  return retrieve_rank(queries, n_queries, dim, table, n_items, norms, metric, target, ex, rank_out, error_flag,
+                       workspace, workspace_bytes, st);
 }

@@ -167,6 +167,60 @@ __device__ __forceinline__ bool set_has(const SetView& v, const int* s_ids, int 
   return lo < v.n && __ldg(v.g + lo) == id;
 }
 
+// ---- Exact rank of a row's target: the number of eligible items that the row's top-k would put before it ----------
+// A rank pass counts every id j != t of a column block whose (key, id) beats the target's, then subtracts the excluded
+// ones: the distinct ids of the row's segment inside the block that beat it, t itself never (a target is not
+// excluded).  A sorted segment is cut to the block by two binary searches, so exclusion costs one read per excluded id
+// of the block, not a search per beating item.
+
+// first index of segment ids[0, n) holding an id >= x
+__device__ __forceinline__ long long seg_lower_bound(const long long* ids, long long n, long long x) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (__ldg(ids + mid) < x) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// Called by every thread of the CTA: this thread's share of the excluded ids of row r inside [id_lo, id_hi) that beat
+// (kt, t); key_at(id) is the key of an id of the block.  A repeated id counts once; an id outside the block (only in a
+// malformed table, which the call's check kernel reports) is skipped, so no read leaves the block.
+template <class KeyAt>
+__device__ int excluded_beaters(const ItemSets& s, long long r, long long id_lo, long long id_hi, float kt, int t,
+                                KeyAt key_at, long long* s_range) {
+  if (threadIdx.x == 0) {
+    long long lo, hi;
+    set_segment(s, r, lo, hi);
+    s_range[0] = lo;
+    s_range[1] = lo + seg_lower_bound(s.ids + lo, hi - lo, id_lo);
+    s_range[2] = lo + seg_lower_bound(s.ids + lo, hi - lo, id_hi);
+  }
+  __syncthreads();
+  const long long first = s_range[0], a = s_range[1], b = s_range[2];
+  int c = 0;
+  for (long long e = a + threadIdx.x; e < b; e += blockDim.x) {
+    const long long x = __ldg(s.ids + e);
+    if (x < id_lo || x >= id_hi || x == t || (e > first && __ldg(s.ids + e - 1) == x)) continue;
+    if (better(key_at(x), (int)x, kt, t)) ++c;
+  }
+  __syncthreads();                                          // s_range is rewritten for the next row
+  return c;
+}
+
+// One thread per row: *flag |= 1 for a target outside [0, items)
+static __global__ void rank_target_check_kernel(const long long* __restrict__ target, long long n, long long items,
+                                                int* flag) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n && (target[r] < 0 || target[r] >= items)) atomicOr(flag, 1);
+}
+
+static inline int rank_target_check(const long long* target, int64_t n, int64_t items, int* flag, cudaStream_t st) {
+  rank_target_check_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(target, n, items, flag);
+  RECNN_CHECK_LAUNCH("rank_target_check_kernel");
+  return RECNN_OK;
+}
+
 // One warp per row of the call: *flag |= 4 for a row_set outside [-1, n_sets), offsets out of [0, total] or
 // decreasing, or a descending pair in the row's segment; |= 1 for an id outside [0, items).  Only the segments the rows
 // reference are read.

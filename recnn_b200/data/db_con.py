@@ -118,6 +118,63 @@ class ItemIndex:
                              "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
         return SearchResult(ids, dist)
 
+    def rank(self, search_vecs, target, exclude=None, exclude_rows=None):
+        """int64 [n]: for offline evaluation, the number of items ``search`` on the same queries would return before
+        ``target[q]`` (better key, equal keys the smaller id), i.e. the target's position in ``search(vecs, k)`` when
+        below k and the target is absent otherwise, at any k.  ``exclude`` / ``exclude_rows`` as in ``search``; a
+        query's target is never excluded.  DDPG / TD3: ``index.rank(actor(state), target, ...)``.  A target or
+        excluded id outside [0, n_items) raises IndexError, a malformed table ValueError."""
+        from .item_sets import ItemSets, row_map
+        q = torch.as_tensor(search_vecs)
+        if q.dim() == 1:
+            q = q.unsqueeze(0)
+        if q.dim() != 2 or q.shape[1] != self.dim:
+            raise ValueError("search_vecs must be [n, %d]" % self.dim)
+        n = int(q.shape[0])
+        if (not torch.is_tensor(target) or target.dim() != 1 or target.shape[0] != n
+                or target.dtype.is_floating_point or target.dtype.is_complex or target.dtype == torch.bool):
+            raise ValueError("target must be an integer tensor [n] with n = %d queries (got %s)"
+                             % (n, "%s %s" % (tuple(target.shape), target.dtype) if torch.is_tensor(target)
+                                else type(target).__name__))
+        sets = rows = None
+        if exclude is not None:
+            if not isinstance(exclude, ItemSets):
+                raise ValueError("exclude must be a recnn_b200.data.ItemSets (got %s)" % type(exclude).__name__)
+            sets, rows = row_map(exclude, exclude_rows, n)
+        elif exclude_rows is not None:
+            raise ValueError("exclude_rows maps queries to the sets of an ItemSets exclude")
+        q = q.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        rank = torch.empty(n, dtype=torch.int64, device=self.device)
+        if n == 0:
+            return rank
+        target = target.detach().to(device=self.device, dtype=torch.int64).contiguous()
+        L = _lib.lib()
+        need = L.recnn_retrieve_rank_workspace_bytes(n, self.n_items)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        args = (q.data_ptr(), n, self.dim, self.table.data_ptr(), self.n_items, _lib.ptr(self.norms), self.metric,
+                target.data_ptr())
+        flag = torch.empty(1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            if sets is None:
+                _lib.check(L.recnn_retrieve_rank(*args, rank.data_ptr(), flag.data_ptr(), self._ws.data_ptr(),
+                                                 self._ws.numel(), _lib.stream_ptr(self.device)))
+            else:
+                sets = sets.to(self.device)
+                rows = None if rows is None else rows.to(self.device).contiguous()
+                _lib.check(L.recnn_retrieve_rank_sets(*args, sets.ids.data_ptr() if sets.ids.numel() else None,
+                                                      sets.ids.numel(), sets.offsets.data_ptr(), len(sets),
+                                                      _lib.ptr(rows), rank.data_ptr(), flag.data_ptr(),
+                                                      self._ws.data_ptr(), self._ws.numel(),
+                                                      _lib.stream_ptr(self.device)))
+        bits = int(flag.item())
+        if bits & 1:
+            raise IndexError("a target or excluded item id is out of range for the index's %d items" % self.n_items)
+        if bits & 4:
+            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
+        return rank
+
 
 class MilvusConnection(ItemIndex):
     """Constructor shape of recnn.data.db_con.MilvusConnection(env, name=..., port=..., param=...): the collection

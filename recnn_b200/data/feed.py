@@ -75,6 +75,16 @@ class HistoryCSR:
                              % self.frame_size)
         return pos
 
+    def holdout_windows(self, pos):
+        """int64 [U]: the id of each user's last window (the leave-last-out row: its action is the user's last item),
+        in the collate's window order over all users.  A user without a window (fewer than F + 1 items) raises
+        ValueError."""
+        pos = self.check_positions(pos)
+        if (self.win_counts[pos] == 0).any():
+            raise ValueError("user(s) with fewer than frame_size + 1 = %d interactions have no held-out item"
+                             % (self.frame_size + 1))
+        return self.win_offsets[pos + 1] - 1
+
     def plan_users(self, pos):
         """row_offsets int64[B+1] (exclusive prefix sum of len - F over the batch's users) and N."""
         pos = self.check_positions(pos)
@@ -268,6 +278,20 @@ class DeviceFrameFeed:
         if int(err.item()) != 0:
             raise IndexError("user_states: a user position or history item outside the resident histories")
         return out
+
+    def holdout(self, user_positions):
+        """The leave-last-out evaluation rows of the given users: ``state`` fp32 [U, F*D + F], the state of each
+        user's last window (bit for bit ``embed(windows(last))["state"]``); ``target`` int64 [U], that window's last
+        item (the user's last rated item); ``exclude_rows`` int64 [U], the user positions, the rows of
+        ``seen_items()``.  ``policy.rank(h["state"], h["target"], exclude=feed.seen_items(),
+        exclude_rows=h["exclude_rows"])`` ranks each held-out item among the items the user has not rated before (the
+        target itself is never excluded).  A user with fewer than F + 1 items raises ValueError."""
+        last = self.csr.holdout_windows(user_positions)
+        pos = np.array(user_positions, dtype=np.int64).reshape(-1)
+        batch = self.windows(torch.from_numpy(last))
+        state = self.embed(batch)["state"]
+        return {"state": state, "target": batch["items"][:, self.frame_size].contiguous(),
+                "exclude_rows": torch.from_numpy(pos).to(self.device), "window_ids": batch["window_ids"]}
 
     def seen_items(self):
         """``ItemSets`` with one set per user position of the CSR: the distinct items of that user's history,

@@ -264,6 +264,99 @@ class DiscreteActor(nn.Module):
                              "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
         return values, ids
 
+    def rank(self, state, target, exclude=None, exclude_rows=None):
+        """``(rank, log_prob)`` of each row's target item, for offline evaluation: ``rank`` int64 [N] is the number of
+        items ``topk`` on the same rows would put before ``target[r]`` (higher logit, equal logits the smaller id), so
+        it is ``target``'s position in ``topk(state, k)`` when below k and the target is absent otherwise, at any k;
+        ``log_prob`` fp32 [N] is log pi(target | state).  ``exclude``: a ``recnn_b200.data.ItemSets`` of ids that do
+        not count (e.g. ``DeviceFrameFeed.seen_items()``), with ``exclude_rows`` as in ``topk``; a row's target is
+        never excluded.  A target or excluded id outside [0, num_items) raises IndexError, a malformed table
+        ValueError.  Never forms the [N, num_items] probabilities; on a vocabulary-parallel policy it ranks over the
+        whole vocabulary (two all-gathers of O(N) records), on a data-parallel replica it stays local.  Inference
+        only: nothing saved for the policy update is touched."""
+        from .update.reinforce import _chunk_items
+        from ..data.item_sets import ItemSets, row_map
+        vp = self.__dict__.get("_recnn_vp")
+        d = self.dims
+        items = d.num_items if vp is None else vp.num_items
+        if not torch.is_tensor(state) or state.dim() != 2 or state.shape[1] != d.state_dim:
+            raise ValueError("state must be a [N, %d] tensor" % d.state_dim)
+        n = state.shape[0]
+        if (not torch.is_tensor(target) or target.dim() != 1 or target.shape[0] != n
+                or target.dtype.is_floating_point or target.dtype.is_complex or target.dtype == torch.bool):
+            raise ValueError("target must be an integer tensor [N] with N = %d rows (got %s)"
+                             % (n, "%s %s" % (tuple(target.shape), target.dtype) if torch.is_tensor(target)
+                                else type(target).__name__))
+        sets = rows = None
+        if isinstance(exclude, ItemSets):
+            sets, rows = row_map(exclude, exclude_rows, n)
+        elif exclude is not None:
+            raise ValueError("exclude must be a recnn_b200.data.ItemSets (got %s)" % type(exclude).__name__)
+        elif exclude_rows is not None:
+            raise ValueError("exclude_rows maps rows to the sets of an ItemSets exclude")
+        dev = self.linear1.weight.device
+        if dev.type != "cuda":
+            raise _lib.RecnnError("recnn_b200 nets run on CUDA only (module is on %s); call .cuda() first" % dev)
+        rank = torch.empty(n, device=dev, dtype=torch.int64)
+        logp = torch.empty(n, device=dev, dtype=torch.float32)
+        if n == 0:
+            return rank, logp
+        _, (state,) = _device_check(self, state)
+        target = target.detach().to(device=dev, dtype=torch.int64).contiguous()
+        table = ()
+        if sets is not None:
+            sets = sets.to(dev)
+            rows = None if rows is None else rows.to(dev).contiguous()
+            table = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
+                     len(sets), _lib.ptr(rows))
+        L = _lib.lib()
+        flat = param_arena(self)
+        chunk = _chunk_items(n, d.num_items)
+        nbytes = L.recnn_discrete_rank_workspace_bytes(d, n, chunk)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        flag = torch.zeros(2, dtype=torch.int32, device=dev)       # the call's bits, the table check's (sharded)
+        st = _lib.stream_ptr(dev)
+        with torch.cuda.device(dev):
+            if vp is None and sets is None:
+                _lib.check(L.recnn_discrete_rank(d, flat.data_ptr(), state.data_ptr(), target.data_ptr(), n, chunk,
+                                                 rank.data_ptr(), logp.data_ptr(), flag.data_ptr(), ws.data_ptr(),
+                                                 nbytes, st))
+            elif vp is None:
+                _lib.check(L.recnn_discrete_rank_sets(d, flat.data_ptr(), state.data_ptr(), target.data_ptr(), n,
+                                                      *table, chunk, rank.data_ptr(), logp.data_ptr(),
+                                                      flag.data_ptr(), ws.data_ptr(), nbytes, st))
+            else:
+                shard = vp.shard()
+                stats = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+                _lib.check(L.recnn_discrete_shard_rank_stats(d, shard, flat.data_ptr(), state.data_ptr(),
+                                                             target.data_ptr(), n, chunk, stats.data_ptr(),
+                                                             ws.data_ptr(), nbytes, st))
+                g_stats = vp.all_gather(stats)
+                counts = torch.empty(L.recnn_vocab_rank_record_floats(n), device=dev, dtype=torch.float32)
+                if sets is None:
+                    _lib.check(L.recnn_discrete_shard_rank(d, shard, flat.data_ptr(), target.data_ptr(), n, chunk,
+                                                           g_stats.data_ptr(), counts.data_ptr(), ws.data_ptr(),
+                                                           nbytes, st))
+                else:
+                    _lib.check(L.recnn_discrete_shard_rank_sets(d, shard, flat.data_ptr(), target.data_ptr(), n,
+                                                                *table, chunk, g_stats.data_ptr(), counts.data_ptr(),
+                                                                flag[1:].data_ptr(), ws.data_ptr(), nbytes, st))
+                del ws
+                g_counts = vp.all_gather(counts)
+                _lib.check(L.recnn_discrete_shard_rank_finish(d, shard, g_stats.data_ptr(), g_counts.data_ptr(),
+                                                              target.data_ptr(), n, rank.data_ptr(), logp.data_ptr(),
+                                                              flag.data_ptr(), st))
+        f = flag.tolist()
+        bits = f[0] | f[1]
+        if bits & 2:
+            raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+        if bits & 1:
+            raise IndexError("a target or excluded item id is out of range for the policy's %d items" % items)
+        if bits & 4:
+            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
+        return rank, logp
+
     def gc(self):
         del self.rewards[:]
         del self.saved_log_probs[:]

@@ -1,2 +1,2 @@
-from . import misc
+from . import metrics, misc
 from .misc import soft_update, write_losses, DummyWriter
