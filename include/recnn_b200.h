@@ -540,6 +540,54 @@ RECNN_API int recnn_discrete_shard_topk_sets(const recnn_discrete_dims* d, const
                                              int64_t n_sets, const int64_t* row_set, int32_t chunk_items,
                                              float* record, int32_t* error_flag, void* workspace,
                                              int64_t workspace_bytes, void* stream);
+/* ---- REINFORCE: serving slates sampled from the policy ---------------------------------------------
+ * Replaces the Categorical(probs) / torch.multinomial draw of recnn/nn/models.py:107-110, applied to a slate: k items
+ * per row drawn without replacement from pi = softmax(z) with the excluded ids' probabilities set to 0, i.e.
+ * torch.multinomial(pi, k, replacement=False), without the [n_rows, num_items] probabilities.  It is the top-k pass
+ * ranking by z + G instead of z (Gumbel-top-k): G = -log(-log u) per (row, item), u = (2 m + 1) 2^-24 with m the top 23
+ * bits of word x of Philox4x32-10 keyed by seed at counter (item id, (row_offset + r) << 8 | 0x67).  Slot 0 is the first
+ * draw.  The ids are thus a function of (seed, global row, item, logit) alone: not of the chunking, the world size or
+ * the batch.  values_out fp32 [n_rows, k] = pi(id) over ALL items (excluded ones stay in S, as in topk), from the
+ * winner's logit recomputed as a dot product of length hidden (fp32, summed in another order than the GEMM);
+ * ids_out int64 [n_rows, k]; a row with fewer than k eligible items ends in id -1, value 0.  exclude / set tables,
+ * *error_flag bits, k range and workspace (recnn_discrete_topk_workspace_bytes) exactly as recnn_discrete_topk(_sets);
+ * 0 <= row_offset and row_offset + n_rows <= 2^55.  Deterministic: the same seed gives the same bits. */
+RECNN_API int recnn_discrete_sample_topk(const recnn_discrete_dims* d, const float* params, const float* state,
+                                         int64_t n_rows, int32_t k, const int64_t* exclude, int32_t n_exclude,
+                                         uint64_t seed, int64_t row_offset, int32_t chunk_items, float* values_out,
+                                         int64_t* ids_out, int32_t* error_flag, void* workspace,
+                                         int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_sample_topk_sets(const recnn_discrete_dims* d, const float* params, const float* state,
+                                              int64_t n_rows, int32_t k, const int64_t* set_ids, int64_t n_set_ids,
+                                              const int64_t* set_offsets, int64_t n_sets, const int64_t* row_set,
+                                              uint64_t seed, int64_t row_offset, int32_t chunk_items,
+                                              float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                              void* workspace, int64_t workspace_bytes, void* stream);
+/* The same on a vocabulary-sharded policy, as recnn_discrete_shard_topk(_sets) + recnn_discrete_shard_topk_finish.
+ * A rank's record of recnn_vocab_sample_topk_record_floats(n_rows, k) floats: the header, the local max and sum-of-exp
+ * planes, k planes of perturbed keys -(z + G) (empty: FLT_MAX), k logit planes, k id planes (int32 bits, empty -1),
+ * then the seed as two int32 words.  shard_sample_topk_finish merges M and S in rank order and k-way merges the W key
+ * lists: every rank writes the same bits, and at world 1 the pair computes exactly what recnn_discrete_sample_topk
+ * does.  It takes the rank's own seed: *error_flag bit 2 when the headers do not tile the vocabulary in rank order with
+ * this rank's block or any record's seed differs from it (so every rank of a disagreeing set raises). */
+RECNN_API int64_t recnn_vocab_sample_topk_record_floats(int64_t n_rows, int32_t k);
+RECNN_API int recnn_discrete_shard_sample_topk(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                               const float* params, const float* state, int64_t n_rows, int32_t k,
+                                               const int64_t* exclude, int32_t n_exclude, uint64_t seed,
+                                               int64_t row_offset, int32_t chunk_items, float* record,
+                                               void* workspace, int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_sample_topk_sets(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                    const float* params, const float* state, int64_t n_rows,
+                                                    int32_t k, const int64_t* set_ids, int64_t n_set_ids,
+                                                    const int64_t* set_offsets, int64_t n_sets,
+                                                    const int64_t* row_set, uint64_t seed, int64_t row_offset,
+                                                    int32_t chunk_items, float* record, int32_t* error_flag,
+                                                    void* workspace, int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_discrete_shard_sample_topk_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                      const float* gathered, int64_t n_rows, int32_t k,
+                                                      const int64_t* exclude, int32_t n_exclude, uint64_t seed,
+                                                      float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                                      void* stream);
 /* Offline evaluation: the exact rank of each row's target item under the policy, rank_out int64 [n_rows] = the number
  * of items j that recnn_discrete_topk(_sets) with the same chunk_items would put before target[r]: j != target, j not in
  * the row's set (the target itself is never excluded) and logit_j > logit_t, equal logits to the smaller id, NaN and

@@ -205,6 +205,26 @@ SIGNATURES = {
                                                  C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
                                                  C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_int64, C.c_void_p]),
+    "recnn_discrete_sample_topk": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                             C.c_void_p, C.c_int32, C.c_uint64, C.c_int64, C.c_int32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_discrete_sample_topk_sets": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_int64,
+                                                  C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                                  C.c_uint64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_vocab_sample_topk_record_floats": (C.c_int64, [C.c_int64, C.c_int32]),
+    "recnn_discrete_shard_sample_topk": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                   C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32,
+                                                   C.c_uint64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p,
+                                                   C.c_int64, C.c_void_p]),
+    "recnn_discrete_shard_sample_topk_sets": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                        C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64,
+                                                        C.c_void_p, C.c_int64, C.c_void_p, C.c_uint64, C.c_int64,
+                                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                                        C.c_void_p]),
+    "recnn_discrete_shard_sample_topk_finish": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
+                                                          C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_uint64,
+                                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_discrete_rank_workspace_bytes": (C.c_int64, [C.POINTER(DiscreteDims), C.c_int64, C.c_int32]),
     "recnn_discrete_rank": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,

@@ -622,14 +622,52 @@ __global__ void cand_fill_kernel(Cand* __restrict__ c, long long count) {
   if (i < count) c[i] = Cand{FLT_MAX, kNoId};
 }
 
+// ---- The key a select pass ranks items by (smaller first).  LogitKey: -z, the top-k.  GumbelKey: -(z + G) with G a
+// standard Gumbel variate per (row, item); the best k of z + G are k draws without replacement from softmax(z), in
+// draw order (Gumbel-top-k, a Plackett-Luce draw), so sampling is the top-k pass with this key.
+struct LogitKey {
+  static constexpr bool kPruned = false;
+  __device__ __forceinline__ float operator()(float z, long long, int) const { return logit_key(z); }
+};
+
+// G = -log(-log u) with u from Philox(seed) at counter (item id, global row << 8 | kGumbelTag); the tag is used by no
+// other draw of the library (dropout / TD3 noise: streams 0..15, Categorical draws: 0x5a), and a row below 2^55 keeps
+// the row bits clear of the tag.  u = (2 m + 1) 2^-24 with m the top 23 bits of word x: exact in fp32 and strictly
+// inside (0, 1) -- the 24-bit (x >> 8) + 0.5 would round to 1 in fp32 at its largest value.
+constexpr unsigned kGumbelTag = 0x67u;
+constexpr long long kMaxSampleRow = 1LL << 55;
+__device__ __forceinline__ float gumbel_noise(unsigned long long seed, long long row, int id) {
+  const uint4 q = Philox(seed)((unsigned long long)id, ((unsigned long long)row << 8) | kGumbelTag);
+  const float u = (float)(2u * (q.x >> 9) + 1u) * 5.9604644775390625e-08f;
+  return -logf(-logf(u));
+}
+
+// The bound that lets the select pass skip the Philox call and the two logs.  u <= 1 - 2^-24, so -log u >=
+// 2^-24 (1 + 2^-25) and G <= -log(2^-24) = 24 ln 2 = 16.6355 in exact arithmetic; logf is within 2 ulp, which moves
+// -log u by a relative 2.4e-7 and G by as much absolutely, so 16.75 bounds every fp32 G.  With G <= kGumbelMax,
+// z + G <= z + kGumbelMax, and fp32 rounding is monotone, so key(z) >= bound(z) for the same id: an item whose bound
+// does not beat the thread's k-th and the row's running k-th cannot enter with its real key either, and skipping it
+// changes no result.
+constexpr float kGumbelMax = 16.75f;
+struct GumbelKey {
+  static constexpr bool kPruned = true;
+  unsigned long long seed;
+  long long row0;               // the global row of the call's row 0
+  __device__ __forceinline__ float bound(float z) const { return fminf(-(z + kGumbelMax), FLT_MAX); }
+  __device__ __forceinline__ float operator()(float z, long long r, int id) const {
+    return fminf(-(z + gumbel_noise(seed, row0 + r, id)), FLT_MAX);     // NaN and -inf logits last, as logit_key
+  }
+};
+
 // grid (splits, rows): the best k of columns [lo, hi) of one row of a chunk's logits z [n, w] (ids id0 + j) that beat
 // the row's running k-th best, ascending, into part [n, splits, k] (empty slots: {FLT_MAX, kNoId}).  A candidate is
 // tested against the row's excluded set (global ids, topk.cuh) only once it beats its thread's list and the running k-th
-// (SETS; without, nothing is staged).
-template <int KMAX, bool SETS>
+// (SETS; without, nothing is staged).  Key: the ranking key of a logit (LogitKey, GumbelKey); it is the last parameter,
+// so the top-k's instantiations keep their parameter offsets.
+template <int KMAX, bool SETS, class Key>
 __global__ void __launch_bounds__(kTopkThreads)
 policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int id0, int k, ItemSets ex, int stage_cap,
-                          const Cand* __restrict__ run, Cand* __restrict__ part) {
+                          const Cand* __restrict__ run, Cand* __restrict__ part, Key key_of) {
   __shared__ float s_key[32];
   __shared__ int s_id[32], s_owner[32];
   extern __shared__ int s_set[];
@@ -648,8 +686,12 @@ policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int i
     list_clear(keys, ids);
     const float* row = z + r * w;
     for (int j = lo + threadIdx.x; j < hi; j += blockDim.x) {
-      const float key = logit_key(row[j]);
       const int id = id0 + j;
+      if constexpr (Key::kPruned) {
+        const float best = key_of.bound(row[j]);
+        if (!better(best, id, keys[KMAX - 1], ids[KMAX - 1]) || !better(best, id, bar.key, bar.id)) continue;
+      }
+      const float key = key_of(row[j], r, id);
       if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && better(key, id, bar.key, bar.id) &&
           (!SETS || set.n == 0 || !set_has(set, s_set, id)))
         list_insert(keys, ids, key, id);
@@ -769,6 +811,116 @@ policy_topk_shard_finish_kernel(const float* __restrict__ g, long long n, int k,
   }
 }
 
+// ---- Sampled slates (serving): the select pass with GumbelKey.  Its lists hold perturbed keys, so a winner's value
+// needs its logit again: one warp per (row, slot) recomputes z = W2[id] . h + b2[id] from the hidden layer the pass left
+// in the workspace (k dot products of length H per row, in a fixed lane order).  It is fp32 like the GEMM's logit but
+// summed in another order, so a value differs from forward()'s by that reordering only.
+__device__ __forceinline__ float item_logit(const float* __restrict__ h, const float* __restrict__ w2, int ld2,
+                                            const float* __restrict__ b2, int H, int local) {
+  const float* wr = w2 + (long long)local * ld2;
+  float acc = 0.f;
+  for (int c = threadIdx.x & 31; c < H; c += 32) acc = fmaf(h[c], wr[c], acc);
+  return warp_sum(acc) + b2[local];
+}
+
+// ids (-1 for an empty slot) and pi = exp(z - M) / S of the final lists of an unsharded call
+__global__ void __launch_bounds__(128)
+policy_sample_finish_kernel(const Cand* __restrict__ run, long long n, int k, const float* __restrict__ h, int H,
+                            const float* __restrict__ w2, int ld2, const float* __restrict__ b2,
+                            const float* __restrict__ run_max, const float* __restrict__ run_sum,
+                            float* __restrict__ values, long long* __restrict__ ids) {
+  const long long i = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= n * k) return;
+  const long long r = i / k;
+  const Cand c = run[i];
+  if (c.id == kNoId) {
+    if ((threadIdx.x & 31) == 0) { ids[i] = -1; values[i] = 0.f; }
+    return;
+  }
+  const float zc = item_logit(h + r * H, w2, ld2, b2, H, c.id);
+  if ((threadIdx.x & 31) == 0) {
+    ids[i] = c.id;
+    values[i] = expf(zc - run_max[r]) / run_sum[r];
+  }
+}
+
+// A rank's sample record: the header {lo, hi, num_items, n_rows}, the m and s planes (written by the passes), k key
+// planes (the perturbed keys -(z + G), an empty slot FLT_MAX), k logit planes, k id planes (int32 bits, empty -1), then
+// the seed as two int32 words (low, high), so that the finish can refuse ranks that drew different noise.
+__host__ __device__ __forceinline__ int64_t sample_record_floats(int64_t n, int k) {
+  return kShardHeader + (2 + 3 * (int64_t)k) * n + 2;
+}
+
+__global__ void __launch_bounds__(128)
+policy_sample_record_kernel(const Cand* __restrict__ run, long long n, int k, const float* __restrict__ h, int H,
+                            const float* __restrict__ w2, int ld2, const float* __restrict__ b2, ShardPlan p,
+                            unsigned long long seed, float* __restrict__ rec) {
+  const long long i = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (i == 0 && lane == 0) {
+    shard_header_write(rec, p, n);
+    int* s = reinterpret_cast<int*>(rec + sample_record_floats(n, k) - 2);
+    s[0] = (int)(unsigned)seed;
+    s[1] = (int)(unsigned)(seed >> 32);
+  }
+  if (i >= n * k) return;
+  const long long r = i / k, j = i % k;
+  const Cand c = run[i];
+  float* planes = shard_plane(rec, n, 2);
+  const float zc = c.id == kNoId ? 0.f : item_logit(h + r * H, w2, ld2, b2, H, c.id - p.lo);
+  if (lane == 0) {
+    planes[j * n + r] = c.key;
+    planes[(k + j) * n + r] = zc;
+    planes[(2 * k + j) * n + r] = __int_as_float(c.id == kNoId ? -1 : c.id);
+  }
+}
+
+// gathered sample records -> every rank's (values, ids): M and S merged in rank order (shard_merge_stats), a k-way merge
+// of the W sorted key lists, the value from the winner's logit.  One warp per row, lane q reads rank q's list (W <= 32).
+// *flag |= 2 when the headers do not tile the vocabulary with this rank's block or a record's seed is not `seed`.
+__global__ void __launch_bounds__(128)
+policy_sample_shard_finish_kernel(const float* __restrict__ g, long long n, int k, ShardPlan p,
+                                  unsigned long long seed, float* __restrict__ values, long long* __restrict__ ids,
+                                  int* flag) {
+  const long long stride = sample_record_floats(n, k);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    bool bad = shard_plan_bad(g, stride, p, n);
+    for (int q = 0; q < p.world; ++q) {
+      const int* s = reinterpret_cast<const int*>(g + q * stride + stride - 2);
+      bad = bad || (unsigned)s[0] != (unsigned)seed || (unsigned)s[1] != (unsigned)(seed >> 32);
+    }
+    if (bad) atomicOr(flag, 2);
+  }
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const int W = p.world;
+  float M, S;
+  shard_merge_stats(g, stride, W, n, r, M, S);
+  const float* planes = shard_plane(g, n, 2, lane < W ? lane : 0, stride);
+  int head = 0;
+  for (int i = 0; i < k; ++i) {
+    float key = FLT_MAX, zc = 0.f;
+    int id = kNoId, owner = lane;
+    if (lane < W && head < k) {
+      const int v = __float_as_int(planes[(2 * k + head) * n + r]);
+      if (v >= 0) {
+        key = planes[head * n + r];
+        zc = planes[(k + head) * n + r];
+        id = v;
+      }
+    }
+    warp_argmin(key, id, owner);
+    zc = __shfl_sync(0xffffffffu, zc, owner);
+    if (lane == owner) ++head;
+    if (lane == 0) {
+      const bool none = id == kNoId;
+      ids[r * k + i] = none ? -1 : id;
+      values[r * k + i] = none ? 0.f : expf(zc - M) / S;
+    }
+  }
+}
+
 struct TopkWorkspace {
   DiscreteScratch s;           // img, h and z ([n, chunk]) for discrete_hidden / discrete_logits
   float *run_max, *run_sum;
@@ -793,16 +945,17 @@ static TopkWorkspace topk_carve(const recnn_discrete_dims& d, int64_t n, int k, 
   return w;
 }
 
-// The hidden layer, then every chunk: logits, row statistics into (run_max, run_sum), selection and merge.  Candidate
-// ids are id0 + the local item.  Returns the final lists.
+// The hidden layer, then every chunk: logits, row statistics into (run_max, run_sum), selection by key_of's key and
+// merge.  Candidate ids are id0 + the local item.  Returns the final lists; the hidden layer stays in w.s.h.
+template <class Key>
 static int policy_topk_pass(const recnn_discrete_dims& d, const float* params, const float* state, int64_t n, int k,
                             const ItemSets& ex, int chunk, int id0, const TopkWorkspace& w, float* run_max,
-                            float* run_sum, const Cand** lists, cudaStream_t st) {
+                            float* run_sum, const Cand** lists, cudaStream_t st, Key key_of = Key()) {
   const int I = d.num_items;
   // the dense form stages its E ids, a table up to kSetStage
   const int cap = !ex.ids ? 0 : (ex.offsets ? kSetStage : ex.stride), stage = cap * (int)sizeof(int);
-  auto select = k <= 16 ? (cap ? policy_topk_select_kernel<16, true> : policy_topk_select_kernel<16, false>)
-                        : (cap ? policy_topk_select_kernel<64, true> : policy_topk_select_kernel<64, false>);
+  auto select = k <= 16 ? (cap ? policy_topk_select_kernel<16, true, Key> : policy_topk_select_kernel<16, false, Key>)
+                        : (cap ? policy_topk_select_kernel<64, true, Key> : policy_topk_select_kernel<64, false, Key>);
   RECNN_PROPAGATE(discrete_hidden(d, params, state, n, w.s, st, nullptr));
   cand_fill_kernel<<<(unsigned)ceil_div(n * k, 256), 256, 0, st>>>(w.list[0], n * k);
   RECNN_CHECK_LAUNCH("cand_fill_kernel");
@@ -815,7 +968,7 @@ static int policy_topk_pass(const recnn_discrete_dims& d, const float* params, c
     RECNN_CHECK_LAUNCH("logit_stats_kernel");
     const int splits = topk_splits(n, cw, kTopkSplitCap);
     const dim3 grid((unsigned)splits, (unsigned)(n < 65535 ? n : 65535));
-    select<<<grid, kTopkThreads, stage, st>>>(w.s.z, n, cw, id0 + c0, k, ex, cap, w.list[cur], w.part);
+    select<<<grid, kTopkThreads, stage, st>>>(w.s.z, n, cw, id0 + c0, k, ex, cap, w.list[cur], w.part, key_of);
     RECNN_CHECK_LAUNCH("policy_topk_select_kernel");
     policy_topk_merge_kernel<<<(unsigned)ceil_div(n, 4), 128, 0, st>>>(w.list[cur], w.part, splits, k, n,
                                                                        w.list[cur ^ 1]);
@@ -1265,8 +1418,8 @@ static int topk_local(const recnn_discrete_dims& d, const float* params, const f
                       const ItemSets& sets, int chunk_items, float* values_out, int64_t* ids_out,
                       const TopkWorkspace& w, cudaStream_t st) {
   const Cand* lists;
-  RECNN_PROPAGATE(policy_topk_pass(d, params, state, n_rows, k, sets, chunk_items, 0, w, w.run_max, w.run_sum, &lists,
-                                   st));
+  RECNN_PROPAGATE(policy_topk_pass<LogitKey>(d, params, state, n_rows, k, sets, chunk_items, 0, w, w.run_max,
+                                             w.run_sum, &lists, st));
   policy_topk_finish_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(
       lists, n_rows, k, w.run_max, w.run_sum, values_out, reinterpret_cast<long long*>(ids_out));
   RECNN_CHECK_LAUNCH("policy_topk_finish_kernel");
@@ -1316,7 +1469,7 @@ static int topk_shard_local(const recnn_discrete_dims& d, const ShardPlan& p, co
                             int64_t n_rows, int k, const ItemSets& sets, int chunk_items, float* record,
                             const TopkWorkspace& w, cudaStream_t st) {
   const Cand* lists;
-  RECNN_PROPAGATE(policy_topk_pass(d, params, state, n_rows, k, sets, chunk_items, p.lo, w,
+  RECNN_PROPAGATE(policy_topk_pass<LogitKey>(d, params, state, n_rows, k, sets, chunk_items, p.lo, w,
                                    shard_plane(record, n_rows, 0), shard_plane(record, n_rows, 1), &lists, st));
   policy_topk_record_kernel<<<(unsigned)ceil_div(n_rows * k, 256), 256, 0, st>>>(lists, n_rows, k, p, record);
   RECNN_CHECK_LAUNCH("policy_topk_record_kernel");
@@ -1375,6 +1528,145 @@ extern "C" int recnn_discrete_shard_topk_finish(const recnn_discrete_dims* d, co
   policy_topk_shard_finish_kernel<<<(unsigned)ceil_div(n_rows, 4), 128, 0, st>>>(
       gathered, n_rows, k, p, values_out, reinterpret_cast<long long*>(ids_out), error_flag);
   RECNN_CHECK_LAUNCH("policy_topk_shard_finish_kernel");
+  return RECNN_OK;
+}
+
+// ---- the policy's sampled slates: topk's checks, workspace and passes with GumbelKey -----------------------------
+static int sample_rows_check(int64_t n_rows, int64_t row_offset) {
+  RECNN_REQUIRE(row_offset >= 0 && row_offset <= kMaxSampleRow - n_rows, "0 <= row_offset <= 2^55 - n_rows");
+  return RECNN_OK;
+}
+
+// the passes and the finish of an unsharded call
+static int sample_local(const recnn_discrete_dims& d, const float* params, const float* state, int64_t n_rows, int k,
+                        const ItemSets& sets, uint64_t seed, int64_t row_offset, int chunk_items, float* values_out,
+                        int64_t* ids_out, const TopkWorkspace& w, cudaStream_t st) {
+  const DiscreteLayout l = discrete_layout(d);
+  const Cand* lists;
+  RECNN_PROPAGATE(policy_topk_pass(d, params, state, n_rows, k, sets, chunk_items, 0, w, w.run_max, w.run_sum, &lists,
+                                   st, GumbelKey{seed, row_offset}));
+  policy_sample_finish_kernel<<<(unsigned)ceil_div(n_rows * k, 4), 128, 0, st>>>(
+      lists, n_rows, k, w.s.h, d.hidden, params + l.w2, l.ld2, params + l.b2, w.run_max, w.run_sum, values_out,
+      reinterpret_cast<long long*>(ids_out));
+  RECNN_CHECK_LAUNCH("policy_sample_finish_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_sample_topk(const recnn_discrete_dims* d, const float* params, const float* state,
+                                          int64_t n_rows, int32_t k, const int64_t* exclude, int32_t n_exclude,
+                                          uint64_t seed, int64_t row_offset, int32_t chunk_items, float* values_out,
+                                          int64_t* ids_out, int32_t* error_flag, void* workspace,
+                                          int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(values_out && ids_out && error_flag, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, exclude, n_exclude, chunk_items, workspace, workspace_bytes));
+  RECNN_REQUIRE(k <= d->num_items, "k <= num_items");
+  RECNN_PROPAGATE(sample_rows_check(n_rows, row_offset));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* ex = reinterpret_cast<const long long*>(exclude);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(exclude_check(ex, n_rows, n_exclude, d->num_items, error_flag, st));
+  ItemSets sets;
+  RECNN_PROPAGATE(dense_sets(ex, n_rows, n_exclude, w, &sets, st));
+  return sample_local(*d, params, state, n_rows, k, sets, seed, row_offset, chunk_items, values_out, ids_out, w, st);
+}
+
+extern "C" int recnn_discrete_sample_topk_sets(const recnn_discrete_dims* d, const float* params, const float* state,
+                                               int64_t n_rows, int32_t k, const int64_t* set_ids, int64_t n_set_ids,
+                                               const int64_t* set_offsets, int64_t n_sets, const int64_t* row_set,
+                                               uint64_t seed, int64_t row_offset, int32_t chunk_items,
+                                               float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                               void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(values_out && ids_out, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, nullptr, 0, chunk_items, workspace, workspace_bytes));
+  RECNN_REQUIRE(k <= d->num_items, "k <= num_items");
+  RECNN_PROPAGATE(sample_rows_check(n_rows, row_offset));
+  ItemSets sets;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_rows, error_flag, &sets));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(item_sets_check(sets, n_rows, d->num_items, error_flag, st));
+  return sample_local(*d, params, state, n_rows, k, sets, seed, row_offset, chunk_items, values_out, ids_out, w, st);
+}
+
+extern "C" int64_t recnn_vocab_sample_topk_record_floats(int64_t n_rows, int32_t k) {
+  return n_rows > 0 && k >= 1 && k <= 64 ? sample_record_floats(n_rows, k) : 0;
+}
+
+// the passes over the rank's block and its record
+static int sample_shard_local(const recnn_discrete_dims& d, const ShardPlan& p, const float* params,
+                              const float* state, int64_t n_rows, int k, const ItemSets& sets, uint64_t seed,
+                              int64_t row_offset, int chunk_items, float* record, const TopkWorkspace& w,
+                              cudaStream_t st) {
+  const DiscreteLayout l = discrete_layout(d);
+  const Cand* lists;
+  RECNN_PROPAGATE(policy_topk_pass(d, params, state, n_rows, k, sets, chunk_items, p.lo, w,
+                                   shard_plane(record, n_rows, 0), shard_plane(record, n_rows, 1), &lists, st,
+                                   GumbelKey{seed, row_offset}));
+  policy_sample_record_kernel<<<(unsigned)ceil_div(n_rows * k, 4), 128, 0, st>>>(
+      lists, n_rows, k, w.s.h, d.hidden, params + l.w2, l.ld2, params + l.b2, p, seed, record);
+  RECNN_CHECK_LAUNCH("policy_sample_record_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_discrete_shard_sample_topk(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                const float* params, const float* state, int64_t n_rows, int32_t k,
+                                                const int64_t* exclude, int32_t n_exclude, uint64_t seed,
+                                                int64_t row_offset, int32_t chunk_items, float* record,
+                                                void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(record, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, exclude, n_exclude, chunk_items, workspace, workspace_bytes));
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(k <= p.items, "k <= num_items (the whole vocabulary)");
+  RECNN_PROPAGATE(sample_rows_check(n_rows, row_offset));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  ItemSets sets;
+  RECNN_PROPAGATE(dense_sets(reinterpret_cast<const long long*>(exclude), n_rows, n_exclude, w, &sets, st));
+  return sample_shard_local(*d, p, params, state, n_rows, k, sets, seed, row_offset, chunk_items, record, w, st);
+}
+
+extern "C" int recnn_discrete_shard_sample_topk_sets(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                     const float* params, const float* state, int64_t n_rows,
+                                                     int32_t k, const int64_t* set_ids, int64_t n_set_ids,
+                                                     const int64_t* set_offsets, int64_t n_sets,
+                                                     const int64_t* row_set, uint64_t seed, int64_t row_offset,
+                                                     int32_t chunk_items, float* record, int32_t* error_flag,
+                                                     void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(record, "null pointer");
+  RECNN_PROPAGATE(topk_check(d, params, state, n_rows, k, nullptr, 0, chunk_items, workspace, workspace_bytes));
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(k <= p.items, "k <= num_items (the whole vocabulary)");
+  RECNN_PROPAGATE(sample_rows_check(n_rows, row_offset));
+  ItemSets sets;
+  RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_rows, error_flag, &sets));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const TopkWorkspace w = topk_carve(*d, n_rows, k, chunk_items, workspace);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(item_sets_check(sets, n_rows, p.items, error_flag, st));   // global ids: every rank agrees
+  return sample_shard_local(*d, p, params, state, n_rows, k, sets, seed, row_offset, chunk_items, record, w, st);
+}
+
+extern "C" int recnn_discrete_shard_sample_topk_finish(const recnn_discrete_dims* d, const recnn_vocab_shard* v,
+                                                       const float* gathered, int64_t n_rows, int32_t k,
+                                                       const int64_t* exclude, int32_t n_exclude, uint64_t seed,
+                                                       float* values_out, int64_t* ids_out, int32_t* error_flag,
+                                                       void* stream) {
+  RECNN_REQUIRE(discrete_dims_ok(d) && gathered && values_out && ids_out && error_flag, "null pointer / dims");
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  RECNN_REQUIRE(p.world <= 32, "world <= 32");
+  RECNN_PROPAGATE(topk_rows_check(n_rows, k, exclude, n_exclude));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(exclude_check(reinterpret_cast<const long long*>(exclude), n_rows, n_exclude, p.items, error_flag,
+                                st));
+  policy_sample_shard_finish_kernel<<<(unsigned)ceil_div(n_rows, 4), 128, 0, st>>>(
+      gathered, n_rows, k, p, seed, values_out, reinterpret_cast<long long*>(ids_out), error_flag);
+  RECNN_CHECK_LAUNCH("policy_sample_shard_finish_kernel");
   return RECNN_OK;
 }
 

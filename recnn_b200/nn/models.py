@@ -8,6 +8,8 @@ calling it on CPU tensors raises.
 """
 from __future__ import annotations
 
+import types
+
 import torch
 import torch.nn as nn
 
@@ -118,7 +120,7 @@ class DiscreteActor(nn.Module):
       ``select_action`` return the rank's column block of the probabilities; draws and log-probs stay global.
     * After ``recnn_b200.dist.enable_data_parallel`` each rank holds a full replica and its own rows: ``select_action``
       / ``pi_beta_sample`` draw row r of the rank at the Philox counter of its global row; ``forward`` and ``topk``
-      stay local, with no exchange.
+      stay local, with no exchange; ``sample_topk`` keys row r by its global row (one all-gather of row counts).
     """
 
     def __init__(self, input_dim, action_dim, hidden_size, init_w=0):
@@ -174,18 +176,10 @@ class DiscreteActor(nn.Module):
             raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
         return out, gathered
 
-    def topk(self, state, k, exclude=None, exclude_rows=None):
-        """``(values, indices)`` as ``torch.topk(self(state), k)`` without forming the [N, num_items] probabilities:
-        the k items of highest logit per row (equal logits: the smaller id first), values fp32 [N, k] = pi(a|s),
-        indices int64 [N, k] global item ids, on a vocabulary-parallel policy too (one all-gather of k candidates per
-        row and rank).  ``exclude``: ids never returned, which stay in the softmax's normaliser (values are not
-        renormalised) -- either an integer tensor [N, E] (E <= 256, e.g. the frame's items; negative ids are padding)
-        or a ``recnn_b200.data.ItemSets`` table of any length (e.g. ``DeviceFrameFeed.seen_items()``: everything the
-        user has rated), with ``exclude_rows`` int64 [N] naming each row's set (-1: none; default row r -> set r).
-        An excluded id outside [0, num_items) raises IndexError, a malformed table ValueError.  A row with fewer than
-        k eligible items ends in id -1, value 0.  1 <= k <= min(64, num_items).  Inference only: nothing saved for
-        the policy update is touched."""
-        from .update.reinforce import _chunk_items
+    def _slate_args(self, state, k, exclude, exclude_rows):
+        """The argument handling of ``topk`` and ``sample_topk``: every refusal before any device work, then the
+        outputs and the device forms of the state and the exclusion.  A namespace of vp, d, items, n, dev, state,
+        values, ids, ex / n_ex (the dense form), sets / table (an ItemSets form, table: its C arguments)."""
         from ..data.item_sets import ItemSets, row_map
         vp = self.__dict__.get("_recnn_vp")
         d = self.dims
@@ -211,17 +205,50 @@ class DiscreteActor(nn.Module):
         dev = self.linear1.weight.device
         if dev.type != "cuda":
             raise _lib.RecnnError("recnn_b200 nets run on CUDA only (module is on %s); call .cuda() first" % dev)
-        values = torch.empty(n, k, device=dev, dtype=torch.float32)
-        ids = torch.empty(n, k, device=dev, dtype=torch.int64)
+        a = types.SimpleNamespace(vp=vp, d=d, items=items, n=n, dev=dev, n_ex=n_ex, ex=None, sets=None, table=None,
+                                  values=torch.empty(n, k, device=dev, dtype=torch.float32),
+                                  ids=torch.empty(n, k, device=dev, dtype=torch.int64))
         if n == 0:
-            return values, ids
-        _, (state,) = _device_check(self, state)
-        ex = None if n_ex == 0 else exclude.detach().to(device=dev, dtype=torch.int64).contiguous()
+            return a
+        _, (a.state,) = _device_check(self, state)
+        a.ex = None if n_ex == 0 else exclude.detach().to(device=dev, dtype=torch.int64).contiguous()
         if sets is not None:
-            sets = sets.to(dev)
+            a.sets = sets = sets.to(dev)
             rows = None if rows is None else rows.to(dev).contiguous()
-            table = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
-                     len(sets), _lib.ptr(rows))
+            a.table = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
+                       len(sets), _lib.ptr(rows))
+        return a
+
+    @staticmethod
+    def _slate_errors(flag, a):
+        """Raise what the error bits of a topk / sample_topk call (the call's word, the table check's) report."""
+        f = flag.tolist()
+        bits = f[0] | f[1]
+        if bits & 2:
+            raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+        if bits & 1:
+            raise IndexError("an excluded item id is out of range for the policy's %d items" % a.items)
+        if bits & 4:
+            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(a.sets))
+
+    def topk(self, state, k, exclude=None, exclude_rows=None):
+        """``(values, indices)`` as ``torch.topk(self(state), k)`` without forming the [N, num_items] probabilities:
+        the k items of highest logit per row (equal logits: the smaller id first), values fp32 [N, k] = pi(a|s),
+        indices int64 [N, k] global item ids, on a vocabulary-parallel policy too (one all-gather of k candidates per
+        row and rank).  ``exclude``: ids never returned, which stay in the softmax's normaliser (values are not
+        renormalised) -- either an integer tensor [N, E] (E <= 256, e.g. the frame's items; negative ids are padding)
+        or a ``recnn_b200.data.ItemSets`` table of any length (e.g. ``DeviceFrameFeed.seen_items()``: everything the
+        user has rated), with ``exclude_rows`` int64 [N] naming each row's set (-1: none; default row r -> set r).
+        An excluded id outside [0, num_items) raises IndexError, a malformed table ValueError.  A row with fewer than
+        k eligible items ends in id -1, value 0.  1 <= k <= min(64, num_items).  Inference only: nothing saved for
+        the policy update is touched."""
+        from .update.reinforce import _chunk_items
+        a = self._slate_args(state, k, exclude, exclude_rows)
+        if a.n == 0:
+            return a.values, a.ids
+        vp, d, n, dev, ex, n_ex = a.vp, a.d, a.n, a.dev, a.ex, a.n_ex
+        values, ids, table = a.values, a.ids, a.table
         L = _lib.lib()
         flat = param_arena(self)
         chunk = _chunk_items(n, d.num_items)
@@ -229,23 +256,23 @@ class DiscreteActor(nn.Module):
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
         flag = torch.zeros(2, dtype=torch.int32, device=dev)       # the call's bits, the table check's (sharded)
         with torch.cuda.device(dev):
-            if vp is None and sets is None:
-                _lib.check(L.recnn_discrete_topk(d, flat.data_ptr(), state.data_ptr(), n, k, _lib.ptr(ex), n_ex, chunk,
-                                                 values.data_ptr(), ids.data_ptr(), flag.data_ptr(), ws.data_ptr(),
-                                                 nbytes, _lib.stream_ptr(dev)))
+            if vp is None and table is None:
+                _lib.check(L.recnn_discrete_topk(d, flat.data_ptr(), a.state.data_ptr(), n, k, _lib.ptr(ex), n_ex,
+                                                 chunk, values.data_ptr(), ids.data_ptr(), flag.data_ptr(),
+                                                 ws.data_ptr(), nbytes, _lib.stream_ptr(dev)))
             elif vp is None:
-                _lib.check(L.recnn_discrete_topk_sets(d, flat.data_ptr(), state.data_ptr(), n, k, *table, chunk,
+                _lib.check(L.recnn_discrete_topk_sets(d, flat.data_ptr(), a.state.data_ptr(), n, k, *table, chunk,
                                                       values.data_ptr(), ids.data_ptr(), flag.data_ptr(),
                                                       ws.data_ptr(), nbytes, _lib.stream_ptr(dev)))
             else:
                 shard = vp.shard()
                 rec = torch.empty(L.recnn_vocab_topk_record_floats(n, k), device=dev, dtype=torch.float32)
-                if sets is None:
-                    _lib.check(L.recnn_discrete_shard_topk(d, shard, flat.data_ptr(), state.data_ptr(), n, k,
+                if table is None:
+                    _lib.check(L.recnn_discrete_shard_topk(d, shard, flat.data_ptr(), a.state.data_ptr(), n, k,
                                                            _lib.ptr(ex), n_ex, chunk, rec.data_ptr(), ws.data_ptr(),
                                                            nbytes, _lib.stream_ptr(dev)))
                 else:
-                    _lib.check(L.recnn_discrete_shard_topk_sets(d, shard, flat.data_ptr(), state.data_ptr(), n, k,
+                    _lib.check(L.recnn_discrete_shard_topk_sets(d, shard, flat.data_ptr(), a.state.data_ptr(), n, k,
                                                                 *table, chunk, rec.data_ptr(), flag[1:].data_ptr(),
                                                                 ws.data_ptr(), nbytes, _lib.stream_ptr(dev)))
                 del ws
@@ -253,15 +280,74 @@ class DiscreteActor(nn.Module):
                 _lib.check(L.recnn_discrete_shard_topk_finish(d, shard, gathered.data_ptr(), n, k, _lib.ptr(ex), n_ex,
                                                               values.data_ptr(), ids.data_ptr(), flag.data_ptr(),
                                                               _lib.stream_ptr(dev)))
-        f = flag.tolist()
-        bits = f[0] | f[1]
-        if bits & 2:
-            raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
-        if bits & 1:
-            raise IndexError("an excluded item id is out of range for the policy's %d items" % items)
-        if bits & 4:
-            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
-                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
+        self._slate_errors(flag, a)
+        return values, ids
+
+    def sample_topk(self, state, k, exclude=None, exclude_rows=None, seed=None):
+        """``(values, indices)`` of a slate of k items per row drawn from the policy without replacement: the
+        distribution of ``torch.multinomial(self(state), k, replacement=False)`` with the excluded items'
+        probabilities set to 0, position 0 the first draw, every row independent -- without forming the
+        [N, num_items] probabilities.  The draw is the top-k of logit + Gumbel noise (Gumbel-top-k), so it runs
+        ``topk``'s pass with another key; ``exclude`` / ``exclude_rows``, k, the errors and the -1 / 0 padding of
+        short rows are ``topk``'s.  values fp32 [N, k] = pi(a|s) under the full softmax (excluded items stay in the
+        normaliser), indices int64 [N, k] global item ids.
+
+        ``seed``: None draws a 63-bit seed from torch's default CPU generator (so ``torch.manual_seed`` makes a call
+        reproducible and successive calls differ); an int in [0, 2^64) keys the noise, which is then a pure function
+        of (seed, global row, item id): the ids do not depend on the chunking, the GEMM back end (beyond the logits'
+        rounding), the world size or the batching.  On a vocabulary-parallel policy the slate is over the whole
+        vocabulary (one all-gather of k candidates per row and rank) and every rank returns the same bits; ranks
+        passing different seeds raise RuntimeError on every rank.  On a data-parallel replica row r is keyed by its
+        global row, so the ranks' rows are the single-GPU call's over the whole batch.  Inference only: nothing saved
+        for the policy update is touched."""
+        from .update.reinforce import _chunk_items
+        if seed is not None and (isinstance(seed, bool) or not isinstance(seed, int) or not 0 <= seed < 2 ** 64):
+            raise ValueError("seed must be None or an int in [0, 2^64), got %r" % (seed,))
+        a = self._slate_args(state, k, exclude, exclude_rows)
+        row0 = self._row_offset(a.n) or 0            # a collective on a data-parallel replica, before any return
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())
+        if a.n == 0:
+            return a.values, a.ids
+        vp, d, n, dev, ex, n_ex = a.vp, a.d, a.n, a.dev, a.ex, a.n_ex
+        values, ids, table = a.values, a.ids, a.table
+        L = _lib.lib()
+        flat = param_arena(self)
+        chunk = _chunk_items(n, d.num_items)
+        nbytes = L.recnn_discrete_topk_workspace_bytes(d, n, k, chunk)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        flag = torch.zeros(2, dtype=torch.int32, device=dev)       # the call's bits, the table check's (sharded)
+        st = _lib.stream_ptr(dev)
+        with torch.cuda.device(dev):
+            if vp is None and table is None:
+                _lib.check(L.recnn_discrete_sample_topk(d, flat.data_ptr(), a.state.data_ptr(), n, k, _lib.ptr(ex),
+                                                        n_ex, seed, row0, chunk, values.data_ptr(), ids.data_ptr(),
+                                                        flag.data_ptr(), ws.data_ptr(), nbytes, st))
+            elif vp is None:
+                _lib.check(L.recnn_discrete_sample_topk_sets(d, flat.data_ptr(), a.state.data_ptr(), n, k, *table,
+                                                             seed, row0, chunk, values.data_ptr(), ids.data_ptr(),
+                                                             flag.data_ptr(), ws.data_ptr(), nbytes, st))
+            else:
+                shard = vp.shard()
+                rec = torch.empty(L.recnn_vocab_sample_topk_record_floats(n, k), device=dev, dtype=torch.float32)
+                if table is None:
+                    _lib.check(L.recnn_discrete_shard_sample_topk(d, shard, flat.data_ptr(), a.state.data_ptr(), n, k,
+                                                                  _lib.ptr(ex), n_ex, seed, row0, chunk,
+                                                                  rec.data_ptr(), ws.data_ptr(), nbytes, st))
+                else:
+                    _lib.check(L.recnn_discrete_shard_sample_topk_sets(d, shard, flat.data_ptr(), a.state.data_ptr(),
+                                                                       n, k, *table, seed, row0, chunk,
+                                                                       rec.data_ptr(), flag[1:].data_ptr(),
+                                                                       ws.data_ptr(), nbytes, st))
+                del ws
+                gathered = vp.all_gather(rec)
+                _lib.check(L.recnn_discrete_shard_sample_topk_finish(d, shard, gathered.data_ptr(), n, k, _lib.ptr(ex),
+                                                                     n_ex, seed, values.data_ptr(), ids.data_ptr(),
+                                                                     flag.data_ptr(), st))
+        if vp is not None and flag.tolist()[0] & 2:
+            raise RuntimeError("the ranks disagree on the vocabulary shard plan, the number of rows or the seed: pass "
+                               "every rank the same seed (or seed every rank's generator the same)")
+        self._slate_errors(flag, a)
         return values, ids
 
     def rank(self, state, target, exclude=None, exclude_rows=None):
