@@ -639,6 +639,24 @@ RECNN_API int recnn_discrete_shard_rank_finish(const recnn_discrete_dims* d, con
                                                const float* gathered_stats, const float* gathered_counts,
                                                const int64_t* target, int64_t n_rows, int64_t* rank_out,
                                                float* log_prob_out, int32_t* error_flag, void* stream);
+/* Off-policy estimation: log pi(a | s) of given items, the pi_categorical.log_prob(pi_action) of recnn/nn/models.py:142
+ * for logged actions, without the Categorical's clamp and without the [n_rows, num_items] probabilities.
+ * log_prob_out fp32 [n_rows] = z_a - M - log S, computed by recnn_discrete_rank's pass 1 (the same chunking, logits and
+ * expression), so it equals recnn_discrete_rank's log_prob_out bit for bit; no count pass.  *error_flag <- 1 when an id
+ * is outside [0, num_items) (its log-prob is 0).  workspace: recnn_discrete_rank_workspace_bytes.  On a
+ * vocabulary-sharded policy, recnn_discrete_shard_rank_stats writes the stats record and, after its all-gather,
+ * recnn_vocab_log_prob_finish below gives every rank the same bits (at world 1, this call's). */
+RECNN_API int recnn_discrete_log_prob(const recnn_discrete_dims* d, const float* params, const float* state,
+                                      const int64_t* action, int64_t n_rows, int32_t chunk_items, float* log_prob_out,
+                                      int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
+/* gathered stats records (recnn_vocab_record_floats(n_rows) floats per rank, rank order: those of
+ * recnn_discrete_shard_rank_stats or recnn_beta_shard_log_prob_stats) -> log_prob_out fp32 [n_rows] = z_a - M - log S
+ * with M, S and z_a merged in rank order, the same bits on every rank.  It serves either net: this rank's block is
+ * [v->item_offset, the hi of its own header).  *error_flag <- bits: 1 = an id outside [0, v->num_items) (log-prob 0);
+ * 2 = the headers do not tile the vocabulary in rank order with this rank's first item, or the ranks disagree on
+ * n_rows. */
+RECNN_API int recnn_vocab_log_prob_finish(const recnn_vocab_shard* v, const float* gathered, const int64_t* action,
+                                          int64_t n_rows, float* log_prob_out, int32_t* error_flag, void* stream);
 
 /* ---- REINFORCE: the critic side with item-id actions ---------------------------------------------
  * The REINFORCE critic is a Critic(S, num_items, H) (recnn/nn/update/reinforce.py:92-102): layer 1 is W1 [H, S + num_items]
@@ -824,6 +842,24 @@ RECNN_API int recnn_beta_shard_rows(const recnn_beta_args* args, const recnn_voc
                                     float* record, void* stream);
 RECNN_API int recnn_beta_shard_end(const recnn_beta_args* args, const recnn_vocab_shard* v, const float* gathered,
                                    void* stream);
+/* Off-policy estimation: log beta(a | s) of given items, inference only -- the beta_categorical.log_prob(beta_action)
+ * of recnn/nn/models.py:143 on the probabilities of :121 for logged actions, without the training step that the
+ * notebook's beta(state, action) takes and without its [n_rows, num_items] output.  Pass 1 of recnn_beta_step (the same
+ * code) with the logits of each chunk in a [n_rows, chunk_items] scratch, then log_prob_out fp32 [n_rows] = z_a - M -
+ * log S.  Reads params only: no gradient, optimizer state or probabilities are touched.  state [n_rows, state_ld].
+ * *error_flag <- 1 when an id is outside [0, num_items) (its log-prob is 0).  workspace_bytes >=
+ * recnn_beta_log_prob_workspace_bytes (0 when chunk_items is refused): the state image, one [n_rows, chunk_items] block
+ * and three [n_rows] planes.  On a sharded beta (d: the LOCAL dims, ids global), shard_log_prob_stats runs the pass over
+ * the rank's block into a stats record of the policy's format (recnn_vocab_record_floats(n_rows)); after its
+ * all-gather, recnn_vocab_log_prob_finish gives every rank the same bits (at world 1, recnn_beta_log_prob's). */
+RECNN_API int64_t recnn_beta_log_prob_workspace_bytes(const recnn_beta_dims* d, int64_t n_rows, int32_t chunk_items);
+RECNN_API int recnn_beta_log_prob(const recnn_beta_dims* d, const float* params, const float* state, int64_t state_ld,
+                                  const int64_t* action, int64_t n_rows, int32_t chunk_items, float* log_prob_out,
+                                  int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
+RECNN_API int recnn_beta_shard_log_prob_stats(const recnn_beta_dims* d, const recnn_vocab_shard* v,
+                                              const float* params, const float* state, int64_t state_ld,
+                                              const int64_t* action, int64_t n_rows, int32_t chunk_items,
+                                              float* record, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- data parallel: all-reduce over NVLink peer memory ------------------------------------------
  * BASELINE north_star: "partition the embedding gather + update across the 8 GPUs of one box with

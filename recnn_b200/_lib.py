@@ -246,6 +246,10 @@ SIGNATURES = {
     "recnn_discrete_shard_rank_finish": (C.c_int, [C.POINTER(DiscreteDims), C.POINTER(VocabShard), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p]),
+    "recnn_discrete_log_prob": (C.c_int, [C.POINTER(DiscreteDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_vocab_log_prob_finish": (C.c_int, [C.POINTER(VocabShard), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]),
     "recnn_critic_action_term_scratch_floats":(C.c_int64, [C.POINTER(Dims), C.POINTER(DiscreteDims), C.c_int64,
                                                             C.c_int32]),
     "recnn_critic_action_term_chunked": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.POINTER(DiscreteDims), C.c_void_p,
@@ -280,6 +284,12 @@ SIGNATURES = {
     "recnn_beta_shard_rows": (C.c_int, [C.POINTER(BetaArgs), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
                                         C.c_void_p]),
     "recnn_beta_shard_end": (C.c_int, [C.POINTER(BetaArgs), C.POINTER(VocabShard), C.c_void_p, C.c_void_p]),
+    "recnn_beta_log_prob_workspace_bytes": (C.c_int64, [C.POINTER(BetaDims), C.c_int64, C.c_int32]),
+    "recnn_beta_log_prob": (C.c_int, [C.POINTER(BetaDims), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                      C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "recnn_beta_shard_log_prob_stats": (C.c_int, [C.POINTER(BetaDims), C.POINTER(VocabShard), C.c_void_p, C.c_void_p,
+                                                  C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p,
+                                                  C.c_int64, C.c_void_p]),
     "recnn_comm_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]),
     "recnn_comm_handle_bytes": (C.c_int32, []),
     "recnn_comm_local_handle": (C.c_int, [C.c_void_p, C.c_void_p]),

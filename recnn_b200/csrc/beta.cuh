@@ -237,28 +237,35 @@ static int beta_check(const recnn_beta_args* a, BetaWorkspace* w) {
   return check_workspace(w->bytes, a->workspace_bytes);
 }
 
-// Pass 1: the flags zeroed, the state re-pitched (when it is not TMA-legal), then the logits of each chunk into
-// probs_out, folded into the row's running max / sum of exp (run_max, run_sum) and the target's logit (za; lo: the
-// global id of the arena's first item).
-static int beta_logits_pass(const recnn_beta_args* a, const BetaWorkspace& w, int lo, float* run_max, float* run_sum,
-                            float* za, cudaStream_t st) {
-  const int S = a->dims.state_dim, I = a->dims.num_items, W = a->chunk_items;
-  const int64_t n = a->n_rows;
-  const BetaLayout l = beta_layout(a->dims);
-  const float* P = a->net.params;
-  const long long* act = reinterpret_cast<const long long*>(a->action);
-  RECNN_CHECK_CUDA(cudaMemsetAsync(w.flags, 0, 8 * sizeof(unsigned), st));
+// Pass 1: the state re-pitched into img (when it is not TMA-legal), then the logits of each chunk of W items into z,
+// folded into the row's running max / sum of exp (run_max, run_sum) and the target's logit (za; lo: the global id of
+// the arena's first item).  z has row pitch ldz: with ldz == num_items it is the step's probs_out and each chunk lands
+// in its own columns; otherwise it is a [n, W] scratch that every chunk overwrites (the inference-only log-prob).
+static int beta_logits_pass(const recnn_beta_dims& d, const float* P, const float* state, int64_t state_ld,
+                            const long long* act, int64_t n, int W, float* img, float* z, int64_t ldz, int lo,
+                            float* run_max, float* run_sum, float* za, cudaStream_t st) {
+  const int S = d.state_dim, I = d.num_items;
+  const BetaLayout l = beta_layout(d);
   Seg xs;
-  RECNN_PROPAGATE(repitch_state(S, a->state, n, w.img, &xs, st, a->state_ld));
+  RECNN_PROPAGATE(repitch_state(S, state, n, img, &xs, st, state_ld));
   for (int c0 = 0; c0 < I; c0 += W) {
     const int wc = I - c0 < W ? I - c0 : W;
-    RECNN_PROPAGATE(linear_out(xs, P + l.w + (int64_t)c0 * l.ldw, l.ldw, P + l.b + c0, wc, n, 0, nullptr,
-                               a->probs_out + c0, I, st));
-    logit_stats_kernel<<<row_grid(n), kRowThreads, 0, st>>>(a->probs_out + c0, I, n, wc, c0, act, lo, run_max, run_sum,
-                                                            za);
+    float* zc = ldz == I ? z + c0 : z;
+    RECNN_PROPAGATE(linear_out(xs, P + l.w + (int64_t)c0 * l.ldw, l.ldw, P + l.b + c0, wc, n, 0, nullptr, zc, ldz,
+                               st));
+    logit_stats_kernel<<<row_grid(n), kRowThreads, 0, st>>>(zc, ldz, n, wc, c0, act, lo, run_max, run_sum, za);
     RECNN_CHECK_LAUNCH("logit_stats_kernel");
   }
   return RECNN_OK;
+}
+
+// Pass 1 of the step and of its sharded begin: the flags zeroed, then beta_logits_pass into probs_out.
+static int beta_step_logits(const recnn_beta_args* a, const BetaWorkspace& w, int lo, float* run_max, float* run_sum,
+                            float* za, cudaStream_t st) {
+  RECNN_CHECK_CUDA(cudaMemsetAsync(w.flags, 0, 8 * sizeof(unsigned), st));
+  return beta_logits_pass(a->dims, a->net.params, a->state, a->state_ld, reinterpret_cast<const long long*>(a->action),
+                          a->n_rows, a->chunk_items, w.img, a->probs_out, a->dims.num_items, lo, run_max, run_sum, za,
+                          st);
 }
 
 // After the row terms: the mean loss, pass 2 (dZ of each chunk, its dW rows and db slice, overwriting the arena:
@@ -295,7 +302,7 @@ extern "C" int recnn_beta_step(const recnn_beta_args* a, void* stream) {
   const int I = a->dims.num_items;
   const int64_t n = a->n_rows;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  RECNN_PROPAGATE(beta_logits_pass(a, w, 0, w.run_max, w.run_sum, w.za, st));
+  RECNN_PROPAGATE(beta_step_logits(a, w, 0, w.run_max, w.run_sum, w.za, st));
   beta_rows_kernel<<<row_grid(n), kRowThreads, 0, st>>>(a->probs_out, I, n, I, reinterpret_cast<const long long*>(
                                                             a->action), w.run_max, w.run_sum, w.za, w.T, w.pe, w.pa,
                                                         w.row_loss, w.flags);
@@ -318,7 +325,7 @@ extern "C" int recnn_beta_shard_begin(const recnn_beta_args* a, const recnn_voca
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t n = a->n_rows;
   RECNN_PROPAGATE(shard_record_init(p, record, n, st));
-  return beta_logits_pass(a, w, p.lo, shard_plane(record, n, 0), shard_plane(record, n, 1), shard_plane(record, n, 2),
+  return beta_step_logits(a, w, p.lo, shard_plane(record, n, 0), shard_plane(record, n, 1), shard_plane(record, n, 2),
                           st);
 }
 
@@ -351,4 +358,77 @@ extern "C" int recnn_beta_shard_end(const recnn_beta_args* a, const recnn_vocab_
       w.row_loss, w.flags);
   RECNN_CHECK_LAUNCH("beta_shard_terms_kernel");
   return beta_grad_pass(a, w, p.lo, p.items, st);
+}
+
+// ---- log beta(a | s) of given items, inference only: pass 1 into a [n, chunk] scratch, then target_log_prob.  No
+// gradient arena, optimizer state or probs_out is read or written.
+struct BetaLogProbWorkspace {
+  float *img, *z, *run_max, *run_sum, *za;       // [n, pad4(S)], [n, chunk], three [n]
+  int64_t bytes;
+};
+static BetaLogProbWorkspace beta_log_prob_carve(const recnn_beta_dims& d, int64_t n, int chunk, void* base) {
+  BetaLogProbWorkspace w;
+  Carve c(base);
+  w.img = c.take(n * pad4(d.state_dim));
+  w.z = c.take(n * (int64_t)chunk);
+  w.run_max = c.take(n);
+  w.run_sum = c.take(n);
+  w.za = c.take(n);
+  w.bytes = c.bytes();
+  return w;
+}
+
+extern "C" int64_t recnn_beta_log_prob_workspace_bytes(const recnn_beta_dims* d, int64_t n_rows, int32_t chunk_items) {
+  if (!beta_dims_ok(d) || n_rows <= 0 || !chunk_ok(d->num_items, chunk_items)) return 0;
+  return beta_log_prob_carve(*d, n_rows, chunk_items, nullptr).bytes;
+}
+
+// the checks of both log-prob entry points (d: the arena's dims, local on a shard); *w <- the carved workspace
+static int beta_log_prob_check(const recnn_beta_dims* d, const float* params, const float* state, int64_t state_ld,
+                               const int64_t* action, int64_t n_rows, int32_t chunk_items, void* workspace,
+                               int64_t workspace_bytes, BetaLogProbWorkspace* w) {
+  RECNN_REQUIRE(beta_dims_ok(d) && params && state && action && workspace, "null pointer / dims");
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  RECNN_REQUIRE(state_ld >= d->state_dim, "state_ld");
+  RECNN_REQUIRE(chunk_ok(d->num_items, chunk_items), "chunk_items must be num_items or a positive multiple of 128 below it");
+  const int64_t widest = pad4(d->state_dim) > chunk_items ? pad4(d->state_dim) : chunk_items;
+  RECNN_REQUIRE(n_rows < (1ll << 31) / (widest + 1), "n_rows too large for int32 tile indexing");
+  *w = beta_log_prob_carve(*d, n_rows, chunk_items, workspace);
+  return check_workspace(w->bytes, workspace_bytes);
+}
+
+extern "C" int recnn_beta_log_prob(const recnn_beta_dims* d, const float* params, const float* state, int64_t state_ld,
+                                   const int64_t* action, int64_t n_rows, int32_t chunk_items, float* log_prob_out,
+                                   int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(log_prob_out && error_flag, "null pointer");
+  BetaLogProbWorkspace w;
+  RECNN_PROPAGATE(beta_log_prob_check(d, params, state, state_ld, action, n_rows, chunk_items, workspace,
+                                      workspace_bytes, &w));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long* act = reinterpret_cast<const long long*>(action);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(rank_target_check(act, n_rows, d->num_items, error_flag, st));
+  RECNN_PROPAGATE(beta_logits_pass(*d, params, state, state_ld, act, n_rows, chunk_items, w.img, w.z, chunk_items, 0,
+                                   w.run_max, w.run_sum, w.za, st));
+  log_prob_finish_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(w.za, w.run_max, w.run_sum, act, n_rows,
+                                                                          d->num_items, log_prob_out);
+  RECNN_CHECK_LAUNCH("log_prob_finish_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_beta_shard_log_prob_stats(const recnn_beta_dims* d, const recnn_vocab_shard* v,
+                                               const float* params, const float* state, int64_t state_ld,
+                                               const int64_t* action, int64_t n_rows, int32_t chunk_items,
+                                               float* record, void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(record, "null pointer");
+  BetaLogProbWorkspace w;
+  RECNN_PROPAGATE(beta_log_prob_check(d, params, state, state_ld, action, n_rows, chunk_items, workspace,
+                                      workspace_bytes, &w));
+  ShardPlan p;
+  RECNN_PROPAGATE(shard_plan(d->num_items, v, &p));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_PROPAGATE(shard_record_init(p, record, n_rows, st));
+  return beta_logits_pass(*d, params, state, state_ld, reinterpret_cast<const long long*>(action), n_rows, chunk_items,
+                          w.img, w.z, chunk_items, p.lo, shard_plane(record, n_rows, 0),
+                          shard_plane(record, n_rows, 1), shard_plane(record, n_rows, 2), st);
 }

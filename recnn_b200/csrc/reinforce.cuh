@@ -1133,6 +1133,43 @@ __global__ void shard_rank_finish_kernel(const float* __restrict__ gs, const flo
   logp[r] = target_log_prob(za, M, S);
 }
 
+// ---- log pi(a | s) and log beta(a | s) of given items (off-policy estimation): pass 1 alone, then target_log_prob.
+
+// one thread per row: log-prob of action[r] from the row's statistics (0 for an id outside [0, items), which the
+// caller's check flags)
+__global__ void log_prob_finish_kernel(const float* __restrict__ za, const float* __restrict__ run_max,
+                                       const float* __restrict__ run_sum, const long long* __restrict__ action,
+                                       long long n, int items, float* __restrict__ logp) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const bool ok = action[r] >= 0 && action[r] < items;
+  logp[r] = ok ? target_log_prob(za[r], run_max[r], run_sum[r]) : 0.f;
+}
+
+// gathered stats records (either net's) -> every rank's log-prob: M, S and the action's logit merged in rank order
+// (shard_merge_row).  The finish sees no arena, so this rank's block ends where its own header says.  *flag |= 2 when
+// the headers do not tile the vocabulary with this rank's first item, |= 1 for an id outside [0, items).
+__global__ void vocab_log_prob_finish_kernel(const float* __restrict__ g, long long n, ShardPlan p,
+                                             const long long* __restrict__ action, float* __restrict__ logp,
+                                             int* flag) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = shard_record_floats(n);
+  if (r == 0) {
+    p.hi = reinterpret_cast<const int*>(g + p.rank * stride)[1];
+    if (shard_plan_bad(g, stride, p, n)) atomicOr(flag, 2);
+  }
+  if (r >= n) return;
+  const long long a = action[r];
+  if (a < 0 || a >= p.items) {
+    atomicOr(flag, 1);
+    logp[r] = 0.f;
+    return;
+  }
+  float M, S, za;
+  shard_merge_row(g, p.world, n, r, M, S, za);
+  logp[r] = target_log_prob(za, M, S);
+}
+
 }  // namespace recnn
 
 using namespace recnn;
@@ -1686,15 +1723,23 @@ static int rank_check(const recnn_discrete_dims* d, const float* params, const i
   return check_workspace(rank_carve(*d, n_rows, chunk_items, nullptr).bytes, workspace_bytes);
 }
 
+// pass 1 of an unsharded call: the target check, the hidden layer and the stats pass into w.s (run_max, run_sum, za)
+static int rank_stats_local(const recnn_discrete_dims& d, const float* params, const float* state,
+                            const long long* target, int64_t n, int chunk, int* flag, const RankWorkspace& w,
+                            cudaStream_t st) {
+  const DiscreteScratch& s = w.s;
+  RECNN_PROPAGATE(rank_target_check(target, n, d.num_items, flag, st));
+  RECNN_PROPAGATE(discrete_hidden(d, params, state, n, s, st, nullptr));
+  return reinforce_stats_pass(d, params, n, s, chunk, target, 0, s.run_max, s.run_sum, s.za, st);
+}
+
 // both passes and the finish of an unsharded call
 static int rank_local(const recnn_discrete_dims& d, const float* params, const float* state, const long long* target,
                       int64_t n, const ItemSets& sets, int chunk, int64_t* rank_out, float* log_prob_out, int* flag,
                       const RankWorkspace& w, cudaStream_t st) {
   const DiscreteScratch& s = w.s;
   RECNN_CHECK_CUDA(cudaMemsetAsync(w.counts, 0, n * sizeof(int), st));
-  RECNN_PROPAGATE(rank_target_check(target, n, d.num_items, flag, st));
-  RECNN_PROPAGATE(discrete_hidden(d, params, state, n, s, st, nullptr));
-  RECNN_PROPAGATE(reinforce_stats_pass(d, params, n, s, chunk, target, 0, s.run_max, s.run_sum, s.za, st));
+  RECNN_PROPAGATE(rank_stats_local(d, params, state, target, n, chunk, flag, w, st));
   RECNN_PROPAGATE(rank_count_pass(d, params, n, s, chunk, 0, d.num_items, target, s.za, sets, w.counts, st));
   policy_rank_finish_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(
       w.counts, s.za, s.run_max, s.run_sum, target, n, d.num_items, reinterpret_cast<long long*>(rank_out),
@@ -1821,5 +1866,38 @@ extern "C" int recnn_discrete_shard_rank_finish(const recnn_discrete_dims* d, co
       gathered_stats, gathered_counts, n_rows, p, reinterpret_cast<const long long*>(target),
       reinterpret_cast<long long*>(rank_out), log_prob_out, error_flag);
   RECNN_CHECK_LAUNCH("shard_rank_finish_kernel");
+  return RECNN_OK;
+}
+
+// ---- log-probs of given items (off-policy estimation) ---------------------------------------------------------
+extern "C" int recnn_discrete_log_prob(const recnn_discrete_dims* d, const float* params, const float* state,
+                                       const int64_t* action, int64_t n_rows, int32_t chunk_items, float* log_prob_out,
+                                       int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream) {
+  RECNN_REQUIRE(state && log_prob_out, "null pointer");
+  RECNN_PROPAGATE(rank_check(d, params, action, n_rows, chunk_items, error_flag, workspace, workspace_bytes));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const RankWorkspace w = rank_carve(*d, n_rows, chunk_items, workspace);
+  const long long* act = reinterpret_cast<const long long*>(action);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  RECNN_PROPAGATE(rank_stats_local(*d, params, state, act, n_rows, chunk_items, error_flag, w, st));
+  log_prob_finish_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(w.s.za, w.s.run_max, w.s.run_sum, act,
+                                                                          n_rows, d->num_items, log_prob_out);
+  RECNN_CHECK_LAUNCH("log_prob_finish_kernel");
+  return RECNN_OK;
+}
+
+extern "C" int recnn_vocab_log_prob_finish(const recnn_vocab_shard* v, const float* gathered, const int64_t* action,
+                                           int64_t n_rows, float* log_prob_out, int32_t* error_flag, void* stream) {
+  RECNN_REQUIRE(gathered && action && log_prob_out && error_flag, "null pointer");
+  RECNN_REQUIRE(v && v->num_items > 0 && v->world >= 1 && v->rank >= 0 && v->rank < v->world &&
+                    v->item_offset >= 0 && v->item_offset < v->num_items,
+                "shard: rank / world / item_offset outside the vocabulary");
+  RECNN_REQUIRE(n_rows > 0, "n_rows");
+  const ShardPlan p{v->world, v->rank, v->item_offset, -1, v->num_items};      // hi: from the rank's own header
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
+  vocab_log_prob_finish_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, st>>>(
+      gathered, n_rows, p, reinterpret_cast<const long long*>(action), log_prob_out, error_flag);
+  RECNN_CHECK_LAUNCH("vocab_log_prob_finish_kernel");
   return RECNN_OK;
 }

@@ -285,13 +285,17 @@ class DeviceFrameFeed:
         item (the user's last rated item); ``exclude_rows`` int64 [U], the user positions, the rows of
         ``seen_items()``.  ``policy.rank(h["state"], h["target"], exclude=feed.seen_items(),
         exclude_rows=h["exclude_rows"])`` ranks each held-out item among the items the user has not rated before (the
-        target itself is never excluded).  A user with fewer than F + 1 items raises ValueError."""
+        target itself is never excluded).  ``reward`` fp32 [U] is the held-out item's rating (bit for bit
+        ``embed(windows(last))["reward"]``): with ``target`` as the logged action, the logged data of an off-policy
+        estimate (``recnn_b200.utils.metrics.off_policy_estimates``).  A user with fewer than F + 1 items raises
+        ValueError."""
         last = self.csr.holdout_windows(user_positions)
         pos = np.array(user_positions, dtype=np.int64).reshape(-1)
         batch = self.windows(torch.from_numpy(last))
-        state = self.embed(batch)["state"]
-        return {"state": state, "target": batch["items"][:, self.frame_size].contiguous(),
-                "exclude_rows": torch.from_numpy(pos).to(self.device), "window_ids": batch["window_ids"]}
+        emb = self.embed(batch)
+        return {"state": emb["state"], "target": batch["items"][:, self.frame_size].contiguous(),
+                "reward": emb["reward"], "exclude_rows": torch.from_numpy(pos).to(self.device),
+                "window_ids": batch["window_ids"]}
 
     def seen_items(self):
         """``ItemSets`` with one set per user position of the CSR: the distinct items of that user's history,

@@ -84,12 +84,18 @@ class Beta(nn.Module):
                              % (n, num_items, n, tuple(action.shape)))
         return action.argmax(1)
 
-    def forward(self, state, action):
+    def _states(self, state):
+        """``state`` as a tensor [N, state_dim] (ValueError otherwise)."""
         d = self.dims
         if not torch.is_tensor(state):
             state = torch.as_tensor(state)
         if state.dim() != 2 or state.shape[1] != d.state_dim:
             raise ValueError("state must be [N, %d] (got shape %s)" % (d.state_dim, tuple(state.shape)))
+        return state
+
+    def forward(self, state, action):
+        d = self.dims
+        state = self._states(state)
         n = int(state.shape[0])
         vp = self.__dict__.get("_recnn_vp")
         self.__dict__.pop("_recnn_block", None)
@@ -155,6 +161,56 @@ class Beta(nn.Module):
         if vp is not None:
             self.__dict__["_recnn_block"] = (weakref.ref(probs), gathered)
         return probs
+
+    def log_prob(self, state, action):
+        """fp32 [N]: log beta(action | state) of given (e.g. logged) actions -- item ids [N] or a one-hot
+        [N, num_items] matrix, as ``forward`` takes -- the exact log-softmax of the logits, for off-policy estimation
+        (``recnn_b200.utils.metrics.off_policy_estimates``).  Inference only: unlike ``forward`` it takes no step, and
+        ``last_loss``, the weights, the optimizer state and the sharded block of the last ``forward`` stay as they
+        are; nothing of size [N, num_items] is allocated.  On a vocabulary-parallel Beta it covers the whole vocabulary
+        (one all-gather of O(N) records) and every rank returns the same bits; on a data-parallel replica it stays
+        local.  A bad shape raises ValueError, an id outside [0, num_items) IndexError."""
+        from .models import _log_prob_errors
+        d = self.dims
+        state = self._states(state)
+        n = int(state.shape[0])
+        vp = self.__dict__.get("_recnn_vp")
+        items = d.num_items if vp is None else vp.num_items
+        target = self._targets(action, n, items)
+        dev = self.net[0].weight.device
+        if dev.type != "cuda":
+            raise _lib.RecnnError("recnn_b200 nets run on CUDA only (Beta is on %s); call .cuda() first" % dev)
+        logp = torch.empty(n, device=dev, dtype=torch.float32)
+        if n == 0:
+            return logp
+        L = _lib.lib()
+        st = _lib.stream_ptr(dev)
+        with torch.cuda.device(dev):
+            state = state.detach().to(device=dev, dtype=torch.float32)
+            if state.stride(1) != 1:
+                state = state.contiguous()
+            target = target.detach().to(device=dev, dtype=torch.int64).contiguous()
+            flat = param_arena(self)
+            chunk = _chunk_items(n, d.num_items)
+            nbytes = L.recnn_beta_log_prob_workspace_bytes(d, n, chunk)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            flag = torch.zeros(1, dtype=torch.int32, device=dev)
+            if vp is None:
+                _lib.check(L.recnn_beta_log_prob(d, flat.data_ptr(), state.data_ptr(), state.stride(0),
+                                                 target.data_ptr(), n, chunk, logp.data_ptr(), flag.data_ptr(),
+                                                 ws.data_ptr(), nbytes, st))
+            else:
+                shard = vp.shard()
+                rec = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+                _lib.check(L.recnn_beta_shard_log_prob_stats(d, shard, flat.data_ptr(), state.data_ptr(),
+                                                             state.stride(0), target.data_ptr(), n, chunk,
+                                                             rec.data_ptr(), ws.data_ptr(), nbytes, st))
+                del ws
+                gathered = vp.all_gather(rec)
+                _lib.check(L.recnn_vocab_log_prob_finish(shard, gathered.data_ptr(), target.data_ptr(), n,
+                                                         logp.data_ptr(), flag.data_ptr(), st))
+        _log_prob_errors(int(flag.item()), items)
+        return logp
 
     def _row_parallel_grad(self, a, rows, n, dev, loss, error):
         """Data parallel: this rank's rows' share of the gradient of the cross-entropy mean over the global batch,

@@ -31,6 +31,23 @@ def _device_check(module, *tensors):
     return dev, out
 
 
+def _check_row_ids(ids, n, name):
+    """ValueError unless ``ids`` is an integer tensor [n] (one item id per row)."""
+    if (not torch.is_tensor(ids) or ids.dim() != 1 or ids.shape[0] != n
+            or ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool):
+        raise ValueError("%s must be an integer tensor [N] with N = %d rows (got %s)"
+                         % (name, n, "%s %s" % (tuple(ids.shape), ids.dtype) if torch.is_tensor(ids)
+                            else type(ids).__name__))
+
+
+def _log_prob_errors(bits, items):
+    """Raise what the error bits of a log-prob call (unsharded, or recnn_vocab_log_prob_finish) report."""
+    if bits & 2:
+        raise RuntimeError("the ranks disagree on the vocabulary shard plan or on the number of rows")
+    if bits & 1:
+        raise IndexError("an item id is out of range for the net's %d items" % items)
+
+
 def _train_masks(module, n_rows, hidden, device):
     """Dropout(p=0.5) keep-masks for the two hidden layers (train mode only)."""
     if not module.training:
@@ -368,11 +385,7 @@ class DiscreteActor(nn.Module):
         if not torch.is_tensor(state) or state.dim() != 2 or state.shape[1] != d.state_dim:
             raise ValueError("state must be a [N, %d] tensor" % d.state_dim)
         n = state.shape[0]
-        if (not torch.is_tensor(target) or target.dim() != 1 or target.shape[0] != n
-                or target.dtype.is_floating_point or target.dtype.is_complex or target.dtype == torch.bool):
-            raise ValueError("target must be an integer tensor [N] with N = %d rows (got %s)"
-                             % (n, "%s %s" % (tuple(target.shape), target.dtype) if torch.is_tensor(target)
-                                else type(target).__name__))
+        _check_row_ids(target, n, "target")
         sets = rows = None
         if isinstance(exclude, ItemSets):
             sets, rows = row_map(exclude, exclude_rows, n)
@@ -442,6 +455,54 @@ class DiscreteActor(nn.Module):
             raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
                              "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
         return rank, logp
+
+    def log_prob(self, state, action):
+        """fp32 [N]: log pi(action | state) of given (e.g. logged) item ids, the exact log-softmax z_a - M - log S --
+        not the Categorical's clamped value -- for off-policy estimation
+        (``recnn_b200.utils.metrics.off_policy_estimates``).  It is ``rank``'s pass 1 alone, so it equals ``rank``'s
+        ``log_prob`` bit for bit at a lower cost, and never forms the [N, num_items] probabilities.  On a
+        vocabulary-parallel policy it covers the whole vocabulary (one all-gather of O(N) records) and every rank
+        returns the same bits; on a data-parallel replica it stays local.  A bad shape raises ValueError, an id
+        outside [0, num_items) IndexError.  Inference only: nothing saved for the policy update is touched."""
+        from .update.reinforce import _chunk_items
+        vp = self.__dict__.get("_recnn_vp")
+        d = self.dims
+        items = d.num_items if vp is None else vp.num_items
+        if not torch.is_tensor(state) or state.dim() != 2 or state.shape[1] != d.state_dim:
+            raise ValueError("state must be a [N, %d] tensor" % d.state_dim)
+        n = state.shape[0]
+        _check_row_ids(action, n, "action")
+        dev = self.linear1.weight.device
+        if dev.type != "cuda":
+            raise _lib.RecnnError("recnn_b200 nets run on CUDA only (module is on %s); call .cuda() first" % dev)
+        logp = torch.empty(n, device=dev, dtype=torch.float32)
+        if n == 0:
+            return logp
+        _, (state,) = _device_check(self, state)
+        action = action.detach().to(device=dev, dtype=torch.int64).contiguous()
+        L = _lib.lib()
+        flat = param_arena(self)
+        chunk = _chunk_items(n, d.num_items)
+        nbytes = L.recnn_discrete_rank_workspace_bytes(d, n, chunk)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        st = _lib.stream_ptr(dev)
+        with torch.cuda.device(dev):
+            if vp is None:
+                _lib.check(L.recnn_discrete_log_prob(d, flat.data_ptr(), state.data_ptr(), action.data_ptr(), n, chunk,
+                                                     logp.data_ptr(), flag.data_ptr(), ws.data_ptr(), nbytes, st))
+            else:
+                shard = vp.shard()
+                stats = torch.empty(L.recnn_vocab_record_floats(n), device=dev, dtype=torch.float32)
+                _lib.check(L.recnn_discrete_shard_rank_stats(d, shard, flat.data_ptr(), state.data_ptr(),
+                                                             action.data_ptr(), n, chunk, stats.data_ptr(),
+                                                             ws.data_ptr(), nbytes, st))
+                del ws
+                gathered = vp.all_gather(stats)
+                _lib.check(L.recnn_vocab_log_prob_finish(shard, gathered.data_ptr(), action.data_ptr(), n,
+                                                         logp.data_ptr(), flag.data_ptr(), st))
+        _log_prob_errors(int(flag.item()), items)
+        return logp
 
     def gc(self):
         del self.rewards[:]
