@@ -372,6 +372,43 @@ RECNN_API int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries, 
                                        int64_t n_sets, const int64_t* row_set, int64_t* rank_out,
                                        int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- serving: items scored by the DDPG / TD3 critic (the Wolpertinger policy) ------------------------
+ * Q(s_r, e_j) = critic(state[r], table[j]) in eval mode (no dropout), params a Critic arena of dims d (TD3: value_net1),
+ * table fp32 [n_items, d->action_dim] dense, state fp32 [n_rows, d->state_dim] dense.  The columns of a row are its
+ * candidates, candidates int64 [n_rows, n_candidates] (-1: padding; e.g. a recnn_retrieve_topk of the actor's action),
+ * or, with candidates NULL and n_candidates 0, every item of the table.  Layer 1 is split into a row term (once per row)
+ * and an item term (once per item of a chunk, or per candidate), so a pair costs one H x H layer on the tensor cores;
+ * nothing of size [n_rows, n_items] or [n_rows * n_candidates, S + A] is formed.  The columns are visited in chunks of
+ * `chunk` (0: 4096); Q of a pair is the same bits at every chunk width, in both modes and whatever rows share the call.
+ * Exclusion: the set table of recnn_retrieve_topk_sets (set_ids, n_set_ids, set_offsets, n_sets, row_set), with
+ * set_offsets NULL for none.  *error_flag <- bits: 1 = a candidate outside [-1, n_items), a set id or (rank) a target
+ * outside [0, n_items); 4 = a malformed table; 8 = an id repeated within a row's candidates.  Nothing is read out of
+ * bounds either way; the results are then meaningless.
+ *
+ * workspace_bytes >= recnn_critic_serve_workspace_bytes(d, n_rows, n_candidates, n_items, k, chunk), k = 0 for a rank
+ * call.  With every item (n_candidates 0) it does not grow with n_items beyond one chunk: O(n_rows (S + H + k)) plus
+ * one block of L2-sized pair buffers. */
+RECNN_API int64_t recnn_critic_serve_workspace_bytes(const recnn_dims* d, int64_t n_rows, int64_t n_candidates,
+                                                     int64_t n_items, int32_t k, int32_t chunk);
+/* values_out fp32 [n_rows, k], ids_out int64 [n_rows, k]: the k eligible columns of highest Q per row, best first, equal
+ * Q the smaller id first; a row with fewer than k eligible columns ends in id -1, value -FLT_MAX.  1 <= k <= 64. */
+RECNN_API int recnn_critic_topk(const recnn_dims* d, const float* params, const float* state, int64_t n_rows,
+                                const float* table, int64_t n_items, const int64_t* candidates, int64_t n_candidates,
+                                int32_t k, const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
+                                int64_t n_sets, const int64_t* row_set, int32_t chunk, float* values_out,
+                                int64_t* ids_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                                void* stream);
+/* rank_out int64 [n_rows]: the number of eligible columns that beat target[r] (higher Q, or equal Q and a smaller id),
+ * i.e. its position in recnn_critic_topk on the same inputs when below k, at any k.  The target is never excluded.  A
+ * target missing from its row's candidates gets the row's count of eligible candidates; one outside [0, n_items) gets
+ * -1 and bit 1. */
+RECNN_API int recnn_critic_rank(const recnn_dims* d, const float* params, const float* state, int64_t n_rows,
+                                const float* table, int64_t n_items, const int64_t* candidates, int64_t n_candidates,
+                                const int64_t* target, const int64_t* set_ids, int64_t n_set_ids,
+                                const int64_t* set_offsets, int64_t n_sets, const int64_t* row_set, int32_t chunk,
+                                int64_t* rank_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
+                                void* stream);
+
 /* ---- REINFORCE with (Top-K) off-policy correction: the policy side (SURVEY 8f-2) ------------------
  * DiscreteActor (recnn/nn/models.py:76-99): probs = softmax(W2 relu(W1 s + b1) + b2), one output per item.
  * Parameter arena in nn.Module.parameters() order -- linear1.weight [H, S], linear1.bias, linear2.weight

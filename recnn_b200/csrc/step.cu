@@ -195,6 +195,16 @@ struct AloneScope {
   ~AloneScope() { t_alone = prev; }
 };
 
+// A call whose GEMMs must all run on one back end (critic serving: a pair's Q may not depend on which GEMM an operand
+// went through) forces the CUDA-core kernel for every gemm_nt() inside the scope when one of them cannot take the
+// tensor-core path.
+static thread_local bool t_simt = false;
+struct SimtScope {
+  bool prev;
+  explicit SimtScope(bool on) : prev(t_simt) { t_simt = on; }
+  ~SimtScope() { t_simt = prev; }
+};
+
 static int pick_bn(int64_t M, int N) {
   // 128-wide tiles when they still yield >= 64 CTAs; otherwise 64-wide (more CTAs, less reuse)
   const int64_t mt = ceil_div(M, 128);
@@ -208,7 +218,7 @@ template <int EPI>
 static int gemm_nt(const Seg& x0, const Seg& x1, const float* W, long long ldw, int N, int64_t n, const Epilogue& e,
                    cudaStream_t st) {
   const int K = x0.cols + x1.cols - x1.lead;             // logical contraction length == W's columns
-  const bool tc_ok = math_tc() && aligned16(x0.p) && (x1.cols == 0 || aligned16(x1.p)) && aligned16(W) &&
+  const bool tc_ok = math_tc() && !t_simt && aligned16(x0.p) && (x1.cols == 0 || aligned16(x1.p)) && aligned16(W) &&
                      x0.ld % 4 == 0 && (x1.cols == 0 || x1.ld % 4 == 0) && ldw % 4 == 0 && x0.lead == 0 &&
                      (x1.cols == 0 || (x0.cols - x1.lead) % 4 == 0);
   if (tc_ok) {
@@ -936,3 +946,5 @@ extern "C" int recnn_linear_forward(const float* x, int64_t n_rows, int in_dim, 
 #include "critic_ids.cuh"
 // ---------------------------------------------------------------- REINFORCE Top-K: the behaviour policy beta
 #include "beta.cuh"
+// ---------------------------------------------------------------- DDPG / TD3 serving: items scored by the critic's Q
+#include "critic_serve.cuh"

@@ -120,6 +120,137 @@ class Critic(nn.Module):
                 out.data_ptr(), scratch.data_ptr(), _lib.stream_ptr(dev)))
         return out
 
+    # -- serving: items scored by Q (the Wolpertinger policy) --------------------------------------------------------
+    def _serve_args(self, state, items, candidates, exclude, exclude_rows, chunk, target=None):
+        """The argument handling of ``topk`` and ``rank``: every refusal before any device work, then the device
+        forms.  A namespace of d, n, dev, state, items, cand / m (m = 0: every item), table (the C arguments of the
+        exclusion: five values, offsets None for none), target, chunk."""
+        from ..data.item_sets import ItemSets, row_map
+        d = self.dims
+        if not torch.is_tensor(state) or state.dim() != 2 or state.shape[1] != d.state_dim \
+                or not state.dtype.is_floating_point:
+            raise ValueError("state must be a floating-point tensor [N, %d]" % d.state_dim)
+        n = state.shape[0]
+        if not torch.is_tensor(items) or items.dim() != 2 or items.dtype != torch.float32 or items.shape[0] < 1:
+            raise ValueError("items must be the fp32 embedding table [n_items, %d] (got %s)"
+                             % (d.action_dim, "%s %s" % (tuple(items.shape), items.dtype) if torch.is_tensor(items)
+                                else type(items).__name__))
+        if items.shape[1] != d.action_dim:
+            raise ValueError("items has %d columns but the critic's action_dim is %d" % (items.shape[1], d.action_dim))
+        if candidates is not None:
+            if (not torch.is_tensor(candidates) or candidates.dim() != 2 or candidates.shape[0] != n
+                    or candidates.shape[1] < 1 or candidates.dtype.is_floating_point or candidates.dtype.is_complex
+                    or candidates.dtype == torch.bool):
+                raise ValueError("candidates must be an integer tensor [N, M] with N = %d rows and M >= 1 (got %s)"
+                                 % (n, "%s %s" % (tuple(candidates.shape), candidates.dtype)
+                                    if torch.is_tensor(candidates) else type(candidates).__name__))
+        sets = rows = None
+        if isinstance(exclude, ItemSets):
+            sets, rows = row_map(exclude, exclude_rows, n)
+        elif exclude is not None:
+            raise ValueError("exclude must be a recnn_b200.data.ItemSets (got %s)" % type(exclude).__name__)
+        elif exclude_rows is not None:
+            raise ValueError("exclude_rows maps rows to the sets of an ItemSets exclude")
+        if target is not None:
+            _check_row_ids(target, n, "target")
+        if chunk is None:
+            chunk = 0
+        if isinstance(chunk, bool) or not isinstance(chunk, int) or not 0 <= chunk < 2 ** 31:
+            raise ValueError("chunk must be None (auto) or an int in [1, 2^31), got %r" % (chunk,))
+        dev = self.linear1.weight.device
+        if dev.type != "cuda":
+            raise _lib.RecnnError("recnn_b200 nets run on CUDA only (module is on %s); call .cuda() first" % dev)
+        if items.device != dev:
+            raise ValueError("items must be on the critic's device %s (got %s)" % (dev, items.device))
+        a = types.SimpleNamespace(d=d, n=n, dev=dev, chunk=chunk, n_items=int(items.shape[0]), cand=None, m=0,
+                                  table=(None, 0, None, 0, None), target=None, sets=sets)
+        if n == 0:
+            return a
+        _, (a.state,) = _device_check(self, state)
+        a.items = items.contiguous()
+        if candidates is not None:
+            a.cand = candidates.detach().to(device=dev, dtype=torch.int64).contiguous()
+            a.m = int(candidates.shape[1])
+        if target is not None:
+            a.target = target.detach().to(device=dev, dtype=torch.int64).contiguous()
+        if sets is not None:
+            a.sets = sets = sets.to(dev)
+            rows = None if rows is None else rows.to(dev).contiguous()
+            a.rows = rows                       # keeps the device copy alive: the table holds its pointer
+            a.table = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
+                       len(sets), _lib.ptr(rows))
+        return a
+
+    @staticmethod
+    def _serve_errors(flag, a):
+        bits = int(flag.item())
+        if bits & 1:
+            raise IndexError("a candidate, target or excluded item id is out of range for the table's %d items"
+                             % a.n_items)
+        if bits & 4:
+            raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(a.sets))
+        if bits & 8:
+            raise ValueError("an item id is repeated within a row's candidates")
+
+    def topk(self, state, k, items, candidates=None, exclude=None, exclude_rows=None, chunk=None):
+        """``(values, ids)``: the k items of highest Q(state[r], items[j]) per row, best first (equal Q: the smaller
+        id first) -- the Wolpertinger policy's choice when ``candidates`` holds the actor's nearest items.
+
+        ``items``: the fp32 embedding table [n_items, action_dim] on the critic's device (e.g. ``ItemIndex.table``).
+        ``candidates``: int [N, M] item ids per row, -1 padding (e.g. ``index.search(actor(state), 64).id()``, or
+        several such lists concatenated); None scores every item of the table.  ``exclude`` / ``exclude_rows``: an
+        ``ItemSets`` of ids never returned (e.g. ``DeviceFrameFeed.seen_items()``), as in ``ItemIndex.search``.
+        values fp32 [N, k] are the Q values, ids int64 [N, k]; a row with fewer than k eligible items ends in id -1,
+        value -FLT_MAX.  1 <= k <= 64.  ``chunk``: columns per chunk (None: auto); it does not change a bit.
+
+        Scores are the eval-mode forward whatever ``self.training`` says; nothing of the critic is changed.  A repeated
+        id within a row's candidates or a malformed table raises ValueError, an id out of range IndexError.  Nothing of
+        size [N, n_items] is formed: layer 1 is split into a per-row and a per-item term, and each pair costs one
+        H x H layer on the tensor cores."""
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= 64:
+            raise ValueError("k must be an int in [1, 64], got %r" % (k,))
+        a = self._serve_args(state, items, candidates, exclude, exclude_rows, chunk)
+        values = torch.empty(a.n, k, device=a.dev, dtype=torch.float32)
+        ids = torch.empty(a.n, k, device=a.dev, dtype=torch.int64)
+        if a.n == 0:
+            return values, ids
+        L = _lib.lib()
+        flat = param_arena(self)
+        nbytes = L.recnn_critic_serve_workspace_bytes(a.d, a.n, a.m, a.n_items, k, a.chunk)
+        ws = torch.empty(nbytes, device=a.dev, dtype=torch.uint8)
+        flag = torch.zeros(1, dtype=torch.int32, device=a.dev)
+        with torch.cuda.device(a.dev):
+            _lib.check(L.recnn_critic_topk(a.d, flat.data_ptr(), a.state.data_ptr(), a.n, a.items.data_ptr(),
+                                           a.n_items, _lib.ptr(a.cand), a.m, k, *a.table, a.chunk,
+                                           values.data_ptr(), ids.data_ptr(), flag.data_ptr(), ws.data_ptr(), nbytes,
+                                           _lib.stream_ptr(a.dev)))
+        self._serve_errors(flag, a)
+        return values, ids
+
+    def rank(self, state, target, items, candidates=None, exclude=None, exclude_rows=None, chunk=None):
+        """int64 [N]: for offline evaluation, the number of eligible items that beat ``target[r]`` under Q (a higher
+        Q, or an equal Q and a smaller id), i.e. the target's position in ``topk`` on the same inputs when below k, at
+        any k.  Arguments as in ``topk``; a row's target is never excluded.  With ``candidates``, a target missing from
+        its row's candidates gets the row's count of eligible candidates (it is absent from every list, so
+        ``ranking_metrics`` at k <= M stays exact).  A target out of range raises IndexError."""
+        a = self._serve_args(state, items, candidates, exclude, exclude_rows, chunk, target=target)
+        rank = torch.empty(a.n, device=a.dev, dtype=torch.int64)
+        if a.n == 0:
+            return rank
+        L = _lib.lib()
+        flat = param_arena(self)
+        nbytes = L.recnn_critic_serve_workspace_bytes(a.d, a.n, a.m, a.n_items, 0, a.chunk)
+        ws = torch.empty(nbytes, device=a.dev, dtype=torch.uint8)
+        flag = torch.zeros(1, dtype=torch.int32, device=a.dev)
+        with torch.cuda.device(a.dev):
+            _lib.check(L.recnn_critic_rank(a.d, flat.data_ptr(), a.state.data_ptr(), a.n, a.items.data_ptr(),
+                                           a.n_items, _lib.ptr(a.cand), a.m, a.target.data_ptr(), *a.table, a.chunk,
+                                           rank.data_ptr(), flag.data_ptr(), ws.data_ptr(), nbytes,
+                                           _lib.stream_ptr(a.dev)))
+        self._serve_errors(flag, a)
+        return rank
+
 
 class DiscreteActor(nn.Module):
     """REINFORCE policy over a discrete item set: state -> probabilities [N, action_dim]
