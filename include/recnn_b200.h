@@ -372,6 +372,33 @@ RECNN_API int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries, 
                                        int64_t n_sets, const int64_t* row_set, int64_t* rank_out,
                                        int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- offline evaluation: distances between the items of each served slate ---------------------------
+ * The reference's diversity test: examples/streamlit_demo.py:355-445 ("Test Diversity") draws heatmaps of
+ * recnn/utils/plot.py:9-35 pairwise_distances_fig, i.e. scipy cdist(..., "cosine") and cdist(..., "euclidean") over
+ * the recommended items' embeddings.  Here the distances are read straight from the resident table and reduced per row.
+ *   ids int64 [n_rows, k] (1 <= k <= 64; -1 = empty slot), e.g. the ids of any top-k / sample / search call;
+ *   table fp32 [n_items, dim] row-major, any dim >= 1.
+ * Per row, over the unordered pairs i < j of filled slots:
+ *   mean_out fp32 [n_rows]    mean pairwise distance      (NaN when the row has < 2 filled slots)
+ *   min_out  fp32 [n_rows]    smallest pairwise distance  (NaN likewise)
+ *   count_out int32 [n_rows]  filled slots
+ *   matrix_out fp32 [n_rows, k, k] or NULL: the full matrix, symmetric bit for bit, 0 on the diagonal of filled slots,
+ *   NaN in every entry that involves an empty slot.
+ * *error_flag <- 1 when an id is outside [-1, n_items); such a slot is read as empty (nothing is read out of bounds),
+ * the results are then meaningless.
+ * Numerical contract:
+ *   EUCLIDEAN  sqrt(sum_d (a_d - b_d)^2) from the differences, never |a|^2 + |b|^2 - 2 a.b: a repeated id gives exactly 0;
+ *   COSINE     1 - a.b / (|a| |b|), clipped to [0, 2] as scipy does, norms from the staged rows in the same fma order as
+ *              the dot products, so a repeated id gives exactly 0.  A pair with a zero vector has distance 1 (scipy
+ *              gives NaN, which would poison every mean above it);
+ *   fp32 per pair; each row's pair sum in fp64 in a fixed order, no float atomics: a row's outputs depend only on its
+ *   own ids, bit for bit, whatever rows share the call.
+ * No workspace, nothing allocated: graph-capturable. */
+enum { RECNN_SLATE_EUCLIDEAN = 0, RECNN_SLATE_COSINE = 1 };
+RECNN_API int recnn_slate_distances(const int64_t* ids, int64_t n_rows, int32_t k, const float* table,
+                                    int64_t n_items, int32_t dim, int32_t metric, float* mean_out, float* min_out,
+                                    int32_t* count_out, float* matrix_out, int32_t* error_flag, void* stream);
+
 /* ---- serving: items scored by the DDPG / TD3 critic (the Wolpertinger policy) ------------------------
  * Q(s_r, e_j) = critic(state[r], table[j]) in eval mode (no dropout), params a Critic arena of dims d (TD3: value_net1),
  * table fp32 [n_items, d->action_dim] dense, state fp32 [n_rows, d->state_dim] dense.  The columns of a row are its

@@ -145,6 +145,7 @@ class DeviceFrameFeed:
         self.win_offsets = up(csr.win_offsets)
         self._err = torch.zeros(1, dtype=torch.int32, device=self.device)
         self._seen = None
+        self._popularity = None
         self.kernels = 0
 
     # ------------------------------------------------------------------ helpers
@@ -305,3 +306,11 @@ class DeviceFrameFeed:
             from .item_sets import ItemSets
             self._seen = ItemSets(self.hist_items, self.hist_offsets, unique=True)
         return self._seen
+
+    def item_popularity(self):
+        """int64 [n_items] on the feed's device: the number of resident users whose history holds each item (the
+        bincount of ``seen_items()``' ids).  Built once and cached.  With ``n_users = feed.csr.n_users`` it is the
+        popularity that ``recnn_b200.utils.metrics.slate_metrics`` scores novelty against."""
+        if self._popularity is None:
+            self._popularity = torch.bincount(self.seen_items().ids, minlength=self.table.shape[0])
+        return self._popularity

@@ -12,10 +12,31 @@ Pure torch on the ranks' device; ``ranking_metrics(..., group=)`` all-reduces th
 
 ``off_policy_estimates`` estimates the reward the policy pi would earn from logged rows (s, a, r) of the behaviour
 policy beta, with the Top-K off-policy correction's importance weights (DESIGN.md, 4d-ope).
+
+``slate_distances`` and ``slate_metrics`` describe served slates as sets (DESIGN.md, 4d-diversity).  ``ids`` is the
+int64 [N, k] output of any serving call (``DiscreteActor.topk`` / ``sample_topk``, ``ItemIndex.search``,
+``Critic.topk``), -1 marking an empty slot; a filled slot is an id >= 0.  With c_j the number of filled slots that
+hold item j (the exposure counts, over all n_items items, zeros included):
+
+  ild               mean over rows with >= 2 filled slots of the row's mean pairwise distance (intra-list diversity)
+  ild_min           the same mean, of each row's smallest pairwise distance
+  coverage          distinct recommended items / n_items
+  gini              Gini index of c: sum_i (2i - n - 1) c_(i) / (n sum c), c sorted ascending, i from 1, n = n_items;
+                    uniform exposure gives 0, all exposure on one item (n - 1) / n
+  exposure_entropy  Shannon entropy, in bits, of c / sum c
+  novelty           mean over filled slots of -log2((pop_j + 1) / (n_users + 1)), pop_j the number of users whose
+                    history holds item j (``DeviceFrameFeed.item_popularity()``)
+  rows, slots       rows and filled slots counted
+
+Distances are scipy's ``cdist`` metrics between table rows: "euclidean" sqrt(sum_d (a_d - b_d)^2) and "cosine"
+1 - a.b / (|a| |b|) clipped to [0, 2], except that a pair with a zero vector has cosine distance 1 (scipy: NaN).  They
+are computed on the device from the resident table by one kernel (recnn_slate_distances), never through an
+[N, k, dim] gather.
 """
 from __future__ import annotations
 
 import math
+import numbers
 
 import torch
 
@@ -163,4 +184,137 @@ def off_policy_estimates(pi_log_prob, beta_log_prob, reward, K=1, clip=None, gro
     if clip is not None:
         out["clipped_ips"] = s[6] / n if n else nan
         out["clipped_share"] = s[7] / n if n else nan
+    return out
+
+
+_SLATE_METRICS = {"euclidean": 0, "cosine": 1}
+
+
+def _slate_ids(ids):
+    if not torch.is_tensor(ids) or ids.dim() != 2 or ids.dtype != torch.int64:
+        raise ValueError("ids must be an int64 [N, k] tensor (got %s)"
+                         % ("%s %s" % (tuple(ids.shape), ids.dtype) if torch.is_tensor(ids) else type(ids).__name__))
+    if not 1 <= ids.shape[1] <= 64:
+        raise ValueError("a slate holds 1 <= k <= 64 slots (got k = %d)" % ids.shape[1])
+    return ids
+
+
+def _slate_args(ids, table, metric):
+    """The checks of a distance call, before any device work: (ids, table), both contiguous."""
+    from .. import _lib
+    ids = _slate_ids(ids)
+    if metric not in _SLATE_METRICS:
+        raise ValueError("metric must be one of %s (got %r)" % (sorted(_SLATE_METRICS), metric))
+    if not torch.is_tensor(table) or table.dim() != 2 or table.dtype != torch.float32 or table.shape[0] < 1 \
+            or not 1 <= table.shape[1] < 2 ** 31:
+        raise ValueError("table must be a non-empty fp32 [n_items, dim] tensor")
+    if ids.device != table.device:
+        raise ValueError("ids and table must be on the same device (ids on %s, table on %s)" % (ids.device, table.device))
+    if table.device.type != "cuda":
+        raise _lib.RecnnError("slate_distances runs on CUDA only (the table is on %s)" % table.device)
+    return ids.contiguous(), table.detach().contiguous()
+
+
+def slate_distances(ids, table, metric="cosine", matrix=False):
+    """Pairwise distances between the items of each slate, from the embedding table: ``(mean, min, count)`` or, with
+    ``matrix=True``, ``(mean, min, count, matrix)``, on the table's device.  Over the unordered pairs of filled slots
+    of row n: ``mean`` fp32 [N] their mean distance, ``min`` fp32 [N] the smallest (both NaN for a row with fewer than
+    2 filled slots), ``count`` int32 [N] the filled slots; ``matrix`` fp32 [N, k, k] every distance, symmetric bit for
+    bit, 0 on the diagonal of filled slots and NaN wherever an empty slot is involved.
+
+    ``ids`` int64 [N, k], 1 <= k <= 64, -1 for an empty slot; ``table`` fp32 [n_items, dim] on a CUDA device, the
+    ids on the same device; ``metric`` "cosine" or "euclidean" (module docstring).  A row's results depend only on
+    its own ids, bit for bit.  Nothing but the outputs is allocated.  Refused with ValueError before any device work:
+    malformed ids, k outside [1, 64], an unknown metric, a table that is not fp32 [n_items, dim], and ids on another
+    device than the table.  An id outside [-1, n_items) raises IndexError (after the call's one read-back)."""
+    from .. import _lib
+    ids, table = _slate_args(ids, table, metric)
+    n, k = ids.shape
+    dev = table.device
+    mean = torch.empty(n, dtype=torch.float32, device=dev)
+    mn = torch.empty(n, dtype=torch.float32, device=dev)
+    count = torch.empty(n, dtype=torch.int32, device=dev)
+    mat = torch.empty(n, k, k, dtype=torch.float32, device=dev) if matrix else None
+    flag = torch.empty(1, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().recnn_slate_distances(
+            ids.data_ptr(), n, k, table.data_ptr(), table.shape[0], table.shape[1], _SLATE_METRICS[metric],
+            mean.data_ptr(), mn.data_ptr(), count.data_ptr(), _lib.ptr(mat), flag.data_ptr(), _lib.stream_ptr(dev)))
+    if int(flag.item()) != 0:
+        raise IndexError("a slate id is outside [-1, %d)" % table.shape[0])
+    return (mean, mn, count, mat) if matrix else (mean, mn, count)
+
+
+def slate_metrics(ids, table=None, n_items=None, metric="cosine", popularity=None, n_users=None, group=None):
+    """Diversity, coverage, exposure concentration and novelty of served slates ``ids`` int64 [N, k] (-1: empty slot),
+    as a dict of floats with the definitions of the module docstring.  ``table`` (fp32 [n_items, dim], the ids'
+    device) adds ``ild`` and ``ild_min`` under ``metric`` (``slate_distances``); ``n_items`` defaults to the table's or
+    the popularity's length; ``popularity`` (integer counts [n_items], e.g. ``DeviceFrameFeed.item_popularity()``) with
+    ``n_users`` (e.g. ``feed.csr.n_users``) adds ``novelty``.  A mean over nothing is NaN.
+
+    ``group``: a torch.distributed process group; the exposure counts and the sums are all-reduced first, so
+    data-parallel ranks that each hold their own rows report the global values.  The ids' device must suit the group's
+    backend (CPU for gloo, CUDA for NCCL).  Refused with ValueError before any device work: what ``slate_distances``
+    refuses, no ``n_items``, a popularity that is not an integer vector of n_items counts, and popularity without
+    ``n_users``.  An id outside [-1, n_items) raises IndexError."""
+    ids = _slate_ids(ids)
+    if table is not None:
+        ids, table = _slate_args(ids, table, metric)
+        if n_items is None:
+            n_items = int(table.shape[0])
+        elif int(n_items) != table.shape[0]:
+            raise ValueError("n_items = %d but the table has %d rows" % (n_items, table.shape[0]))
+    if popularity is not None:
+        popularity = torch.as_tensor(popularity)
+        if popularity.dim() != 1 or popularity.dtype.is_floating_point or popularity.dtype == torch.bool \
+                or popularity.dtype.is_complex:
+            raise ValueError("popularity must be a 1-D integer tensor of counts")
+        if n_items is None:
+            n_items = int(popularity.shape[0])
+        if popularity.shape[0] != n_items:
+            raise ValueError("popularity holds %d counts for %d items" % (popularity.shape[0], n_items))
+        if isinstance(n_users, bool) or not isinstance(n_users, numbers.Integral) or n_users < 0:
+            raise ValueError("novelty needs n_users, an int >= 0 (got %r)" % (n_users,))
+    if isinstance(n_items, bool) or not isinstance(n_items, numbers.Integral) or n_items < 1:
+        raise ValueError("slate_metrics needs n_items >= 1 (or a table or popularity to take it from), got %r"
+                         % (n_items,))
+    n_items = int(n_items)
+    dev = ids.device
+    filled = ids[ids >= 0]
+    if ids.numel() and (int(ids.min()) < -1 or (filled.numel() and int(filled.max()) >= n_items)):
+        raise IndexError("a slate id is outside [-1, %d)" % n_items)
+    counts = torch.bincount(filled, minlength=n_items)
+    f64 = lambda x: torch.as_tensor(x, dtype=torch.float64, device=dev).reshape(())
+    parts = [f64(ids.shape[0]), f64(filled.numel())]
+    if table is not None:
+        mean, mn, count = slate_distances(ids, table, metric)
+        ok = count >= 2
+        parts += [mean[ok].double().sum(), mn[ok].double().sum(), ok.sum().double()]
+    if popularity is not None:
+        pop = popularity.to(device=dev, dtype=torch.float64)[filled]
+        parts.append((math.log2(n_users + 1.0) - torch.log2(pop + 1.0)).sum())
+    sums = torch.stack(parts)
+    if group is not None:
+        import torch.distributed as dist
+        dist.all_reduce(counts, group=group)
+        dist.all_reduce(sums, group=group)
+    s = sums.tolist()
+    nan = float("nan")
+    c = counts.double()
+    total = float(c.sum())
+    out = {"coverage": float((counts > 0).sum()) / n_items}
+    if total > 0:
+        ranks = torch.arange(1, n_items + 1, dtype=torch.float64, device=dev)
+        out["gini"] = float(((2 * ranks - n_items - 1) * torch.sort(c).values).sum()) / (n_items * total)
+        p = c[c > 0] / total
+        out["exposure_entropy"] = float(-(p * torch.log2(p)).sum())
+    else:
+        out["gini"] = out["exposure_entropy"] = nan
+    if table is not None:
+        out["ild"] = s[2] / s[4] if s[4] else nan
+        out["ild_min"] = s[3] / s[4] if s[4] else nan
+    if popularity is not None:
+        out["novelty"] = s[-1] / s[1] if s[1] else nan
+    out["rows"] = int(s[0])
+    out["slots"] = int(s[1])
     return out
