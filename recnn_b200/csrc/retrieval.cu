@@ -241,16 +241,24 @@ static int retrieve_check(const float* queries, int64_t n_queries, int32_t dim, 
   return RECNN_OK;
 }
 
-// the search behind both entry points; ex.ids NULL: no exclusion
-static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
-                    const float* norms, int32_t metric, int32_t k, const ItemSets& ex, int64_t* ids_out,
-                    float* dist_out, void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+// the checks of a search: the arguments, then the workspace carved at n_queries rows against workspace_bytes.  Every
+// refusal comes before any device work (the *_sets forms zero the caller's flag and check the table only after it).
+static int retrieve_topk_check(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                               int64_t n_items, const float* norms, int32_t metric, int32_t k, const int64_t* ids_out,
+                               const float* dist_out, void* workspace, int64_t workspace_bytes, RetrieveWorkspace* w) {
   RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
   RECNN_REQUIRE(ids_out && dist_out, "null pointer");
   RECNN_REQUIRE(k >= 1 && k <= 64 && k <= n_items, "1 <= k <= min(64, n_items)");
   if (n_queries == 0) return RECNN_OK;
-  const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, k, workspace);
-  RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
+  *w = retrieve_carve(n_queries, n_items, k, workspace);
+  return check_workspace(w->bytes, workspace_bytes);
+}
+
+// the search behind both entry points, on a checked workspace; ex.ids NULL: no exclusion
+static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
+                    const float* norms, int32_t metric, int32_t k, const ItemSets& ex, int64_t* ids_out,
+                    float* dist_out, const RetrieveWorkspace& w, cudaStream_t st) {
+  if (n_queries == 0) return RECNN_OK;
   const int stage = set_stage_bytes(ex);
   auto kernel = k <= 16 ? (stage ? topk_partial_kernel<16, true> : topk_partial_kernel<16, false>)
                         : (stage ? topk_partial_kernel<64, true> : topk_partial_kernel<64, false>);
@@ -268,14 +276,23 @@ static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const 
   });
 }
 
-// the rank behind both entry points: the slab's GEMM, then one count kernel per slab
+// the checks of a rank, as retrieve_topk_check
+static int retrieve_rank_check(const float* queries, int64_t n_queries, int32_t dim, const float* table,
+                               int64_t n_items, const float* norms, int32_t metric, const int64_t* target,
+                               const int64_t* rank_out, const int32_t* error_flag, void* workspace,
+                               int64_t workspace_bytes, RetrieveWorkspace* w) {
+  RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
+  RECNN_REQUIRE(target && rank_out && error_flag, "null pointer");
+  if (n_queries == 0) return RECNN_OK;
+  *w = retrieve_carve(n_queries, n_items, 0, workspace);
+  return check_workspace(w->bytes, workspace_bytes);
+}
+
+// the rank behind both entry points, on a checked workspace: the slab's GEMM, then one count kernel per slab
 static int retrieve_rank(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
                          const float* norms, int32_t metric, const int64_t* target, const ItemSets& ex,
-                         int64_t* rank_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
-                         cudaStream_t st) {
+                         int64_t* rank_out, int32_t* error_flag, const RetrieveWorkspace& w, cudaStream_t st) {
   if (n_queries == 0) return RECNN_OK;
-  const RetrieveWorkspace w = retrieve_carve(n_queries, n_items, 0, workspace);
-  RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
   const long long* tgt = reinterpret_cast<const long long*>(target);
   long long* rank = reinterpret_cast<long long*>(rank_out);
   rank_init_kernel<<<(unsigned)ceil_div(n_queries, 256), 256, 0, st>>>(tgt, n_queries, n_items, rank, error_flag);
@@ -292,9 +309,12 @@ static int retrieve_rank(const float* queries, int64_t n_queries, int32_t dim, c
 extern "C" int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
                                    int64_t n_items, const float* norms, int32_t metric, int32_t k, int64_t* ids_out,
                                    float* dist_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  RetrieveWorkspace w{};
+  RECNN_PROPAGATE(retrieve_topk_check(queries, n_queries, dim, table, n_items, norms, metric, k, ids_out, dist_out,
+                                      workspace, workspace_bytes, &w));
   const ItemSets none = {nullptr, nullptr, nullptr, 0, 0, 0};
-  return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, none, ids_out, dist_out, workspace,
-                  workspace_bytes, static_cast<cudaStream_t>(stream));
+  return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, none, ids_out, dist_out, w,
+                  static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
@@ -302,13 +322,15 @@ extern "C" int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries,
                                         const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
                                         int64_t n_sets, const int64_t* row_set, int64_t* ids_out, float* dist_out,
                                         int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream) {
+  RetrieveWorkspace w{};
+  RECNN_PROPAGATE(retrieve_topk_check(queries, n_queries, dim, table, n_items, norms, metric, k, ids_out, dist_out,
+                                      workspace, workspace_bytes, &w));
   ItemSets ex;
   RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_queries, error_flag, &ex));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
   if (n_queries > 0) RECNN_PROPAGATE(item_sets_check(ex, n_queries, n_items, error_flag, st));
-  return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, ex, ids_out, dist_out, workspace,
-                  workspace_bytes, st);
+  return retrieve(queries, n_queries, dim, table, n_items, norms, metric, k, ex, ids_out, dist_out, w, st);
 }
 
 extern "C" int64_t recnn_retrieve_rank_workspace_bytes(int64_t n_queries, int64_t n_items) {
@@ -320,13 +342,14 @@ extern "C" int recnn_retrieve_rank(const float* queries, int64_t n_queries, int3
                                    int64_t n_items, const float* norms, int32_t metric, const int64_t* target,
                                    int64_t* rank_out, int32_t* error_flag, void* workspace, int64_t workspace_bytes,
                                    void* stream) {
-  RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
-  RECNN_REQUIRE(target && rank_out && error_flag, "null pointer");
+  RetrieveWorkspace w{};
+  RECNN_PROPAGATE(retrieve_rank_check(queries, n_queries, dim, table, n_items, norms, metric, target, rank_out,
+                                      error_flag, workspace, workspace_bytes, &w));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
   const ItemSets none = {nullptr, nullptr, nullptr, 0, 0, 0};
-  return retrieve_rank(queries, n_queries, dim, table, n_items, norms, metric, target, none, rank_out, error_flag,
-                       workspace, workspace_bytes, st);
+  return retrieve_rank(queries, n_queries, dim, table, n_items, norms, metric, target, none, rank_out, error_flag, w,
+                       st);
 }
 
 extern "C" int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
@@ -334,13 +357,13 @@ extern "C" int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries,
                                         const int64_t* set_ids, int64_t n_set_ids, const int64_t* set_offsets,
                                         int64_t n_sets, const int64_t* row_set, int64_t* rank_out,
                                         int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream) {
-  RECNN_PROPAGATE(retrieve_check(queries, n_queries, dim, table, n_items, norms, metric, workspace));
-  RECNN_REQUIRE(target && rank_out, "null pointer");
+  RetrieveWorkspace w{};
+  RECNN_PROPAGATE(retrieve_rank_check(queries, n_queries, dim, table, n_items, norms, metric, target, rank_out,
+                                      error_flag, workspace, workspace_bytes, &w));
   ItemSets ex;
   RECNN_PROPAGATE(item_sets_args(set_ids, n_set_ids, set_offsets, n_sets, row_set, n_queries, error_flag, &ex));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
   if (n_queries > 0) RECNN_PROPAGATE(item_sets_check(ex, n_queries, n_items, error_flag, st));
-  return retrieve_rank(queries, n_queries, dim, table, n_items, norms, metric, target, ex, rank_out, error_flag,
-                       workspace, workspace_bytes, st);
+  return retrieve_rank(queries, n_queries, dim, table, n_items, norms, metric, target, ex, rank_out, error_flag, w, st);
 }
