@@ -399,6 +399,35 @@ RECNN_API int recnn_slate_distances(const int64_t* ids, int64_t n_rows, int32_t 
                                     int64_t n_items, int32_t dim, int32_t metric, float* mean_out, float* min_out,
                                     int32_t* count_out, float* matrix_out, int32_t* error_flag, void* stream);
 
+/* ---- serving: diversified re-ranking of each row's candidate pool ------------------------------------
+ * Greedy MMR (Carbonell & Goldstein, 1998) or greedy DPP MAP inference (Chen, Zhang & Zhou, NeurIPS 2018) over a scored
+ * pool, e.g. the output of a top-k, sampled top-k, critic or search call, against the resident table:
+ *   ids int64 [n_rows, m] (1 <= m <= 256; -1 = padding), scores fp32 [n_rows, m] (relevance, higher is better);
+ *   table fp32 [n_items, dim] row-major, 1 <= dim <= 1024; 1 <= k <= min(64, m); weight in [0, 1]:
+ *   1 = relevance only, 0 = diversity only.
+ * Outputs, [n_rows, k] each, in selection order: ids_out the slate, pos_out each pick's pool column, gain_out the
+ * objective at selection; unfilled positions hold -1 / -1 / NaN.
+ * Similarity: cosine, sim(a, b) = a.b / (|a| |b|) clipped to [-1, 1], 0 with a zero vector (1 - the cosine distance of
+ * recnn_slate_distances); norms in the same fma order as the dot products, so a repeated item has sim exactly 1.
+ * A slot is eligible while its id >= 0 and that id has not been selected: a slate never repeats an id, even when the
+ * pool does.  Ties go to the smaller id, then the smaller column.
+ *   MMR: step t picks the eligible i maximising weight s_i - (1 - weight) max_{j in S} sim(i, j) (penalty 0 at t = 0);
+ *        gain = that objective.
+ *   DPP: L = Diag(q) S Diag(q), S_ij = (1 + sim_ij) / 2, q_i = exp(alpha s_i), alpha = weight / (2 (1 - weight)).  The
+ *        paper's incremental Cholesky (c-vectors, d^2) runs on S alone (chol(Diag(q) S Diag(q)) = Diag(q) chol(S)), so
+ *        q is never formed: pick argmax 2 alpha s_i + log d_i^2, stop when the chosen d^2 < 1e-4 and pad the rest.
+ *        gain = 2 alpha s_j + log d_j^2, the increase of log det L_S.  At weight = 1 the DPP orders by score (gain =
+ *        the score, no stopping rule).  S has rank <= dim + 1, so a DPP slate holds at most dim + 1 items.
+ * *error_flag: bit 1 = an id outside [-1, n_items) (that slot is read as padding), bit 2 = a non-finite score on a
+ * filled slot.  A row's outputs depend only on its own ids, scores and the table, bit for bit: across repeats, batch
+ * composition, row order, launch plan and appended -1 columns.
+ * No workspace, nothing allocated: graph-capturable. */
+enum { RECNN_DIVERSIFY_MMR = 0, RECNN_DIVERSIFY_DPP = 1 };
+RECNN_API int recnn_slate_diversify(const int64_t* ids, const float* scores, int64_t n_rows, int32_t m, int32_t k,
+                                    const float* table, int64_t n_items, int32_t dim, int32_t method, float weight,
+                                    int64_t* ids_out, int64_t* pos_out, float* gain_out,
+                                    int32_t* error_flag, void* stream);
+
 /* ---- serving: items scored by the DDPG / TD3 critic (the Wolpertinger policy) ------------------------
  * Q(s_r, e_j) = critic(state[r], table[j]) in eval mode (no dropout), params a Critic arena of dims d (TD3: value_net1),
  * table fp32 [n_items, d->action_dim] dense, state fp32 [n_rows, d->state_dim] dense.  The columns of a row are its

@@ -156,6 +156,9 @@ SIGNATURES = {
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "recnn_slate_distances": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "recnn_slate_diversify": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
+                                        C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
     "recnn_critic_serve_workspace_bytes": (C.c_int64, [C.POINTER(Dims), C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                                        C.c_int32]),
     "recnn_critic_topk": (C.c_int, [C.POINTER(Dims), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,

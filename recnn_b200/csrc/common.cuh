@@ -138,6 +138,12 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return t;
 }
 
+// 16-byte global -> shared copy that bypasses the registers (cp.async; both addresses 16-byte aligned)
+__device__ __forceinline__ void cp_async16(float* dst, const float* src) {
+  const unsigned s = (unsigned)__cvta_generic_to_shared(dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(src) : "memory");
+}
+
 // ---- Philox4x32-10 (perf-mode dropout / TD3 noise) ---------------------------
 struct Philox {
   uint32_t key0, key1;

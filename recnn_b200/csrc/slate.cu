@@ -46,11 +46,6 @@ static SlatePlan slate_plan(int k) {
   return p;
 }
 
-__device__ __forceinline__ void cp_async16(float* dst, const float* src) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(src) : "memory");
-}
-
 __device__ __forceinline__ float slate_nan() { return __int_as_float(0x7fffffff); }
 
 // acc: the sum of squared differences (EUCLIDEAN) or the dot product (COSINE); na, nb the squared norms (COSINE)
