@@ -372,6 +372,92 @@ RECNN_API int recnn_retrieve_rank_sets(const float* queries, int64_t n_queries, 
                                        int64_t n_sets, const int64_t* row_set, int64_t* rank_out,
                                        int32_t* error_flag, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- serving: approximate nearest-item search through an inverted-file index (IVF_FLAT) ---------------
+ * The index the reference's MilvusConnection.search addresses with search_param {"nprobe": 16}
+ * (recnn/data/db_con.py:45-56), built on the device from the resident table and searched there.
+ *
+ * The index's arrays travel in one descriptor, and the build and the search take their arguments as one struct each, as
+ * recnn_ddpg_step and recnn_beta_step do (recnn_sizeof_* / recnn_offsetof_* let a foreign binding verify its mirror).
+ *
+ * recnn_ivf_index: the lists, as recnn_ivf_build writes them and recnn_ivf_search reads them.
+ *   n_items < 2^31, dim, metric (RECNN_METRIC_*), nlist describe the table [n_items, dim] the index was built over;
+ *   centroids fp32 [nlist, dim]; centroid_norms fp32 [nlist] (recnn_item_norms of the centroids; NULL for IP);
+ *   list_offsets int64 [nlist + 1]; list_ids int64 [n_items], ascending within each list;
+ *   list_table fp32 [n_items, pitch], 16-byte aligned, pitch = dim rounded up to a multiple of 4 (pad columns 0): the
+ *   rows in list order; list_norms fp32 [n_items] (NULL for IP): recnn_item_norms in list order. */
+typedef struct recnn_ivf_index {
+  int64_t n_items;
+  int32_t dim, metric, nlist, reserved;
+  float* centroids;
+  float* centroid_norms;
+  int64_t* list_offsets;
+  int64_t* list_ids;
+  float* list_table;
+  float* list_norms;
+} recnn_ivf_index;
+RECNN_API int64_t recnn_sizeof_ivf_index(void);
+
+/* recnn_ivf_build: Lloyd k-means, then the inverted lists, written into args->index.
+ *   sample_ids int64 [n_sample] (items of the training sample, host-chosen), init int64 [nlist] (positions in the sample
+ *   of the initial centroids); nlist <= n_sample <= n_items.  n_iter >= 0 rounds of: every sample point to its nearest
+ *   centroid in L2 (recnn_retrieve_topk, ties to the smaller id), each centroid the mean of its members summed in fp64 in
+ *   ascending point order, then each empty list, in ascending id, splits the list of the largest count (ties: smaller id)
+ *   as faiss does: the empty one takes the donor's centroid with even dims * (1 + 1/1024) and odd dims * (1 - 1/1024),
+ *   the donor the opposite, and the donor's count is halved between the two.  COS trains on unit rows and renormalises
+ *   the centroids after each round (spherical k-means); L2 and IP train in L2 on the raw rows.  Finally every item goes
+ *   to its nearest centroid (COS: the largest cosine) and every array of the index is written.  The same inputs give the
+ *   same bits.  workspace_bytes >= recnn_ivf_build_workspace_bytes (else RECNN_E_WORKSPACE, before any device work). */
+typedef struct recnn_ivf_build_args {
+  recnn_ivf_index index;      /* sizes in, arrays out */
+  const float* table;         /* [n_items, dim] */
+  const int64_t* sample_ids;  /* [n_sample] */
+  int64_t n_sample;
+  const int64_t* init;        /* [nlist] */
+  int32_t n_iter, reserved;
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_ivf_build_args;
+RECNN_API int64_t recnn_sizeof_ivf_build_args(void);
+RECNN_API int64_t recnn_offsetof_ivf_build_args(int field);
+RECNN_API int64_t recnn_ivf_build_workspace_bytes(int64_t n_items, int32_t dim, int32_t nlist, int64_t n_sample);
+RECNN_API int recnn_ivf_build(const recnn_ivf_build_args* args, void* stream);
+/* The list table and list norms of recnn_ivf_build for given list_ids (a permutation of [0, n_items), not checked here):
+ * rebuilds a saved index from its ids and the table.  No workspace. */
+RECNN_API int recnn_ivf_list_table(const float* table, int64_t n_items, int32_t dim, int32_t metric,
+                                   const int64_t* list_ids, float* list_table_out, float* list_norms_out, void* stream);
+
+/* recnn_ivf_search: the k best items of each query among the lists of its nprobe nearest centroids.
+ *   coarse: recnn_retrieve_topk over the centroids with the index's metric, k = nprobe (1 <= nprobe <= min(nlist, 64));
+ *   fine: every item of the probed lists, key as recnn_retrieve_topk (L2 |x|^2 - 2 q.x, IP -q.x, COS -q.x / |x|) from an
+ *   fp32 fma dot product in ascending d, ties to the smaller id; distances reported as recnn_retrieve_topk reports them.
+ *   A (query, item) key is the same bits whatever queries share the call and whichever list tile computes it, so the
+ *   result is the exact top-k of the union of the probed lists.  A query whose probed lists hold fewer than k eligible
+ *   items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  queries fp32 [n_queries, dim], 1 <= dim <= 512,
+ *   1 <= k <= min(64, n_items); ids_out int64 / dist_out fp32 [n_queries, k].  Exclusion: set_offsets NULL for none,
+ *   else the set table of recnn_retrieve_topk_sets with its error bits in *error_flag.
+ *   workspace_bytes >= recnn_ivf_search_workspace_bytes (else RECNN_E_WORKSPACE, before any device work); it does not
+ *   depend on the lists. */
+typedef struct recnn_ivf_search_args {
+  recnn_ivf_index index;      /* read only */
+  const float* queries;
+  int64_t n_queries;
+  int32_t nprobe, k;
+  const int64_t* set_ids;
+  int64_t n_set_ids;
+  const int64_t* set_offsets;
+  int64_t n_sets;
+  const int64_t* row_set;
+  int64_t* ids_out;
+  float* dist_out;
+  int32_t* error_flag;
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_ivf_search_args;
+RECNN_API int64_t recnn_sizeof_ivf_search_args(void);
+RECNN_API int64_t recnn_offsetof_ivf_search_args(int field);
+RECNN_API int64_t recnn_ivf_search_workspace_bytes(int64_t n_queries, int32_t nlist, int32_t nprobe, int32_t k);
+RECNN_API int recnn_ivf_search(const recnn_ivf_search_args* args, void* stream);
+
 /* ---- offline evaluation: distances between the items of each served slate ---------------------------
  * The reference's diversity test: examples/streamlit_demo.py:355-445 ("Test Diversity") draws heatmaps of
  * recnn/utils/plot.py:9-35 pairwise_distances_fig, i.e. scipy cdist(..., "cosine") and cdist(..., "euclidean") over

@@ -14,8 +14,17 @@ the reference's accessors ``.id(device)`` / ``.dist(device)``; ``exclude=`` an
 results (recnn_retrieve_topk_sets).
 ``MilvusConnection(env, ...)`` keeps the reference's constructor shape for code
 written against recnn.data.db_con.
+
+``ItemIndex.build_ivf(nlist)`` adds an inverted-file index (IVF_FLAT, as Milvus
+and faiss name it), built on the device: k-means lists over the table, after
+which ``search(..., search_param={"nprobe": p})`` scans only the lists of each
+query's p nearest centroids (recnn_ivf_build / recnn_ivf_search).  ``rank``
+stays exact, so recall can be measured against it or against a flat index.
 """
 from __future__ import annotations
+
+import ctypes
+from typing import NamedTuple
 
 import torch
 
@@ -37,11 +46,38 @@ class SearchResult:
         return self.distances if device is None else self.distances.to(device)
 
 
+IVF_MAX_DIM = 512          # the fine scan stages a tile of queries and two chunks of list rows in shared memory
+IVF_MAX_NPROBE = 64
+
+
+def ivf_sample(n_items, nlist, seed=0, max_points_per_centroid=256):
+    """(sample, init), int64 CPU tensors: the k-means training sample and the positions in it of the initial centroids.
+    Every item when n_items <= nlist * max_points_per_centroid, else the first nlist * max_points_per_centroid of
+    torch.randperm(n_items) drawn from torch.Generator().manual_seed(seed); init is the first nlist of a second
+    randperm(len(sample)) from the same generator."""
+    g = torch.Generator().manual_seed(int(seed))
+    cap = int(nlist) * int(max_points_per_centroid)
+    sample = torch.randperm(n_items, generator=g)[:cap] if n_items > cap else torch.arange(n_items)
+    init = torch.randperm(len(sample), generator=g)[:nlist]
+    return sample.to(torch.int64), init.to(torch.int64)
+
+
+class IVFLists(NamedTuple):
+    """The inverted lists of an ItemIndex: list l holds list_ids[list_offsets[l]:list_offsets[l + 1]], ascending, around
+    centroids[l].  The tensors are the index's own device storage: read them, do not write them."""
+    centroids: torch.Tensor      # fp32 [nlist, dim]
+    list_offsets: torch.Tensor   # int64 [nlist + 1]
+    list_ids: torch.Tensor       # int64 [n_items]
+
+
 class ItemIndex:
     """Exact top-k search over an item-embedding matrix resident on one GPU.
 
     metric: "L2" (squared Euclidean distance, smallest first -- faiss IndexFlatL2 / Milvus L2),
             "IP" (inner product, largest first), "COS" (cosine similarity, largest first).
+
+    ``build_ivf`` turns ``search`` into an IVF_FLAT search (see there); the index is a snapshot of the table at build
+    time, which RecNN's workflows keep fixed.
     """
 
     def __init__(self, embeddings, metric="L2"):
@@ -63,14 +99,163 @@ class ItemIndex:
                 _lib.check(_lib.lib().recnn_item_norms(self.table.data_ptr(), self.n_items, self.dim, self.metric,
                                                        self.norms.data_ptr(), _lib.stream_ptr(self.device)))
         self._ws = None
+        self._ivf = None
+
+    # ------------------------------------------------------------------------------------------------ IVF index
+    @property
+    def ivf(self):
+        """None, or the IVFLists (centroids, list_offsets, list_ids) of the index built by build_ivf / load_ivf."""
+        if self._ivf is None:
+            return None
+        return IVFLists(self._ivf["centroids"], self._ivf["list_offsets"], self._ivf["list_ids"])
+
+    def build_ivf(self, nlist, n_iter=25, seed=0, max_points_per_centroid=256):
+        """Build an inverted-file index (IVF_FLAT) over the table on the device and return self.
+
+        k-means (Lloyd, ``n_iter`` rounds) on a sample of at most ``nlist * max_points_per_centroid`` items chosen by
+        ``ivf_sample(n_items, nlist, seed, ...)``, initialised at ``nlist`` of its points; empty lists are split as
+        faiss does.  COS runs spherical k-means on unit rows, L2 and IP k-means in L2 on the raw rows.  Every item then
+        goes to the list of its nearest centroid.  The same table and arguments give the same index, bit for bit.
+
+        The index stores the table a second time, in list order (what IVF_FLAT stores): ``n_items * dim * 4`` bytes, 1 GB
+        at 1M x 256, plus the ids and norms.  It is a snapshot of the table at build time."""
+        nlist, n_iter, mppc = int(nlist), int(n_iter), int(max_points_per_centroid)
+        if not 1 <= nlist <= self.n_items:
+            raise ValueError("nlist must be in [1, n_items = %d] (got %d)" % (self.n_items, nlist))
+        if n_iter < 0:
+            raise ValueError("n_iter must be >= 0 (got %d)" % n_iter)
+        if mppc < 1:
+            raise ValueError("max_points_per_centroid must be >= 1 (got %d)" % mppc)
+        if self.dim > IVF_MAX_DIM:
+            raise ValueError("an IVF index supports dim <= %d (got %d)" % (IVF_MAX_DIM, self.dim))
+        sample, init = ivf_sample(self.n_items, nlist, seed, mppc)
+        dev = self.device
+        sample, init = sample.to(dev), init.to(dev)
+        ivf = self._ivf_buffers(nlist)
+        L = _lib.lib()
+        ws = torch.empty(L.recnn_ivf_build_workspace_bytes(self.n_items, self.dim, nlist, len(sample)),
+                         dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            args = _lib.IvfBuildArgs(self._ivf_descriptor(ivf), self.table.data_ptr(), sample.data_ptr(), len(sample),
+                                     init.data_ptr(), n_iter, 0, ws.data_ptr(), ws.numel())
+            _lib.check(L.recnn_ivf_build(ctypes.byref(args), _lib.stream_ptr(dev)))
+        del ws
+        ivf["params"] = dict(nlist=nlist, n_iter=n_iter, seed=int(seed), max_points_per_centroid=mppc)
+        self._ivf_finish(ivf)
+        return self
+
+    def _ivf_buffers(self, nlist):
+        dev, pitch = self.device, (self.dim + 3) // 4 * 4
+        norms = self.metric != _lib.METRIC_IP
+        return dict(centroids=torch.empty(nlist, self.dim, dtype=torch.float32, device=dev),
+                    centroid_norms=torch.empty(nlist, dtype=torch.float32, device=dev) if norms else None,
+                    list_offsets=torch.empty(nlist + 1, dtype=torch.int64, device=dev),
+                    list_ids=torch.empty(self.n_items, dtype=torch.int64, device=dev),
+                    list_table=torch.empty(self.n_items, pitch, dtype=torch.float32, device=dev),
+                    list_norms=torch.empty(self.n_items, dtype=torch.float32, device=dev) if norms else None)
+
+    def _ivf_descriptor(self, ivf):
+        """the recnn_ivf_index of the buffers in ivf"""
+        return _lib.ivf_index(self.n_items, self.dim, self.metric, int(ivf["centroids"].shape[0]), ivf["centroids"],
+                              ivf["centroid_norms"], ivf["list_offsets"], ivf["list_ids"], ivf["list_table"],
+                              ivf["list_norms"])
+
+    def _ivf_finish(self, ivf):
+        ivf["nlist"] = int(ivf["centroids"].shape[0])
+        ivf["max_list_len"] = int((ivf["list_offsets"][1:] - ivf["list_offsets"][:-1]).max())
+        self._ivf = ivf
+
+    def ivf_state(self):
+        """The IVF index as host tensors and plain values, for torch.save: centroids, list_offsets, list_ids, the build
+        parameters, the metric and the table's shape.  None without an index."""
+        if self._ivf is None:
+            return None
+        return dict(centroids=self._ivf["centroids"].cpu(), list_offsets=self._ivf["list_offsets"].cpu(),
+                    list_ids=self._ivf["list_ids"].cpu(), params=dict(self._ivf["params"]), metric=self.metric_name,
+                    n_items=self.n_items, dim=self.dim)
+
+    def load_ivf(self, state):
+        """Restore an index saved by ivf_state over this index's table (the same table it was built on) and return
+        self.  The shapes and the metric must match, and list_ids must be a permutation of the items, ascending within
+        each list, with monotone offsets from 0 to n_items (checked on the device): ValueError otherwise.  The
+        list-ordered table and the norms are rebuilt from this index's table."""
+        try:
+            cent, offs, ids = state["centroids"], state["list_offsets"], state["list_ids"]
+            metric, n_items, dim = state["metric"], int(state["n_items"]), int(state["dim"])
+            params = dict(state["params"])
+        except (KeyError, TypeError) as e:
+            raise ValueError("not an ivf_state() dict: %s" % e)
+        if metric != self.metric_name:
+            raise ValueError("the index was built for metric %s, this ItemIndex is %s" % (metric, self.metric_name))
+        if (n_items, dim) != (self.n_items, self.dim):
+            raise ValueError("the index was built over a [%d, %d] table, this one is [%d, %d]"
+                             % (n_items, dim, self.n_items, self.dim))
+        if self.dim > IVF_MAX_DIM:
+            raise ValueError("an IVF index supports dim <= %d (got %d)" % (IVF_MAX_DIM, self.dim))
+        if not all(torch.is_tensor(t) for t in (cent, offs, ids)):
+            raise ValueError("centroids, list_offsets and list_ids must be tensors")
+        nlist = int(cent.shape[0]) if cent.dim() == 2 else -1
+        if (cent.dim() != 2 or cent.shape[1] != dim or not 1 <= nlist <= n_items or not cent.dtype.is_floating_point
+                or tuple(offs.shape) != (nlist + 1,) or tuple(ids.shape) != (n_items,)
+                or offs.dtype != torch.int64 or ids.dtype != torch.int64):
+            raise ValueError("malformed ivf state: centroids [nlist, %d] float, list_offsets int64 [nlist + 1], "
+                             "list_ids int64 [%d]" % (dim, n_items))
+        dev = self.device
+        offs, ids = offs.to(dev).contiguous(), ids.to(dev).contiguous()
+        counts = offs[1:] - offs[:-1]
+        ok = bool(offs[0] == 0) and bool(offs[-1] == n_items) and bool((counts >= 0).all())
+        if ok:
+            ok = bool(((ids >= 0) & (ids < n_items)).all())
+        if ok:
+            ok = bool((torch.bincount(ids, minlength=n_items) == 1).all())
+        if ok and n_items > 1:
+            # ascending inside a list: a descent is allowed only where a new list starts
+            starts = torch.zeros(n_items, dtype=torch.bool, device=dev)
+            starts[offs[1:-1][offs[1:-1] < n_items]] = True
+            ok = bool(((ids[1:] > ids[:-1]) | starts[1:]).all())
+        if not ok:
+            raise ValueError("malformed ivf state: list_ids must be a permutation of [0, %d), ascending within each "
+                             "list, and list_offsets monotone from 0 to %d" % (n_items, n_items))
+        ivf = self._ivf_buffers(nlist)
+        ivf["centroids"].copy_(cent.to(device=dev, dtype=torch.float32))
+        ivf["list_offsets"].copy_(offs)
+        ivf["list_ids"].copy_(ids)
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            if ivf["centroid_norms"] is not None:
+                _lib.check(L.recnn_item_norms(ivf["centroids"].data_ptr(), nlist, self.dim, self.metric,
+                                              ivf["centroid_norms"].data_ptr(), _lib.stream_ptr(dev)))
+            _lib.check(L.recnn_ivf_list_table(self.table.data_ptr(), self.n_items, self.dim, self.metric,
+                                              ivf["list_ids"].data_ptr(), ivf["list_table"].data_ptr(),
+                                              _lib.ptr(ivf["list_norms"]), _lib.stream_ptr(dev)))
+        ivf["params"] = params
+        self._ivf_finish(ivf)
+        return self
+
+    def _nprobe(self, search_param):
+        nlist = self._ivf["nlist"]
+        p = dict(search_param or {})
+        unknown = sorted(set(p) - {"nprobe"})
+        if unknown:
+            raise ValueError("unknown search_param keys %s (an IVF index takes only nprobe)" % unknown)
+        nprobe = int(p.get("nprobe", min(16, nlist)))
+        if not 1 <= nprobe <= min(nlist, IVF_MAX_NPROBE):
+            raise ValueError("nprobe must be in [1, min(nlist = %d, %d)] (got %d)" % (nlist, IVF_MAX_NPROBE, nprobe))
+        return nprobe
 
     def search(self, search_vecs, topk=10, search_param=None, exclude=None, exclude_rows=None):
         """search_vecs: [n, dim] (tensor / array on any device).  Returns SearchResult on the index's device.
         ``exclude``: an ``ItemSets`` of item ids never returned (e.g. ``DeviceFrameFeed.seen_items()``), with
         ``exclude_rows`` int64 [n] naming each query's set (-1: none; default query r -> set r).  A query with fewer
         than topk eligible items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  An excluded id outside
-        [0, n_items) raises IndexError, a malformed table ValueError."""
+        [0, n_items) raises IndexError, a malformed table ValueError.
+
+        Without an IVF index the search is exact and ``search_param`` is ignored.  After ``build_ivf`` / ``load_ivf``
+        it is the IVF_FLAT search: ``search_param={"nprobe": p}`` (default 16, at most min(nlist, 64); any other key
+        raises ValueError) scans the lists of each query's p nearest centroids, and the result is the exact top-k over
+        those lists -- the same for a query whatever other queries share the call."""
         from .item_sets import ItemSets, row_map
+        nprobe = self._nprobe(search_param) if self._ivf is not None else None
         q = torch.as_tensor(search_vecs)
         if q.dim() == 1:
             q = q.unsqueeze(0)
@@ -93,6 +278,8 @@ class ItemIndex:
         if n == 0:
             return SearchResult(ids, dist)
         L = _lib.lib()
+        if nprobe is not None:
+            return self._ivf_search(q, n, topk, nprobe, sets, rows)
         need = L.recnn_retrieve_workspace_bytes(n, self.n_items, topk)
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
@@ -110,18 +297,44 @@ class ItemIndex:
                                                   _lib.ptr(rows), ids.data_ptr(), dist.data_ptr(), flag.data_ptr(),
                                                   self._ws.data_ptr(), self._ws.numel(),
                                                   _lib.stream_ptr(self.device)))
-        bits = int(flag.item())
+        self._raise_set_bits(int(flag.item()), len(sets))
+        return SearchResult(ids, dist)
+
+    def _raise_set_bits(self, bits, n_sets):
         if bits & 1:
             raise IndexError("an excluded item id is out of range for the index's %d items" % self.n_items)
         if bits & 4:
             raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
-                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % len(sets))
+                             "decreasing, or an exclude_rows entry is outside [-1, %d)" % n_sets)
+
+    def _ivf_search(self, q, n, topk, nprobe, sets, rows):
+        L, iv, dev = _lib.lib(), self._ivf, self.device
+        ids = torch.empty(n, topk, dtype=torch.int64, device=dev)
+        dist = torch.empty(n, topk, dtype=torch.float32, device=dev)
+        need = L.recnn_ivf_search_workspace_bytes(n, iv["nlist"], nprobe, topk)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        set_args, flag = (None, 0, None, 0, None), None
+        if sets is not None:
+            sets = sets.to(dev)
+            rows = None if rows is None else rows.to(dev).contiguous()
+            flag = torch.empty(1, dtype=torch.int32, device=dev)
+            set_args = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
+                        len(sets), _lib.ptr(rows))
+        with torch.cuda.device(dev):
+            args = _lib.IvfSearchArgs(self._ivf_descriptor(iv), q.data_ptr(), n, nprobe, topk, *set_args,
+                                      ids.data_ptr(), dist.data_ptr(), _lib.ptr(flag), self._ws.data_ptr(),
+                                      self._ws.numel())
+            _lib.check(L.recnn_ivf_search(ctypes.byref(args), _lib.stream_ptr(dev)))
+        if flag is not None:
+            self._raise_set_bits(int(flag.item()), len(sets))
         return SearchResult(ids, dist)
 
     def rank(self, search_vecs, target, exclude=None, exclude_rows=None):
         """int64 [n]: for offline evaluation, the number of items ``search`` on the same queries would return before
         ``target[q]`` (better key, equal keys the smaller id), i.e. the target's position in ``search(vecs, k)`` when
-        below k and the target is absent otherwise, at any k.  ``exclude`` / ``exclude_rows`` as in ``search``; a
+        below k and the target is absent otherwise, at any k.  Ranks are always the exact ones, also on an index with
+        IVF lists, so the recall of an ``nprobe`` can be measured against them.  ``exclude`` / ``exclude_rows`` as in ``search``; a
         query's target is never excluded.  DDPG / TD3: ``index.rank(actor(state), target, ...)``.  A target or
         excluded id outside [0, n_items) raises IndexError, a malformed table ValueError."""
         from .item_sets import ItemSets, row_map
@@ -178,15 +391,25 @@ class ItemIndex:
 
 class MilvusConnection(ItemIndex):
     """Constructor shape of recnn.data.db_con.MilvusConnection(env, name=..., port=..., param=...): the collection
-    is ``env.base.embeddings``; ``param["metric_type"]`` may be "L2" (default) or "IP".  No Milvus server is involved."""
+    is ``env.base.embeddings``; ``param["metric_type"]`` may be "L2" (default) or "IP".  ``param["index_type"]``
+    "IVF_FLAT" with ``param["nlist"]`` builds the IVF index at construction (Milvus create_index(IVF_FLAT, {"nlist"})),
+    so that ``search(..., search_param={"nprobe": p})`` means what it means to Milvus; without it, or with "FLAT", the
+    search is exact.  No Milvus server is involved."""
 
     def __init__(self, env, name="movies_L2", port="19530", param=None):
         metric = "L2"
         if param and "metric_type" in param:
             mt = str(param["metric_type"]).upper()
             metric = "IP" if mt.endswith("IP") else "L2"
+        index_type = str(param.get("index_type", "FLAT")).upper() if param else "FLAT"
+        if index_type not in ("FLAT", "IVF_FLAT"):
+            raise ValueError("index_type must be FLAT or IVF_FLAT (got %s)" % index_type)
+        if index_type == "IVF_FLAT" and "nlist" not in param:
+            raise ValueError("index_type IVF_FLAT needs param['nlist']")
         emb = env.base.embeddings if hasattr(env, "base") else env
         super().__init__(emb, metric)
+        if index_type == "IVF_FLAT":
+            self.build_ivf(int(param["nlist"]))
         self.name = name
         self.statuses = {}
 

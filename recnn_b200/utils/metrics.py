@@ -13,6 +13,8 @@ Pure torch on the ranks' device; ``ranking_metrics(..., group=)`` all-reduces th
 ``off_policy_estimates`` estimates the reward the policy pi would earn from logged rows (s, a, r) of the behaviour
 policy beta, with the Top-K off-policy correction's importance weights (DESIGN.md, 4d-ope).
 
+``recall_at_k`` compares an approximate search's ids (an IVF ``nprobe``) with the exact ones.
+
 ``slate_distances`` and ``slate_metrics`` describe served slates as sets (DESIGN.md, 4d-diversity).  ``ids`` is the
 int64 [N, k] output of any serving call (``DiscreteActor.topk`` / ``sample_topk``, ``ItemIndex.search``,
 ``Critic.topk``), -1 marking an empty slot; a filled slot is an id >= 0.  With c_j the number of filled slots that
@@ -82,6 +84,29 @@ def mrr(ranks):
     """Mean reciprocal rank."""
     r = _ranks(ranks)
     return float((1.0 / (r + 1.0)).mean()) if r.numel() else float("nan")
+
+
+def recall_at_k(approx_ids, exact_ids):
+    """(per_row, mean): the recall of an approximate search against the exact one, e.g. ``ItemIndex.search`` with an
+    IVF ``nprobe`` against a flat index or ``rank``.  approx_ids and exact_ids are int64 [n, k] (-1 pads an empty slot).
+    per_row float64 [n] = |approx_r & exact_r| / |exact_r| over the filled slots (-1 ignored on both sides; NaN for a
+    row whose exact slots are all empty); mean = the mean over the rows that are not NaN (NaN when there are none)."""
+    a, e = torch.as_tensor(approx_ids), torch.as_tensor(exact_ids)
+    for x, name in ((a, "approx_ids"), (e, "exact_ids")):
+        if x.dim() != 2 or x.dtype.is_floating_point or x.dtype.is_complex or x.dtype == torch.bool:
+            raise ValueError("%s must be a 2-D integer tensor [n, k] (got %s %s)" % (name, tuple(x.shape), x.dtype))
+    if a.shape[0] != e.shape[0]:
+        raise ValueError("approx_ids and exact_ids must have the same rows (got %d and %d)" % (a.shape[0], e.shape[0]))
+    a = a.to(device=e.device, dtype=torch.int64)
+    e = e.to(torch.int64)
+    valid_e = e >= 0
+    hit = ((e[:, :, None] == a[:, None, :]) & (a[:, None, :] >= 0)).any(2) & valid_e
+    n_e = valid_e.sum(1).double()
+    per_row = hit.sum(1).double() / n_e
+    per_row[n_e == 0] = float("nan")
+    ok = ~torch.isnan(per_row)
+    mean = float(per_row[ok].mean()) if bool(ok.any()) else float("nan")
+    return per_row, mean
 
 
 def ranking_metrics(ranks, ks=(1, 5, 10, 20), group=None):
