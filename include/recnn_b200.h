@@ -458,6 +458,100 @@ RECNN_API int64_t recnn_offsetof_ivf_search_args(int field);
 RECNN_API int64_t recnn_ivf_search_workspace_bytes(int64_t n_queries, int32_t nlist, int32_t nprobe, int32_t k);
 RECNN_API int recnn_ivf_search(const recnn_ivf_search_args* args, void* stream);
 
+/* ---- serving: the IVF index with product-quantized lists (IVF_PQ) --------------------------------------
+ * The coarse lists of IVF_FLAT (the same build code, so the same bits) with each item stored as m one-byte codes of its
+ * residual from its list's centroid instead of a list-ordered copy of its row.  Subspace j is dims
+ * [j * dsub, (j + 1) * dsub), dsub = dim / m; codebook j holds 256 codewords of dsub floats.
+ *
+ * recnn_ivf_pq_index: centroids, centroid_norms, list_offsets, list_ids as in recnn_ivf_index;
+ *   1 <= m <= 64, m divides dim; codebooks fp32 [m, 256, dim / m]; codes uint8 [n_items, code_pitch] in list order,
+ *   16-byte aligned, code_pitch = m rounded up to a multiple of 16 (pad bytes 0). */
+typedef struct recnn_ivf_pq_index {
+  int64_t n_items;
+  int32_t dim, metric, nlist, m;
+  float* centroids;
+  float* centroid_norms;
+  int64_t* list_offsets;
+  int64_t* list_ids;
+  float* codebooks;
+  uint8_t* codes;
+} recnn_ivf_pq_index;
+RECNN_API int64_t recnn_sizeof_ivf_pq_index(void);
+
+/* recnn_ivf_pq_build: the coarse lists exactly as recnn_ivf_build (sample_ids, n_sample, init, n_iter as there), then
+ * the codebooks and the codes.  The residual of an item is x - c_list(x) (COS: the unit row).  Codebook training runs on
+ * the residuals of the first n_train = min(n_sample, 65536) sample points, from the codewords pq_init int64 [256]
+ * (positions in [0, n_train), the same for every subspace), n_iter Lloyd rounds per subspace with the coarse build's
+ * rounds (recnn_retrieve_topk assignment at dim dsub, fp64 ordered means, the deterministic empty-list split).  Codes as
+ * recnn_ivf_pq_encode.  n_train >= 256.  The same inputs give the same bits.
+ * workspace_bytes >= recnn_ivf_pq_build_workspace_bytes (else RECNN_E_WORKSPACE, before any device work). */
+typedef struct recnn_ivf_pq_build_args {
+  recnn_ivf_pq_index index;   /* sizes in, arrays out */
+  const float* table;         /* [n_items, dim] */
+  const int64_t* sample_ids;  /* [n_sample] */
+  int64_t n_sample;
+  const int64_t* init;        /* [nlist] */
+  const int64_t* pq_init;     /* [256] */
+  int32_t n_iter, reserved;
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_ivf_pq_build_args;
+RECNN_API int64_t recnn_sizeof_ivf_pq_build_args(void);
+RECNN_API int64_t recnn_offsetof_ivf_pq_build_args(int field);
+RECNN_API int64_t recnn_ivf_pq_build_workspace_bytes(int64_t n_items, int32_t dim, int32_t nlist, int64_t n_sample,
+                                                     int32_t m);
+RECNN_API int recnn_ivf_pq_build(const recnn_ivf_pq_build_args* args, void* stream);
+
+/* recnn_ivf_pq_encode: index->codes from the table, the lists, the centroids and the codebooks (a saved index is
+ * restored this way).  Each code is the argmin over the 256 codewords of sum_t (r_t - B_j[c]_t)^2, fp32 fma in ascending
+ * t, ties to the smaller code.  workspace_bytes >= recnn_ivf_pq_encode_workspace_bytes (a slab of residuals). */
+typedef struct recnn_ivf_pq_encode_args {
+  recnn_ivf_pq_index index;   /* codes out, the rest in */
+  const float* table;         /* [n_items, dim] */
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_ivf_pq_encode_args;
+RECNN_API int64_t recnn_sizeof_ivf_pq_encode_args(void);
+RECNN_API int64_t recnn_offsetof_ivf_pq_encode_args(int field);
+RECNN_API int64_t recnn_ivf_pq_encode_workspace_bytes(int64_t n_items, int32_t dim);
+RECNN_API int recnn_ivf_pq_encode(const recnn_ivf_pq_encode_args* args, void* stream);
+
+/* recnn_ivf_pq_search: the coarse step of recnn_ivf_search, then every item of the probed lists scored by asymmetric
+ * distance computation (ADC) from its codes, in fp32, sums in ascending order:
+ *   L2   key = sum_j LUT[j][code_j], LUT[j][c] = sum_t fma((q_jt - c_l,jt) - B_j[c]_t)^2: |q - reconstruction|^2
+ *   IP   key = -(<q, c_l> + sum_j <q_j, B_j[code_j]>)
+ *   COS  the IP form on the unit query against the unit-row reconstruction (not renormalised)
+ * ordered by (key, id).  refine = 0: the ADC top-k with distances L2 key, IP / COS -key.  refine = r >= 1: the best
+ * k' = r * k ADC candidates of each query are re-scored exactly against table with norms (recnn_item_norms of the table,
+ * L2 / COS), by the instructions of recnn_ivf_search's fine scan and merge, and the exact top-k is returned; when k'
+ * covers every eligible item of the probed lists the result is recnn_ivf_search's, bit for bit.  k' <= 64, nprobe <=
+ * min(nlist, 64), 1 <= dim <= 512.  Padding, exclusion and error bits as recnn_ivf_search.  A query's result does not
+ * depend on the other queries of the call.  workspace_bytes >= recnn_ivf_pq_search_workspace_bytes (else
+ * RECNN_E_WORKSPACE, before any device work). */
+typedef struct recnn_ivf_pq_search_args {
+  recnn_ivf_pq_index index;   /* read only */
+  const float* table;         /* [n_items, dim], refine only */
+  const float* norms;         /* [n_items] (L2 / COS), refine only */
+  const float* queries;
+  int64_t n_queries;
+  int32_t nprobe, k, refine, reserved;
+  const int64_t* set_ids;
+  int64_t n_set_ids;
+  const int64_t* set_offsets;
+  int64_t n_sets;
+  const int64_t* row_set;
+  int64_t* ids_out;
+  float* dist_out;
+  int32_t* error_flag;
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_ivf_pq_search_args;
+RECNN_API int64_t recnn_sizeof_ivf_pq_search_args(void);
+RECNN_API int64_t recnn_offsetof_ivf_pq_search_args(int field);
+RECNN_API int64_t recnn_ivf_pq_search_workspace_bytes(int64_t n_queries, int32_t nlist, int32_t nprobe, int32_t k,
+                                                      int32_t refine);
+RECNN_API int recnn_ivf_pq_search(const recnn_ivf_pq_search_args* args, void* stream);
+
 /* ---- offline evaluation: distances between the items of each served slate ---------------------------
  * The reference's diversity test: examples/streamlit_demo.py:355-445 ("Test Diversity") draws heatmaps of
  * recnn/utils/plot.py:9-35 pairwise_distances_fig, i.e. scipy cdist(..., "cosine") and cdist(..., "euclidean") over

@@ -134,6 +134,52 @@ def ivf_index(n_items, dim, metric, nlist, centroids, centroid_norms, list_offse
                     ptr(list_ids), ptr(list_table), ptr(list_norms))
 
 
+class IvfPqIndex(C.Structure):
+    _fields_ = [
+        ("n_items", C.c_int64), ("dim", C.c_int32), ("metric", C.c_int32), ("nlist", C.c_int32), ("m", C.c_int32),
+        ("centroids", C.c_void_p), ("centroid_norms", C.c_void_p), ("list_offsets", C.c_void_p),
+        ("list_ids", C.c_void_p), ("codebooks", C.c_void_p), ("codes", C.c_void_p),
+    ]
+
+
+class IvfPqBuildArgs(C.Structure):
+    _fields_ = [
+        ("index", IvfPqIndex), ("table", C.c_void_p), ("sample_ids", C.c_void_p), ("n_sample", C.c_int64),
+        ("init", C.c_void_p), ("pq_init", C.c_void_p), ("n_iter", C.c_int32), ("reserved", C.c_int32),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
+class IvfPqEncodeArgs(C.Structure):
+    _fields_ = [("index", IvfPqIndex), ("table", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_int64)]
+
+
+class IvfPqSearchArgs(C.Structure):
+    _fields_ = [
+        ("index", IvfPqIndex), ("table", C.c_void_p), ("norms", C.c_void_p), ("queries", C.c_void_p),
+        ("n_queries", C.c_int64), ("nprobe", C.c_int32), ("k", C.c_int32), ("refine", C.c_int32),
+        ("reserved", C.c_int32), ("set_ids", C.c_void_p), ("n_set_ids", C.c_int64), ("set_offsets", C.c_void_p),
+        ("n_sets", C.c_int64), ("row_set", C.c_void_p), ("ids_out", C.c_void_p), ("dist_out", C.c_void_p),
+        ("error_flag", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
+# the fields recnn_offsetof_ivf_pq_*_args(i) reports, in order
+IVF_PQ_BUILD_PROBE_FIELDS = ["index", "table", "sample_ids", "n_sample", "init", "pq_init", "n_iter", "workspace",
+                             "workspace_bytes"]
+IVF_PQ_ENCODE_PROBE_FIELDS = ["index", "table", "workspace", "workspace_bytes"]
+IVF_PQ_SEARCH_PROBE_FIELDS = ["index", "table", "norms", "queries", "n_queries", "nprobe", "k", "refine", "set_ids",
+                              "n_set_ids", "set_offsets", "n_sets", "row_set", "ids_out", "dist_out", "error_flag",
+                              "workspace", "workspace_bytes"]
+
+
+def ivf_pq_index(n_items, dim, metric, nlist, m, centroids, centroid_norms, list_offsets, list_ids, codebooks, codes):
+    """an IvfPqIndex over device tensors (None -> NULL)"""
+    return IvfPqIndex(n_items, dim, metric, nlist, m, ptr(centroids), ptr(centroid_norms), ptr(list_offsets),
+                      ptr(list_ids), ptr(codebooks), ptr(codes))
+
+
 _BETA_PROBE_FIELDS = ["dims", "n_rows", "net", "optim", "state", "action", "probs_out", "loss", "error",
                       "workspace_bytes", "n_rows_global"]
 
@@ -202,6 +248,19 @@ SIGNATURES = {
     "recnn_offsetof_ivf_search_args": (C.c_int64, [C.c_int]),
     "recnn_ivf_search_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
     "recnn_ivf_search": (C.c_int, [C.POINTER(IvfSearchArgs), C.c_void_p]),
+    "recnn_sizeof_ivf_pq_index": (C.c_int64, []),
+    "recnn_sizeof_ivf_pq_build_args": (C.c_int64, []),
+    "recnn_offsetof_ivf_pq_build_args": (C.c_int64, [C.c_int]),
+    "recnn_ivf_pq_build_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int32]),
+    "recnn_ivf_pq_build": (C.c_int, [C.POINTER(IvfPqBuildArgs), C.c_void_p]),
+    "recnn_sizeof_ivf_pq_encode_args": (C.c_int64, []),
+    "recnn_offsetof_ivf_pq_encode_args": (C.c_int64, [C.c_int]),
+    "recnn_ivf_pq_encode_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
+    "recnn_ivf_pq_encode": (C.c_int, [C.POINTER(IvfPqEncodeArgs), C.c_void_p]),
+    "recnn_sizeof_ivf_pq_search_args": (C.c_int64, []),
+    "recnn_offsetof_ivf_pq_search_args": (C.c_int64, [C.c_int]),
+    "recnn_ivf_pq_search_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "recnn_ivf_pq_search": (C.c_int, [C.POINTER(IvfPqSearchArgs), C.c_void_p]),
     "recnn_slate_distances": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_slate_diversify": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,

@@ -26,16 +26,12 @@
 
 #include <cub/device/device_radix_sort.cuh>
 
-#include "common.cuh"
-#include "tc_gemm.cuh"
-#include "topk.cuh"
+#include "ivf.cuh"
 
 namespace recnn {
 
-constexpr int kIvfTileQ = 32;          // queries of a fine-scan work unit: one per lane
 constexpr int kIvfWarps = 4;           // warps of a fine-scan CTA: each takes 4 rows of a 16-row chunk
 constexpr int kIvfChunk = 16;          // list rows per bulk copy
-constexpr int kIvfMaxDim = 512;        // the query tile and both row buffers fit shared memory up to here
 constexpr float kSplitEps = 1.0f / 1024.0f;
 
 static inline int ivf_pitch(int dim) { return (int)round_up(dim, 4); }   // list-table row pitch: 16-byte rows
@@ -157,9 +153,9 @@ __global__ void ivf_count_kernel(const int64_t* __restrict__ probe, long long pa
 }
 
 // one CTA, in order over chunks of 1024 lists: list_start = exclusive scan of the counts, unit_start = exclusive scan of
-// the work units ceil(count / 32); the counts are zeroed for the scatter that follows (they become its fill cursors)
+// the work units ceil(count / tile); the counts are zeroed for the scatter that follows (they become its fill cursors)
 __global__ void __launch_bounds__(1024)
-ivf_scan_kernel(int* __restrict__ cnt, int nlist, int* __restrict__ list_start, int* __restrict__ unit_start) {
+ivf_scan_kernel(int* __restrict__ cnt, int nlist, int tile, int* __restrict__ list_start, int* __restrict__ unit_start) {
   __shared__ int s_a[32], s_b[32];
   __shared__ int s_carry[2];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -168,7 +164,7 @@ ivf_scan_kernel(int* __restrict__ cnt, int nlist, int* __restrict__ list_start, 
   for (int base = 0; base < nlist; base += 1024) {
     const int l = base + threadIdx.x;
     const int c = l < nlist ? cnt[l] : 0;
-    const int u = (c + kIvfTileQ - 1) / kIvfTileQ;
+    const int u = (c + tile - 1) / tile;
     int a = c, b = u;                                  // inclusive warp scans
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
@@ -211,12 +207,6 @@ __global__ void ivf_scatter_kernel(const int64_t* __restrict__ probe, long long 
   group[list_start[l] + atomicAdd(fill + l, 1)] = (int)i;
 }
 
-__device__ __forceinline__ void bulk_copy(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
-               : "memory");
-}
-
 struct IvfLists {
   const long long* offsets;   // [nlist + 1]
   const float* table;         // [n_items, pitch], list order
@@ -236,12 +226,7 @@ ivf_scan_lists_kernel(const float* __restrict__ queries, int dim, int pitch, int
   extern __shared__ __align__(128) unsigned char smem[];
   const int u = blockIdx.x;
   if (u >= unit_start[nlist]) return;
-  int lo = 0, hi = nlist;                              // the largest l with unit_start[l] <= u (< nlist)
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (unit_start[mid] <= u) lo = mid; else hi = mid;
-  }
-  const int l = lo;
+  const int l = ivf_unit_list(unit_start, nlist, u);
   const int g0 = list_start[l] + (u - unit_start[l]) * kIvfTileQ;
   const int nq = min(kIvfTileQ, list_start[l + 1] - g0);
   const long long r0 = L.offsets[l], n_rows = L.offsets[l + 1] - r0;
@@ -363,17 +348,7 @@ ivf_merge_kernel(const Cand* __restrict__ part, int nprobe, int k, long long n_q
   float qn = 0.f;
   for (int d = lane; d < dim; d += 32) { const float v = queries[q * dim + d]; qn = fmaf(v, v, qn); }
   qn = warp_sum(qn);
-  const Cand* mine = part + q * (long long)nprobe * k;
-  int h0 = 0, h1 = 0;
-  for (int r = 0; r < k; ++r) {
-    float k0 = FLT_MAX, k1 = FLT_MAX; int i0 = kNoId, i1 = kNoId;
-    if (lane < nprobe && h0 < k) { const Cand c = mine[(long long)lane * k + h0]; k0 = c.key; i0 = c.id; }
-    if (lane + 32 < nprobe && h1 < k) { const Cand c = mine[(long long)(lane + 32) * k + h1]; k1 = c.key; i1 = c.id; }
-    const bool second = better(k1, i1, k0, i0);
-    float key = second ? k1 : k0;
-    int id = second ? i1 : i0, owner = lane;
-    warp_argmin(key, id, owner);
-    if (lane == owner) { if (second) ++h1; else ++h0; }
+  ivf_merge_warp(part + q * (long long)nprobe * k, nprobe, k, [&](int r, float key, int id) {
     if (lane == 0) {
       float d;
       if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);
@@ -383,7 +358,7 @@ ivf_merge_kernel(const Cand* __restrict__ part, int nprobe, int k, long long n_q
       ids_out[q * k + r] = id == kNoId ? -1 : (int64_t)id;
       dist_out[q * k + r] = d;
     }
-  }
+  });
 }
 
 // ------------------------------------------------------------------------------------------------------- workspaces
@@ -402,55 +377,45 @@ static size_t sort_temp_bytes(int64_t n, int nlist) {
 
 struct IvfBuildWorkspace {
   float* train;       // [n_sample, dim] the sample (COS: unit rows)
-  float* cnorm;       // [nlist] |c|^2 for the L2 assignment
-  float* count;       // [nlist] member counts (the split halves them)
-  int64_t* assign;    // [n_items] nearest centroid of each point
-  float* adist;       // [n_items]
-  void* coarse;       // the assignment search's own workspace
-  int64_t coarse_bytes;
-  int *keys_in, *vals_in, *keys_out, *vals_out;   // [n_items] each
-  long long* offs;    // [nlist + 1] training lists
-  void* sort_tmp;
-  size_t sort_bytes;
+  IvfKmeans km;       // for n_items points: the training rounds and the final assignment
   int64_t bytes;
 };
+
+// the k-means buffers for n points and k centroids; the assignment search is sized for n_other points as well
+IvfKmeans kmeans_carve(Carve& c, int64_t n, int64_t n_other, int k) {
+  IvfKmeans w;
+  w.cnorm = c.take(k);
+  w.count = c.take(k);
+  w.assign = c.take<int64_t>(n);
+  w.adist = c.take(n);
+  const int64_t a = recnn_retrieve_workspace_bytes(n_other, k, 1), b = recnn_retrieve_workspace_bytes(n, k, 1);
+  w.coarse_bytes = a > b ? a : b;
+  w.coarse = c.take<char>(w.coarse_bytes);
+  w.keys_in = c.take<int>(n);
+  w.vals_in = c.take<int>(n);
+  w.keys_out = c.take<int>(n);
+  w.vals_out = c.take<int>(n);
+  w.offs = c.take<long long>(k + 1);
+  w.sort_bytes = sort_temp_bytes(n, k);
+  w.sort_tmp = c.take<char>((int64_t)w.sort_bytes);
+  return w;
+}
 
 static IvfBuildWorkspace build_carve(int64_t n_items, int dim, int nlist, int64_t n_sample, void* base) {
   IvfBuildWorkspace w;
   Carve c(base);
   w.train = c.take(n_sample * dim);
-  w.cnorm = c.take(nlist);
-  w.count = c.take(nlist);
-  w.assign = c.take<int64_t>(n_items);
-  w.adist = c.take(n_items);
-  const int64_t a = recnn_retrieve_workspace_bytes(n_sample, nlist, 1), b = recnn_retrieve_workspace_bytes(n_items, nlist, 1);
-  w.coarse_bytes = a > b ? a : b;
-  w.coarse = c.take<char>(w.coarse_bytes);
-  w.keys_in = c.take<int>(n_items);
-  w.vals_in = c.take<int>(n_items);
-  w.keys_out = c.take<int>(n_items);
-  w.vals_out = c.take<int>(n_items);
-  w.offs = c.take<long long>(nlist + 1);
-  w.sort_bytes = sort_temp_bytes(n_items, nlist);
-  w.sort_tmp = c.take<char>((int64_t)w.sort_bytes);
+  w.km = kmeans_carve(c, n_items, n_sample, nlist);
   w.bytes = c.bytes();
   return w;
 }
 
-struct IvfSearchWorkspace {
-  int64_t* probe;     // [n, p] the coarse step's lists
-  float* pdist;       // [n, p]
-  void* coarse;
-  int64_t coarse_bytes;
-  int *cnt, *list_start, *unit_start;   // [nlist], [nlist + 1], [nlist + 1]
-  int* group;         // [n * p] output slots grouped by list
-  Cand* part;         // [n * p, k]
-  int64_t bytes;
-};
+int64_t ivf_build_lists_bytes(int64_t n_items, int dim, int nlist, int64_t n_sample) {
+  return build_carve(n_items, dim, nlist, n_sample, nullptr).bytes;
+}
 
-static IvfSearchWorkspace search_carve(int64_t n, int nlist, int p, int k, void* base) {
-  IvfSearchWorkspace w;
-  Carve c(base);
+IvfProbes ivf_probes_carve(Carve& c, int64_t n, int nlist, int p) {
+  IvfProbes w;
   w.probe = c.take<int64_t>(n * p);
   w.pdist = c.take(n * p);
   w.coarse_bytes = recnn_retrieve_workspace_bytes(n, nlist, p);
@@ -459,6 +424,19 @@ static IvfSearchWorkspace search_carve(int64_t n, int nlist, int p, int k, void*
   w.list_start = c.take<int>(nlist + 1);
   w.unit_start = c.take<int>(nlist + 1);
   w.group = c.take<int>(n * p);
+  return w;
+}
+
+struct IvfSearchWorkspace {
+  IvfProbes pr;
+  Cand* part;         // [n * p, k]
+  int64_t bytes;
+};
+
+static IvfSearchWorkspace search_carve(int64_t n, int nlist, int p, int k, void* base) {
+  IvfSearchWorkspace w;
+  Carve c(base);
+  w.pr = ivf_probes_carve(c, n, nlist, p);
   w.part = c.take<Cand>(n * p * k);
   w.bytes = c.bytes();
   return w;
@@ -471,7 +449,7 @@ static int ivf_smem_bytes(int dim, int kmax) {
 }
 
 // sorted (centroid, point) pairs of `assign` -> vals_out grouped by list, ascending inside; offs [nlist + 1]
-static int group_by_list(const IvfBuildWorkspace& w, int64_t n, int nlist, long long* offs, cudaStream_t st) {
+static int group_by_list(const IvfKmeans& w, int64_t n, int nlist, long long* offs, cudaStream_t st) {
   ivf_keys_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(w.assign, n, w.keys_in, w.vals_in);
   RECNN_CHECK_LAUNCH("ivf_keys_kernel");
   size_t bytes = w.sort_bytes;
@@ -480,6 +458,75 @@ static int group_by_list(const IvfBuildWorkspace& w, int64_t n, int nlist, long 
   count_launch();
   ivf_offsets_kernel<<<(unsigned)ceil_div(nlist + 1, 256), 256, 0, st>>>(w.keys_out, n, nlist, offs);
   RECNN_CHECK_LAUNCH("ivf_offsets_kernel");
+  return RECNN_OK;
+}
+
+int ivf_gather(const float* src, int dim, const long long* idx, long long n, bool unit, float* dst, int ld_dst,
+               cudaStream_t st) {
+  ivf_gather_kernel<<<(unsigned)ceil_div(n, 8), 256, 0, st>>>(src, dim, idx, n, unit, dst, ld_dst, RECNN_METRIC_L2,
+                                                              nullptr);
+  RECNN_CHECK_LAUNCH("ivf_gather_kernel");
+  return RECNN_OK;
+}
+
+int ivf_lloyd(const IvfKmeans& w, const float* train, int64_t n, int dim, float* centroids, int k, int n_iter,
+              bool spherical, cudaStream_t st) {
+  for (int it = 0; it < n_iter; ++it) {
+    RECNN_PROPAGATE(recnn_item_norms(centroids, k, dim, RECNN_METRIC_L2, w.cnorm, st));
+    RECNN_PROPAGATE(recnn_retrieve_topk(train, n, dim, centroids, k, w.cnorm, RECNN_METRIC_L2, 1, w.assign, w.adist,
+                                        w.coarse, w.coarse_bytes, st));
+    RECNN_PROPAGATE(group_by_list(w, n, k, w.offs, st));
+    ivf_update_kernel<<<(unsigned)k, 128, 0, st>>>(train, dim, w.vals_out, w.offs, centroids, w.count);
+    RECNN_CHECK_LAUNCH("ivf_update_kernel");
+    ivf_split_kernel<<<1, 256, 0, st>>>(centroids, dim, w.count, k);
+    RECNN_CHECK_LAUNCH("ivf_split_kernel");
+    if (spherical) {
+      ivf_normalize_kernel<<<(unsigned)ceil_div(k, 8), 256, 0, st>>>(centroids, k, dim);
+      RECNN_CHECK_LAUNCH("ivf_normalize_kernel");
+    }
+  }
+  return RECNN_OK;
+}
+
+int ivf_build_lists(const float* table, int64_t n_items, int dim, int metric, const int64_t* sample_ids,
+                    int64_t n_sample, const int64_t* init, int nlist, int n_iter, float* centroids_out,
+                    float* centroid_norms_out, int64_t* list_offsets_out, int64_t* list_ids_out, void* workspace,
+                    const int64_t** assign_out, cudaStream_t st) {
+  const IvfBuildWorkspace w = build_carve(n_items, dim, nlist, n_sample, workspace);
+  const bool cos = metric == RECNN_METRIC_COS;
+  RECNN_PROPAGATE(ivf_gather(table, dim, reinterpret_cast<const long long*>(sample_ids), n_sample, cos, w.train, dim,
+                             st));
+  RECNN_PROPAGATE(ivf_gather(w.train, dim, reinterpret_cast<const long long*>(init), nlist, false, centroids_out, dim,
+                             st));
+  RECNN_PROPAGATE(ivf_lloyd(w.km, w.train, n_sample, dim, centroids_out, nlist, n_iter, cos, st));
+  // final lists: every item to its nearest centroid (L2 on the raw rows; COS: the largest cosine, i.e. L2 on unit
+  // rows).  The centroid norms of L2 and COS are the search's coarse norms too; IP's coarse step needs none.
+  const int assign_metric = cos ? RECNN_METRIC_COS : RECNN_METRIC_L2;
+  float* cnorm = metric == RECNN_METRIC_IP ? w.km.cnorm : centroid_norms_out;
+  RECNN_PROPAGATE(recnn_item_norms(centroids_out, nlist, dim, assign_metric, cnorm, st));
+  RECNN_PROPAGATE(recnn_retrieve_topk(table, n_items, dim, centroids_out, nlist, cnorm, assign_metric, 1, w.km.assign,
+                                      w.km.adist, w.km.coarse, w.km.coarse_bytes, st));
+  RECNN_PROPAGATE(group_by_list(w.km, n_items, nlist, reinterpret_cast<long long*>(list_offsets_out), st));
+  ivf_widen_kernel<<<(unsigned)ceil_div(n_items, 256), 256, 0, st>>>(w.km.vals_out, n_items, list_ids_out);
+  RECNN_CHECK_LAUNCH("ivf_widen_kernel");
+  if (assign_out) *assign_out = w.km.assign;
+  return RECNN_OK;
+}
+
+int ivf_probe(const IvfProbes& w, const float* queries, int64_t n, int dim, const float* centroids,
+              const float* centroid_norms, int nlist, int metric, int nprobe, int tile, cudaStream_t st) {
+  // 1. coarse: the nprobe best centroids of each query under the index's metric
+  RECNN_PROPAGATE(recnn_retrieve_topk(queries, n, dim, centroids, nlist, centroid_norms, metric, nprobe, w.probe,
+                                      w.pdist, w.coarse, w.coarse_bytes, st));
+  // 2. probe inversion
+  const long long pairs = n * nprobe;
+  RECNN_CHECK_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int) * nlist, st));
+  ivf_count_kernel<<<(unsigned)ceil_div(pairs, 256), 256, 0, st>>>(w.probe, pairs, w.cnt);
+  RECNN_CHECK_LAUNCH("ivf_count_kernel");
+  ivf_scan_kernel<<<1, 1024, 0, st>>>(w.cnt, nlist, tile, w.list_start, w.unit_start);
+  RECNN_CHECK_LAUNCH("ivf_scan_kernel");
+  ivf_scatter_kernel<<<(unsigned)ceil_div(pairs, 256), 256, 0, st>>>(w.probe, pairs, w.list_start, w.cnt, w.group);
+  RECNN_CHECK_LAUNCH("ivf_scatter_kernel");
   return RECNN_OK;
 }
 
@@ -520,39 +567,9 @@ static int ivf_build(const float* table, int64_t n_items, int32_t dim, int32_t m
   RECNN_REQUIRE(n_iter >= 0, "n_iter >= 0");
   const IvfBuildWorkspace w = build_carve(n_items, dim, nlist, n_sample, workspace);
   RECNN_PROPAGATE(check_workspace(w.bytes, workspace_bytes));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool cos = metric == RECNN_METRIC_COS;
-  const long long* sample = reinterpret_cast<const long long*>(sample_ids);
-  ivf_gather_kernel<<<(unsigned)ceil_div(n_sample, 8), 256, 0, st>>>(table, dim, sample, n_sample, cos, w.train, dim,
-                                                                     metric, nullptr);
-  RECNN_CHECK_LAUNCH("ivf_gather_kernel");
-  ivf_gather_kernel<<<(unsigned)ceil_div(nlist, 8), 256, 0, st>>>(w.train, dim, reinterpret_cast<const long long*>(init),
-                                                                  nlist, false, centroids_out, dim, metric, nullptr);
-  RECNN_CHECK_LAUNCH("ivf_gather_kernel");
-  for (int it = 0; it < n_iter; ++it) {
-    RECNN_PROPAGATE(recnn_item_norms(centroids_out, nlist, dim, RECNN_METRIC_L2, w.cnorm, st));
-    RECNN_PROPAGATE(recnn_retrieve_topk(w.train, n_sample, dim, centroids_out, nlist, w.cnorm, RECNN_METRIC_L2, 1,
-                                        w.assign, w.adist, w.coarse, w.coarse_bytes, st));
-    RECNN_PROPAGATE(group_by_list(w, n_sample, nlist, w.offs, st));
-    ivf_update_kernel<<<(unsigned)nlist, 128, 0, st>>>(w.train, dim, w.vals_out, w.offs, centroids_out, w.count);
-    RECNN_CHECK_LAUNCH("ivf_update_kernel");
-    ivf_split_kernel<<<1, 256, 0, st>>>(centroids_out, dim, w.count, nlist);
-    RECNN_CHECK_LAUNCH("ivf_split_kernel");
-    if (cos) {
-      ivf_normalize_kernel<<<(unsigned)ceil_div(nlist, 8), 256, 0, st>>>(centroids_out, nlist, dim);
-      RECNN_CHECK_LAUNCH("ivf_normalize_kernel");
-    }
-  }
-  // final lists: every item to its nearest centroid (L2 on the raw rows; COS: the largest cosine, i.e. L2 on unit
-  // rows).  The centroid norms of L2 and COS are the search's coarse norms too; IP's coarse step needs none.
-  const int assign_metric = cos ? RECNN_METRIC_COS : RECNN_METRIC_L2;
-  float* cnorm = metric == RECNN_METRIC_IP ? w.cnorm : centroid_norms_out;
-  RECNN_PROPAGATE(recnn_item_norms(centroids_out, nlist, dim, assign_metric, cnorm, st));
-  RECNN_PROPAGATE(recnn_retrieve_topk(table, n_items, dim, centroids_out, nlist, cnorm, assign_metric, 1, w.assign,
-                                      w.adist, w.coarse, w.coarse_bytes, st));
-  RECNN_PROPAGATE(group_by_list(w, n_items, nlist, reinterpret_cast<long long*>(list_offsets_out), st));
-  ivf_widen_kernel<<<(unsigned)ceil_div(n_items, 256), 256, 0, st>>>(w.vals_out, n_items, list_ids_out);
-  RECNN_CHECK_LAUNCH("ivf_widen_kernel");
+  RECNN_PROPAGATE(ivf_build_lists(table, n_items, dim, metric, sample_ids, n_sample, init, nlist, n_iter, centroids_out,
+                                  centroid_norms_out, list_offsets_out, list_ids_out, workspace, nullptr,
+                                  static_cast<cudaStream_t>(stream)));
   return recnn_ivf_list_table(table, n_items, dim, metric, list_ids_out, list_table_out, list_norms_out, stream);
 }
 
@@ -590,18 +607,10 @@ static int ivf_search(const float* queries, int64_t n_queries, int32_t dim, cons
     RECNN_CHECK_CUDA(cudaMemsetAsync(error_flag, 0, sizeof(int32_t), st));
     RECNN_PROPAGATE(item_sets_check(ex, n_queries, n_items, error_flag, st));
   }
-  // 1. coarse: the nprobe best centroids of each query under the index's metric
-  RECNN_PROPAGATE(recnn_retrieve_topk(queries, n_queries, dim, centroids, nlist, centroid_norms, metric, nprobe, w.probe,
-                                      w.pdist, w.coarse, w.coarse_bytes, st));
-  // 2. probe inversion
+  // 1, 2. coarse step and probe inversion
+  RECNN_PROPAGATE(ivf_probe(w.pr, queries, n_queries, dim, centroids, centroid_norms, nlist, metric, nprobe, kIvfTileQ,
+                            st));
   const long long pairs = n_queries * nprobe;
-  RECNN_CHECK_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int) * nlist, st));
-  ivf_count_kernel<<<(unsigned)ceil_div(pairs, 256), 256, 0, st>>>(w.probe, pairs, w.cnt);
-  RECNN_CHECK_LAUNCH("ivf_count_kernel");
-  ivf_scan_kernel<<<1, 1024, 0, st>>>(w.cnt, nlist, w.list_start, w.unit_start);
-  RECNN_CHECK_LAUNCH("ivf_scan_kernel");
-  ivf_scatter_kernel<<<(unsigned)ceil_div(pairs, 256), 256, 0, st>>>(w.probe, pairs, w.list_start, w.cnt, w.group);
-  RECNN_CHECK_LAUNCH("ivf_scatter_kernel");
   // 3. fine scan: at most ceil(pairs / 32) + min(nlist, pairs) units; the surplus CTAs exit at once
   const int kmax = k <= 16 ? 16 : 64;
   auto kernel = k <= 16 ? (sets ? ivf_scan_lists_kernel<16, true> : ivf_scan_lists_kernel<16, false>)
@@ -611,8 +620,8 @@ static int ivf_search(const float* queries, int64_t n_queries, int32_t dim, cons
   const long long units = ceil_div(pairs, kIvfTileQ) + (pairs < nlist ? pairs : nlist);
   const IvfLists L = {reinterpret_cast<const long long*>(list_offsets), list_table, list_norms,
                       reinterpret_cast<const long long*>(list_ids)};
-  kernel<<<(unsigned)units, kIvfWarps * 32, smem, st>>>(queries, dim, ivf_pitch(dim), nprobe, nlist, w.list_start,
-                                                        w.unit_start, w.group, L, metric, k, ex, w.part);
+  kernel<<<(unsigned)units, kIvfWarps * 32, smem, st>>>(queries, dim, ivf_pitch(dim), nprobe, nlist, w.pr.list_start,
+                                                        w.pr.unit_start, w.pr.group, L, metric, k, ex, w.part);
   RECNN_CHECK_LAUNCH("ivf_scan_lists_kernel");
   // 4. merge the nprobe lists of each query
   ivf_merge_kernel<<<(unsigned)ceil_div(n_queries, 4), 128, 0, st>>>(w.part, nprobe, k, n_queries, metric, queries, dim,

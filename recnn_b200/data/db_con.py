@@ -20,6 +20,9 @@ and faiss name it), built on the device: k-means lists over the table, after
 which ``search(..., search_param={"nprobe": p})`` scans only the lists of each
 query's p nearest centroids (recnn_ivf_build / recnn_ivf_search).  ``rank``
 stays exact, so recall can be measured against it or against a flat index.
+``build_ivf(nlist, m=M)`` builds IVF_PQ instead: the same lists, each item
+stored as M one-byte codes of its residual, scanned through lookup tables and
+optionally re-ranked exactly from the table (``search_param={"refine": r}``).
 """
 from __future__ import annotations
 
@@ -60,6 +63,23 @@ def ivf_sample(n_items, nlist, seed=0, max_points_per_centroid=256):
     sample = torch.randperm(n_items, generator=g)[:cap] if n_items > cap else torch.arange(n_items)
     init = torch.randperm(len(sample), generator=g)[:nlist]
     return sample.to(torch.int64), init.to(torch.int64)
+
+
+PQ_CODEWORDS = 256         # 8-bit codes
+PQ_MAX_M = 64
+PQ_TRAIN_MAX = 65536       # codebook training points: the first this many of ivf_sample's sample
+
+
+def ivf_pq_sample(n_sample, seed=0):
+    """int64 CPU tensor [256]: the positions, among the first min(n_sample, 65536) points of ivf_sample's sample, of the
+    initial codewords of every subspace: the first 256 of torch.randperm(min(n_sample, 65536)) drawn from
+    torch.Generator().manual_seed(seed + 1)."""
+    n_train = min(int(n_sample), PQ_TRAIN_MAX)
+    if n_train < PQ_CODEWORDS:
+        raise ValueError("IVF_PQ trains 256 codewords per subspace: it needs a training sample of at least 256 points "
+                         "(got %d)" % n_train)
+    g = torch.Generator().manual_seed(int(seed) + 1)
+    return torch.randperm(n_train, generator=g)[:PQ_CODEWORDS].to(torch.int64)
 
 
 class IVFLists(NamedTuple):
@@ -109,16 +129,43 @@ class ItemIndex:
             return None
         return IVFLists(self._ivf["centroids"], self._ivf["list_offsets"], self._ivf["list_ids"])
 
-    def build_ivf(self, nlist, n_iter=25, seed=0, max_points_per_centroid=256):
-        """Build an inverted-file index (IVF_FLAT) over the table on the device and return self.
+    @property
+    def pq(self):
+        """None, or for an IVF_PQ index (codebooks fp32 [m, 256, dim / m], codes uint8 [n_items, m] in list order: the
+        codes of the item list_ids[p] are row p).  Views of the index's own device storage: read them, do not write
+        them."""
+        if self._ivf is None or "codes" not in self._ivf:
+            return None
+        return self._ivf["codebooks"], self._ivf["codes"][:, :self._ivf["m"]]
+
+    def _pq_check(self, m):
+        m = int(m)
+        if not 1 <= m <= PQ_MAX_M or self.dim % m != 0:
+            raise ValueError("IVF_PQ needs 1 <= m <= %d dividing dim = %d (got m = %d)" % (PQ_MAX_M, self.dim, m))
+        if self.n_items < PQ_CODEWORDS:
+            raise ValueError("IVF_PQ trains 256 codewords per subspace: it needs n_items >= 256 (got %d)"
+                             % self.n_items)
+        return m
+
+    def build_ivf(self, nlist, n_iter=25, seed=0, max_points_per_centroid=256, m=None):
+        """Build an inverted-file index over the table on the device and return self: IVF_FLAT when ``m`` is None,
+        IVF_PQ with ``m`` one-byte codes per item otherwise.
 
         k-means (Lloyd, ``n_iter`` rounds) on a sample of at most ``nlist * max_points_per_centroid`` items chosen by
         ``ivf_sample(n_items, nlist, seed, ...)``, initialised at ``nlist`` of its points; empty lists are split as
         faiss does.  COS runs spherical k-means on unit rows, L2 and IP k-means in L2 on the raw rows.  Every item then
         goes to the list of its nearest centroid.  The same table and arguments give the same index, bit for bit.
 
-        The index stores the table a second time, in list order (what IVF_FLAT stores): ``n_items * dim * 4`` bytes, 1 GB
-        at 1M x 256, plus the ids and norms.  It is a snapshot of the table at build time."""
+        IVF_FLAT stores the table a second time, in list order: ``n_items * dim * 4`` bytes, 1 GB at 1M x 256, plus the
+        ids and norms.  It is a snapshot of the table at build time.
+
+        IVF_PQ (``m`` dividing dim, 1 <= m <= 64, n_items >= 256) builds the same lists, bit for bit, and stores each item
+        as m codes instead of its row: ``n_items * (m + 8)`` bytes plus the centroids and 256 * dim * 4 bytes of
+        codebooks (41 MB at 1M x 256, m = 32).  The residual of an item is r = x - c_list(x) (COS: x the unit row);
+        subspace j is dims [j * dim / m, (j + 1) * dim / m).  Each subspace's 256 codewords are trained by ``n_iter``
+        Lloyd rounds (the coarse build's) on the residuals of the first min(len(sample), 65536) sample points, from the
+        codewords ``ivf_pq_sample(len(sample), seed)`` picks; each code is the nearest codeword (fp32, ties to the
+        smaller code).  See ``search`` for how the codes are scored."""
         nlist, n_iter, mppc = int(nlist), int(n_iter), int(max_points_per_centroid)
         if not 1 <= nlist <= self.n_items:
             raise ValueError("nlist must be in [1, n_items = %d] (got %d)" % (self.n_items, nlist))
@@ -128,37 +175,63 @@ class ItemIndex:
             raise ValueError("max_points_per_centroid must be >= 1 (got %d)" % mppc)
         if self.dim > IVF_MAX_DIM:
             raise ValueError("an IVF index supports dim <= %d (got %d)" % (IVF_MAX_DIM, self.dim))
+        if m is not None:
+            m = self._pq_check(m)
         sample, init = ivf_sample(self.n_items, nlist, seed, mppc)
+        pq_init = ivf_pq_sample(len(sample), seed) if m is not None else None
         dev = self.device
         sample, init = sample.to(dev), init.to(dev)
-        ivf = self._ivf_buffers(nlist)
+        ivf = self._ivf_buffers(nlist, m)
         L = _lib.lib()
-        ws = torch.empty(L.recnn_ivf_build_workspace_bytes(self.n_items, self.dim, nlist, len(sample)),
-                         dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
-            args = _lib.IvfBuildArgs(self._ivf_descriptor(ivf), self.table.data_ptr(), sample.data_ptr(), len(sample),
-                                     init.data_ptr(), n_iter, 0, ws.data_ptr(), ws.numel())
-            _lib.check(L.recnn_ivf_build(ctypes.byref(args), _lib.stream_ptr(dev)))
+            if m is None:
+                ws = torch.empty(L.recnn_ivf_build_workspace_bytes(self.n_items, self.dim, nlist, len(sample)),
+                                 dtype=torch.uint8, device=dev)
+                args = _lib.IvfBuildArgs(self._ivf_descriptor(ivf), self.table.data_ptr(), sample.data_ptr(),
+                                         len(sample), init.data_ptr(), n_iter, 0, ws.data_ptr(), ws.numel())
+                _lib.check(L.recnn_ivf_build(ctypes.byref(args), _lib.stream_ptr(dev)))
+            else:
+                pq_init = pq_init.to(dev)
+                ws = torch.empty(L.recnn_ivf_pq_build_workspace_bytes(self.n_items, self.dim, nlist, len(sample), m),
+                                 dtype=torch.uint8, device=dev)
+                args = _lib.IvfPqBuildArgs(self._pq_descriptor(ivf), self.table.data_ptr(), sample.data_ptr(),
+                                           len(sample), init.data_ptr(), pq_init.data_ptr(), n_iter, 0, ws.data_ptr(),
+                                           ws.numel())
+                _lib.check(L.recnn_ivf_pq_build(ctypes.byref(args), _lib.stream_ptr(dev)))
         del ws
         ivf["params"] = dict(nlist=nlist, n_iter=n_iter, seed=int(seed), max_points_per_centroid=mppc)
+        if m is not None:
+            ivf["params"]["m"] = m
         self._ivf_finish(ivf)
         return self
 
-    def _ivf_buffers(self, nlist):
+    def _ivf_buffers(self, nlist, m=None):
         dev, pitch = self.device, (self.dim + 3) // 4 * 4
         norms = self.metric != _lib.METRIC_IP
-        return dict(centroids=torch.empty(nlist, self.dim, dtype=torch.float32, device=dev),
-                    centroid_norms=torch.empty(nlist, dtype=torch.float32, device=dev) if norms else None,
-                    list_offsets=torch.empty(nlist + 1, dtype=torch.int64, device=dev),
-                    list_ids=torch.empty(self.n_items, dtype=torch.int64, device=dev),
-                    list_table=torch.empty(self.n_items, pitch, dtype=torch.float32, device=dev),
-                    list_norms=torch.empty(self.n_items, dtype=torch.float32, device=dev) if norms else None)
+        ivf = dict(centroids=torch.empty(nlist, self.dim, dtype=torch.float32, device=dev),
+                   centroid_norms=torch.empty(nlist, dtype=torch.float32, device=dev) if norms else None,
+                   list_offsets=torch.empty(nlist + 1, dtype=torch.int64, device=dev),
+                   list_ids=torch.empty(self.n_items, dtype=torch.int64, device=dev))
+        if m is None:
+            ivf.update(list_table=torch.empty(self.n_items, pitch, dtype=torch.float32, device=dev),
+                       list_norms=torch.empty(self.n_items, dtype=torch.float32, device=dev) if norms else None)
+        else:
+            # codes rows padded to 16 bytes: the search streams them with bulk copies
+            ivf.update(m=m, codebooks=torch.empty(m, PQ_CODEWORDS, self.dim // m, dtype=torch.float32, device=dev),
+                       codes=torch.empty(self.n_items, (m + 15) // 16 * 16, dtype=torch.uint8, device=dev))
+        return ivf
 
     def _ivf_descriptor(self, ivf):
         """the recnn_ivf_index of the buffers in ivf"""
         return _lib.ivf_index(self.n_items, self.dim, self.metric, int(ivf["centroids"].shape[0]), ivf["centroids"],
                               ivf["centroid_norms"], ivf["list_offsets"], ivf["list_ids"], ivf["list_table"],
                               ivf["list_norms"])
+
+    def _pq_descriptor(self, ivf):
+        """the recnn_ivf_pq_index of the buffers in ivf"""
+        return _lib.ivf_pq_index(self.n_items, self.dim, self.metric, int(ivf["centroids"].shape[0]), ivf["m"],
+                                 ivf["centroids"], ivf["centroid_norms"], ivf["list_offsets"], ivf["list_ids"],
+                                 ivf["codebooks"], ivf["codes"])
 
     def _ivf_finish(self, ivf):
         ivf["nlist"] = int(ivf["centroids"].shape[0])
@@ -167,24 +240,40 @@ class ItemIndex:
 
     def ivf_state(self):
         """The IVF index as host tensors and plain values, for torch.save: centroids, list_offsets, list_ids, the build
-        parameters, the metric and the table's shape.  None without an index."""
+        parameters, the metric and the table's shape; an IVF_PQ index adds its codebooks, and ``m`` to the parameters
+        (the codes are rebuilt from the table on loading).  None without an index."""
         if self._ivf is None:
             return None
-        return dict(centroids=self._ivf["centroids"].cpu(), list_offsets=self._ivf["list_offsets"].cpu(),
-                    list_ids=self._ivf["list_ids"].cpu(), params=dict(self._ivf["params"]), metric=self.metric_name,
-                    n_items=self.n_items, dim=self.dim)
+        state = dict(centroids=self._ivf["centroids"].cpu(), list_offsets=self._ivf["list_offsets"].cpu(),
+                     list_ids=self._ivf["list_ids"].cpu(), params=dict(self._ivf["params"]), metric=self.metric_name,
+                     n_items=self.n_items, dim=self.dim)
+        if "codes" in self._ivf:
+            state["codebooks"] = self._ivf["codebooks"].cpu()
+        return state
 
     def load_ivf(self, state):
         """Restore an index saved by ivf_state over this index's table (the same table it was built on) and return
         self.  The shapes and the metric must match, and list_ids must be a permutation of the items, ascending within
         each list, with monotone offsets from 0 to n_items (checked on the device): ValueError otherwise.  The
-        list-ordered table and the norms are rebuilt from this index's table."""
+        list-ordered table and the norms are rebuilt from this index's table.  An IVF_PQ state (``m`` in its params)
+        also needs codebooks [m, 256, dim / m]; its codes are encoded again on the device from the table, the lists
+        and the codebooks, by the build's kernel, so they equal the build's bit for bit."""
         try:
             cent, offs, ids = state["centroids"], state["list_offsets"], state["list_ids"]
             metric, n_items, dim = state["metric"], int(state["n_items"]), int(state["dim"])
             params = dict(state["params"])
         except (KeyError, TypeError) as e:
             raise ValueError("not an ivf_state() dict: %s" % e)
+        m = params.get("m")
+        if m is not None:
+            if not isinstance(m, int):
+                raise ValueError("malformed ivf state: params['m'] must be an int (got %r)" % (m,))
+            m = self._pq_check(m)
+            books = state.get("codebooks")
+            if (not torch.is_tensor(books) or not books.dtype.is_floating_point
+                    or tuple(books.shape) != (m, PQ_CODEWORDS, self.dim // m)):
+                raise ValueError("malformed ivf state: an IVF_PQ state needs codebooks [%d, %d, %d] float"
+                                 % (m, PQ_CODEWORDS, self.dim // m))
         if metric != self.metric_name:
             raise ValueError("the index was built for metric %s, this ItemIndex is %s" % (metric, self.metric_name))
         if (n_items, dim) != (self.n_items, self.dim):
@@ -216,7 +305,7 @@ class ItemIndex:
         if not ok:
             raise ValueError("malformed ivf state: list_ids must be a permutation of [0, %d), ascending within each "
                              "list, and list_offsets monotone from 0 to %d" % (n_items, n_items))
-        ivf = self._ivf_buffers(nlist)
+        ivf = self._ivf_buffers(nlist, m)
         ivf["centroids"].copy_(cent.to(device=dev, dtype=torch.float32))
         ivf["list_offsets"].copy_(offs)
         ivf["list_ids"].copy_(ids)
@@ -225,9 +314,18 @@ class ItemIndex:
             if ivf["centroid_norms"] is not None:
                 _lib.check(L.recnn_item_norms(ivf["centroids"].data_ptr(), nlist, self.dim, self.metric,
                                               ivf["centroid_norms"].data_ptr(), _lib.stream_ptr(dev)))
-            _lib.check(L.recnn_ivf_list_table(self.table.data_ptr(), self.n_items, self.dim, self.metric,
-                                              ivf["list_ids"].data_ptr(), ivf["list_table"].data_ptr(),
-                                              _lib.ptr(ivf["list_norms"]), _lib.stream_ptr(dev)))
+            if m is None:
+                _lib.check(L.recnn_ivf_list_table(self.table.data_ptr(), self.n_items, self.dim, self.metric,
+                                                  ivf["list_ids"].data_ptr(), ivf["list_table"].data_ptr(),
+                                                  _lib.ptr(ivf["list_norms"]), _lib.stream_ptr(dev)))
+            else:
+                ivf["codebooks"].copy_(books.to(device=dev, dtype=torch.float32))
+                ws = torch.empty(L.recnn_ivf_pq_encode_workspace_bytes(self.n_items, self.dim), dtype=torch.uint8,
+                                 device=dev)
+                args = _lib.IvfPqEncodeArgs(self._pq_descriptor(ivf), self.table.data_ptr(), ws.data_ptr(),
+                                            ws.numel())
+                _lib.check(L.recnn_ivf_pq_encode(ctypes.byref(args), _lib.stream_ptr(dev)))
+                del ws
         ivf["params"] = params
         self._ivf_finish(ivf)
         return self
@@ -235,13 +333,21 @@ class ItemIndex:
     def _nprobe(self, search_param):
         nlist = self._ivf["nlist"]
         p = dict(search_param or {})
-        unknown = sorted(set(p) - {"nprobe"})
+        pq = "codes" in self._ivf
+        unknown = sorted(set(p) - ({"nprobe", "refine"} if pq else {"nprobe"}))
         if unknown:
-            raise ValueError("unknown search_param keys %s (an IVF index takes only nprobe)" % unknown)
+            raise ValueError("unknown search_param keys %s (an %s index takes only %s)"
+                             % (unknown, "IVF_PQ" if pq else "IVF_FLAT", "nprobe and refine" if pq else "nprobe"))
         nprobe = int(p.get("nprobe", min(16, nlist)))
         if not 1 <= nprobe <= min(nlist, IVF_MAX_NPROBE):
             raise ValueError("nprobe must be in [1, min(nlist = %d, %d)] (got %d)" % (nlist, IVF_MAX_NPROBE, nprobe))
         return nprobe
+
+    def _refine(self, search_param, topk):
+        refine = int((search_param or {}).get("refine", 0))
+        if refine < 0 or max(refine, 1) * topk > 64:
+            raise ValueError("refine must be >= 0 with refine * topk <= 64 (got refine %d, topk %d)" % (refine, topk))
+        return refine
 
     def search(self, search_vecs, topk=10, search_param=None, exclude=None, exclude_rows=None):
         """search_vecs: [n, dim] (tensor / array on any device).  Returns SearchResult on the index's device.
@@ -253,7 +359,16 @@ class ItemIndex:
         Without an IVF index the search is exact and ``search_param`` is ignored.  After ``build_ivf`` / ``load_ivf``
         it is the IVF_FLAT search: ``search_param={"nprobe": p}`` (default 16, at most min(nlist, 64); any other key
         raises ValueError) scans the lists of each query's p nearest centroids, and the result is the exact top-k over
-        those lists -- the same for a query whatever other queries share the call."""
+        those lists -- the same for a query whatever other queries share the call.
+
+        On an IVF_PQ index (``build_ivf(..., m=M)``) the probed lists are scored from their codes by asymmetric distance
+        computation, in fp32: L2 the squared distance from the query to the item's reconstruction c_list + r_hat (a
+        per-(query, list) table of 256 * M entries), IP <q, c_list> + <q, r_hat> (a per-query table), COS the IP form on
+        the unit query against the unit-row reconstruction, not renormalised.  ``search_param={"nprobe": p,
+        "refine": r}``: r = 0 (default) returns the ADC top-k with ADC distances; r >= 1 re-scores the best r * topk
+        ADC candidates exactly against ``table`` (r * topk <= 64) and returns their exact top-k with exact distances,
+        computed as IVF_FLAT computes them: when r * topk covers every eligible item of the probed lists, the result is
+        IVF_FLAT's at the same nprobe, bit for bit."""
         from .item_sets import ItemSets, row_map
         nprobe = self._nprobe(search_param) if self._ivf is not None else None
         q = torch.as_tensor(search_vecs)
@@ -264,6 +379,7 @@ class ItemIndex:
         topk = int(topk)
         if not 1 <= topk <= min(64, self.n_items):
             raise ValueError("topk must be in [1, min(64, n_items)]")
+        refine = self._refine(search_param, topk) if nprobe is not None and "codes" in self._ivf else None
         n = int(q.shape[0])
         sets = rows = None
         if exclude is not None:
@@ -279,7 +395,7 @@ class ItemIndex:
             return SearchResult(ids, dist)
         L = _lib.lib()
         if nprobe is not None:
-            return self._ivf_search(q, n, topk, nprobe, sets, rows)
+            return self._ivf_search(q, n, topk, nprobe, sets, rows, refine)
         need = L.recnn_retrieve_workspace_bytes(n, self.n_items, topk)
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
@@ -307,11 +423,14 @@ class ItemIndex:
             raise ValueError("malformed exclusion table: a set is not ascending, its offsets are out of range or "
                              "decreasing, or an exclude_rows entry is outside [-1, %d)" % n_sets)
 
-    def _ivf_search(self, q, n, topk, nprobe, sets, rows):
+    def _ivf_search(self, q, n, topk, nprobe, sets, rows, refine=None):
         L, iv, dev = _lib.lib(), self._ivf, self.device
         ids = torch.empty(n, topk, dtype=torch.int64, device=dev)
         dist = torch.empty(n, topk, dtype=torch.float32, device=dev)
-        need = L.recnn_ivf_search_workspace_bytes(n, iv["nlist"], nprobe, topk)
+        if refine is None:
+            need = L.recnn_ivf_search_workspace_bytes(n, iv["nlist"], nprobe, topk)
+        else:
+            need = L.recnn_ivf_pq_search_workspace_bytes(n, iv["nlist"], nprobe, topk, refine)
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
         set_args, flag = (None, 0, None, 0, None), None
@@ -322,10 +441,16 @@ class ItemIndex:
             set_args = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
                         len(sets), _lib.ptr(rows))
         with torch.cuda.device(dev):
-            args = _lib.IvfSearchArgs(self._ivf_descriptor(iv), q.data_ptr(), n, nprobe, topk, *set_args,
-                                      ids.data_ptr(), dist.data_ptr(), _lib.ptr(flag), self._ws.data_ptr(),
-                                      self._ws.numel())
-            _lib.check(L.recnn_ivf_search(ctypes.byref(args), _lib.stream_ptr(dev)))
+            if refine is None:
+                args = _lib.IvfSearchArgs(self._ivf_descriptor(iv), q.data_ptr(), n, nprobe, topk, *set_args,
+                                          ids.data_ptr(), dist.data_ptr(), _lib.ptr(flag), self._ws.data_ptr(),
+                                          self._ws.numel())
+                _lib.check(L.recnn_ivf_search(ctypes.byref(args), _lib.stream_ptr(dev)))
+            else:
+                args = _lib.IvfPqSearchArgs(self._pq_descriptor(iv), self.table.data_ptr(), _lib.ptr(self.norms),
+                                            q.data_ptr(), n, nprobe, topk, refine, 0, *set_args, ids.data_ptr(),
+                                            dist.data_ptr(), _lib.ptr(flag), self._ws.data_ptr(), self._ws.numel())
+                _lib.check(L.recnn_ivf_pq_search(ctypes.byref(args), _lib.stream_ptr(dev)))
         if flag is not None:
             self._raise_set_bits(int(flag.item()), len(sets))
         return SearchResult(ids, dist)
@@ -393,8 +518,10 @@ class MilvusConnection(ItemIndex):
     """Constructor shape of recnn.data.db_con.MilvusConnection(env, name=..., port=..., param=...): the collection
     is ``env.base.embeddings``; ``param["metric_type"]`` may be "L2" (default) or "IP".  ``param["index_type"]``
     "IVF_FLAT" with ``param["nlist"]`` builds the IVF index at construction (Milvus create_index(IVF_FLAT, {"nlist"})),
-    so that ``search(..., search_param={"nprobe": p})`` means what it means to Milvus; without it, or with "FLAT", the
-    search is exact.  No Milvus server is involved."""
+    so that ``search(..., search_param={"nprobe": p})`` means what it means to Milvus; "IVF_PQ" with ``param["nlist"]``,
+    ``param["m"]`` and optionally ``param["nbits"]`` (8, the only width) builds the IVF_PQ index (Milvus
+    create_index(IVF_PQ, {"nlist", "m", "nbits"})); without it, or with "FLAT", the search is exact.  No Milvus server
+    is involved."""
 
     def __init__(self, env, name="movies_L2", port="19530", param=None):
         metric = "L2"
@@ -402,14 +529,21 @@ class MilvusConnection(ItemIndex):
             mt = str(param["metric_type"]).upper()
             metric = "IP" if mt.endswith("IP") else "L2"
         index_type = str(param.get("index_type", "FLAT")).upper() if param else "FLAT"
-        if index_type not in ("FLAT", "IVF_FLAT"):
-            raise ValueError("index_type must be FLAT or IVF_FLAT (got %s)" % index_type)
-        if index_type == "IVF_FLAT" and "nlist" not in param:
-            raise ValueError("index_type IVF_FLAT needs param['nlist']")
+        if index_type not in ("FLAT", "IVF_FLAT", "IVF_PQ"):
+            raise ValueError("index_type must be FLAT, IVF_FLAT or IVF_PQ (got %s)" % index_type)
+        if index_type != "FLAT" and "nlist" not in param:
+            raise ValueError("index_type %s needs param['nlist']" % index_type)
+        if index_type == "IVF_PQ":
+            if "m" not in param:
+                raise ValueError("index_type IVF_PQ needs param['m']")
+            if int(param.get("nbits", 8)) != 8:
+                raise ValueError("IVF_PQ supports nbits = 8 only (got %s)" % param["nbits"])
         emb = env.base.embeddings if hasattr(env, "base") else env
         super().__init__(emb, metric)
         if index_type == "IVF_FLAT":
             self.build_ivf(int(param["nlist"]))
+        elif index_type == "IVF_PQ":
+            self.build_ivf(int(param["nlist"]), m=int(param["m"]))
         self.name = name
         self.statuses = {}
 
