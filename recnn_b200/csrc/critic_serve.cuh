@@ -92,11 +92,8 @@ __device__ __forceinline__ long long serve_id(const long long* __restrict__ ids,
   return ids ? __ldg(ids + r * ld_ids + col) : col;
 }
 
-// smaller is better: -Q, NaN last (as score_key)
-__device__ __forceinline__ float serve_key(float q) {
-  const float key = -q;
-  return key == key ? key : FLT_MAX;
-}
+// smaller is better: -Q, a NaN or -inf Q as FLT_MAX (finite_key, as score_key)
+__device__ __forceinline__ float serve_key(float q) { return finite_key(-q); }
 
 // One CTA per row of the candidates: *flag |= 1 for an id outside [-1, items), |= kServeCandRepeat for an id that
 // appears twice in the row (the row is compared with itself tile by tile in shared memory: O(M^2) compares, cheap next

@@ -299,9 +299,8 @@ ivf_scan_lists_kernel(const float* __restrict__ queries, int dim, int pitch, int
         if (!live || rw + r >= rows) continue;
         const long long row = r0 + c * kIvfChunk + rw + r;
         const float s = acc[r];
-        float key = metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(L.norms + row))
-                  : metric == RECNN_METRIC_COS ? -s * __ldg(L.norms + row) : -s;
-        if (!(key == key)) key = FLT_MAX;
+        const float key = finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(L.norms + row))
+                                     : metric == RECNN_METRIC_COS ? -s * __ldg(L.norms + row) : -s);
         const int id = (int)__ldg(L.ids + row);
         if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && (!SETS || set.n == 0 || !set_has(set, nullptr, id)))
           list_insert(keys, ids, key, id);

@@ -257,8 +257,7 @@ pq_scan_lists_kernel(const float* __restrict__ queries, int dim, int nprobe, int
             if (j < m) s += T[j * kPqCodewords + ((wv[b >> 2] >> (8 * (b & 3))) & 255u)];
           }
         }
-        float key = l2 ? s : -s;
-        if (!(key == key)) key = FLT_MAX;
+        const float key = finite_key(l2 ? s : -s);
         const long long row = r0 + c * kPqChunk + i;
         const int id = (int)__ldg(P.ids + row);
         if (better(key, id, bar_k, bar_i) && (!SETS || set.n == 0 || !set_has(set, nullptr, id))) {
@@ -307,10 +306,8 @@ __device__ __forceinline__ float pq_exact_key(const float* __restrict__ q, const
   const float* x = table + (long long)id * dim;
   float s = 0.f;
   for (int d = 0; d < dim; ++d) s = fmaf(q[d], __ldg(x + d), s);
-  float key = metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + id))
-            : metric == RECNN_METRIC_COS ? -s * __ldg(norms + id) : -s;
-  if (!(key == key)) key = FLT_MAX;
-  return key;
+  return finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + id))
+                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + id) : -s);
 }
 
 // one warp per query: merge its nprobe ascending lists of k' into the k' best (ivf_merge_warp).  Without refine the

@@ -615,7 +615,7 @@ constexpr int kMaxExclude = 256;     // E of the dense [n, E] form
 constexpr int kTopkSplitCap = 31;     // the running list takes lane 0 of the merge warp
 
 // -logit, with NaN and -inf logits ranked after every finite one (and still before an empty slot, by id)
-__device__ __forceinline__ float logit_key(float z) { return fminf(-z, FLT_MAX); }
+__device__ __forceinline__ float logit_key(float z) { return finite_key(-z); }
 
 __global__ void cand_fill_kernel(Cand* __restrict__ c, long long count) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;

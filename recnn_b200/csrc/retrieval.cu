@@ -37,12 +37,11 @@ item_norms_kernel(const float* __restrict__ table, long long n_items, int dim, i
   if (lane == 0) out[row] = metric == RECNN_METRIC_COS ? 1.0f / fmaxf(sqrtf(s), 1e-30f) : s;
 }
 
-// the key of item j from its score: smaller is better; NaN scores rank last
+// the key of item j from its score: smaller is better; a NaN or +inf key ranks as FLT_MAX (finite_key), so the item is
+// still returned, after every finite key
 __device__ __forceinline__ float score_key(float s, const float* __restrict__ norms, long long j, int metric) {
-  float key = metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
-            : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s;
-  if (!(key == key)) key = FLT_MAX;
-  return key;
+  return finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
+                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s);
 }
 
 // grid (splits, n_queries).  scores [n_queries, ld]; writes k candidates per (query, split), ascending.  Query q is

@@ -1,7 +1,7 @@
 // Exact top-k building blocks shared by nearest-item retrieval (retrieval.cu) and the REINFORCE policy's top-k
 // (reinforce.cuh): a candidate is (key, id), smaller key first, ties towards the smaller id (== a stable argsort of the
 // keys).  Each thread keeps the best KMAX of its share in a sorted register list; a CTA merges its lists by rounds of a
-// block arg-min over the list heads.
+// block arg-min over the list heads.  Every selector builds its keys through finite_key: NaN and +inf rank as FLT_MAX.
 #pragma once
 
 #include <float.h>
@@ -29,6 +29,11 @@ static inline int topk_splits(int64_t n_rows, int64_t n_items, int cap) {
 }
 
 __device__ __forceinline__ bool better(float ka, int ia, float kb, int ib) { return ka < kb || (ka == kb && ia < ib); }
+
+// A ranking key as every selector stores it: NaN and +inf become FLT_MAX (fminf returns the other operand of a NaN), so
+// such an item ranks after every finite key, ties by id, and still before an empty slot {FLT_MAX, kNoId}: it is
+// returned before any "fewer than k eligible items" pad.  -inf stays the best key.
+__device__ __forceinline__ float finite_key(float key) { return fminf(key, FLT_MAX); }
 
 // block arg-min over one candidate per thread; returns the winner's (key, id, owner thread) to every thread
 __device__ __forceinline__ void block_argmin(float key, int id, float* s_key, int* s_id, int* s_owner, float& wk,

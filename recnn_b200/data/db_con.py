@@ -353,8 +353,9 @@ class ItemIndex:
         """search_vecs: [n, dim] (tensor / array on any device).  Returns SearchResult on the index's device.
         ``exclude``: an ``ItemSets`` of item ids never returned (e.g. ``DeviceFrameFeed.seen_items()``), with
         ``exclude_rows`` int64 [n] naming each query's set (-1: none; default query r -> set r).  A query with fewer
-        than topk eligible items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  An excluded id outside
-        [0, n_items) raises IndexError, a malformed table ValueError.
+        than topk eligible items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  An item whose key is NaN
+        or +inf (a NaN row, an overflowing |t|^2 or score) ranks as key FLT_MAX: after every finite key, ties by id, and
+        before any -1.  An excluded id outside [0, n_items) raises IndexError, a malformed table ValueError.
 
         Without an IVF index the search is exact and ``search_param`` is ignored.  After ``build_ivf`` / ``load_ivf``
         it is the IVF_FLAT search: ``search_param={"nprobe": p}`` (default 16, at most min(nlist, 64); any other key

@@ -202,7 +202,7 @@ class Critic(nn.Module):
         several such lists concatenated); None scores every item of the table.  ``exclude`` / ``exclude_rows``: an
         ``ItemSets`` of ids never returned (e.g. ``DeviceFrameFeed.seen_items()``), as in ``ItemIndex.search``.
         values fp32 [N, k] are the Q values, ids int64 [N, k]; a row with fewer than k eligible items ends in id -1,
-        value -FLT_MAX.  1 <= k <= 64.  ``chunk``: columns per chunk (None: auto); it does not change a bit.
+        value -FLT_MAX.  A NaN or -inf Q ranks after every finite one (ties by id, value -FLT_MAX), before any -1.  1 <= k <= 64.  ``chunk``: columns per chunk (None: auto); it does not change a bit.
 
         Scores are the eval-mode forward whatever ``self.training`` says; nothing of the critic is changed.  A repeated
         id within a row's candidates or a malformed table raises ValueError, an id out of range IndexError.  Nothing of
