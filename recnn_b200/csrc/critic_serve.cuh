@@ -92,7 +92,7 @@ __device__ __forceinline__ long long serve_id(const long long* __restrict__ ids,
   return ids ? __ldg(ids + r * ld_ids + col) : col;
 }
 
-// smaller is better: -Q, a NaN or -inf Q as FLT_MAX (finite_key, as score_key)
+// smaller is better: -Q, a NaN or -inf Q as FLT_MAX (finite_key, as metric_key)
 __device__ __forceinline__ float serve_key(float q) { return finite_key(-q); }
 
 // One CTA per row of the candidates: *flag |= 1 for an id outside [-1, items), |= kServeCandRepeat for an id that
@@ -197,8 +197,6 @@ __global__ void __launch_bounds__(kTopkThreads)
 serve_topk_kernel(const float* __restrict__ q, long long ldq, const long long* __restrict__ ids, long long ld_ids,
                   long long c0, int w, long long items, long long r0, ItemSets ex, int stage_cap, int k,
                   Cand* __restrict__ part) {
-  __shared__ float s_key[32];
-  __shared__ int s_id[32], s_owner[32];
   extern __shared__ int s_set[];
   const int y = blockIdx.y, sp = blockIdx.x, splits = gridDim.x;
   const long long r = r0 + y;
@@ -219,16 +217,7 @@ serve_topk_kernel(const float* __restrict__ q, long long ldq, const long long* _
     if (better(key, (int)id, keys[KMAX - 1], idl[KMAX - 1]) && (!SETS || set.n == 0 || !set_has(set, s_set, (int)id)))
       list_insert(keys, idl, key, (int)id);
   }
-  int head = 0;
-  Cand* out = part + ((long long)y * splits + sp) * k;
-  for (int i = 0; i < k; ++i) {
-    float hk; int hid;
-    list_at(keys, idl, head, hk, hid);
-    float wk; int wi, wo;
-    block_argmin(hk, hid, s_key, s_id, s_owner, wk, wi, wo);
-    if ((int)threadIdx.x == wo) ++head;
-    if (threadIdx.x == 0) { out[i].key = wk; out[i].id = wi; }
-  }
+  block_merge(keys, idl, k, part + ((long long)y * splits + sp) * k);
 }
 
 // one warp per row of the block: run[r] <- the k best of the row's running list and its `splits` block lists
@@ -240,15 +229,10 @@ serve_merge_kernel(const Cand* __restrict__ part, int splits, int k, long long r
   if (y >= nr) return;
   const Cand* mine = lane == kServeSplitsMax ? run + (r0 + y) * k : part + (y * splits + lane) * k;
   const bool owns = lane < splits || lane == kServeSplitsMax;
-  int head = 0;
-  for (int i = 0; i < k; ++i) {
-    float key = FLT_MAX; int id = kNoId;
-    if (owns && head < k) { key = mine[head].key; id = mine[head].id; }
-    int owner = lane;
-    warp_argmin(key, id, owner);
-    if (lane == owner) ++head;
-    if (lane == 0) { s_out[wi][i].key = key; s_out[wi][i].id = id; }
-  }
+  warp_merge<1>(k, [&](int, int pos) { return owns && pos < k ? mine[pos] : Cand{FLT_MAX, kNoId}; },
+                [&](int i, float key, int id, int) {
+                  if (lane == 0) { s_out[wi][i].key = key; s_out[wi][i].id = id; }
+                });
   __syncwarp();
   for (int i = lane; i < k; i += 32) run[(r0 + y) * k + i] = s_out[wi][i];
 }

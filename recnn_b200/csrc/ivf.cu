@@ -15,9 +15,9 @@
 //                scatter of each pair's output slot (q * p + j)
 //   fine scan    one CTA per (list, tile of <= 32 queries probing it): the tile's queries staged in shared memory,
 //                the list's contiguous rows streamed through two cp.async.bulk buffers; lane = query, each thread keeps
-//                a register top-k list; fp32 fma dot products in ascending d; keys as retrieval's score_key
-//   merge        one warp per query merges its p sorted lists (a lane owns lists lane and lane + 32); the metric is
-//                finished as topk_merge_kernel does
+//                a register top-k list; fp32 fma dot products in ascending d; keys by metric_key (topk.cuh)
+//   merge        one warp per query merges its p sorted lists (warp_merge, a lane owns lists lane and lane + 32) and
+//                reports the distances through metric_distance, as the flat search does
 // A (query, item) key is computed by the same instructions in the same order wherever it lands, so the result at
 // nprobe p is the exact top-k, by (key, id), over the union of the p probed lists, whatever else shares the call.
 #include <float.h>
@@ -298,9 +298,7 @@ ivf_scan_lists_kernel(const float* __restrict__ queries, int dim, int pitch, int
       for (int r = 0; r < 4; ++r) {
         if (!live || rw + r >= rows) continue;
         const long long row = r0 + c * kIvfChunk + rw + r;
-        const float s = acc[r];
-        const float key = finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(L.norms + row))
-                                     : metric == RECNN_METRIC_COS ? -s * __ldg(L.norms + row) : -s);
+        const float key = metric_key(acc[r], L.norms, row, metric);
         const int id = (int)__ldg(L.ids + row);
         if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && (!SETS || set.n == 0 || !set_has(set, nullptr, id)))
           list_insert(keys, ids, key, id);
@@ -336,26 +334,22 @@ ivf_scan_lists_kernel(const float* __restrict__ queries, int dim, int pitch, int
   }
 }
 
-// one warp per query: merge its nprobe ascending lists of k (lane owns lists lane and lane + 32) and finish the metric
-// exactly as topk_merge_kernel does
+// one warp per query: merge its nprobe <= 64 ascending lists of k (lane owns lists lane and lane + 32) and report the
+// distances, as the flat search does (metric_distance)
 __global__ void __launch_bounds__(128)
 ivf_merge_kernel(const Cand* __restrict__ part, int nprobe, int k, long long n_queries, int metric,
                  const float* __restrict__ queries, int dim, int64_t* __restrict__ ids_out, float* __restrict__ dist_out) {
   const long long q = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (q >= n_queries) return;
-  float qn = 0.f;
-  for (int d = lane; d < dim; d += 32) { const float v = queries[q * dim + d]; qn = fmaf(v, v, qn); }
-  qn = warp_sum(qn);
-  ivf_merge_warp(part + q * (long long)nprobe * k, nprobe, k, [&](int r, float key, int id) {
+  const float qn = warp_sq_norm(queries + q * dim, dim);
+  const Cand* mine = part + q * (long long)nprobe * k;
+  warp_merge<2>(k, [&](int l, int pos) {
+    return l < nprobe && pos < k ? mine[(long long)l * k + pos] : Cand{FLT_MAX, kNoId};
+  }, [&](int r, float key, int id, int) {
     if (lane == 0) {
-      float d;
-      if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);
-      else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);
-      else d = -key;
-      if (id == kNoId) d = metric == RECNN_METRIC_L2 ? FLT_MAX : -FLT_MAX;
       ids_out[q * k + r] = id == kNoId ? -1 : (int64_t)id;
-      dist_out[q * k + r] = d;
+      dist_out[q * k + r] = metric_distance(key, id, qn, metric);
     }
   });
 }

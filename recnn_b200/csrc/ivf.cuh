@@ -1,6 +1,6 @@
 // The pieces of the IVF index that IVF_FLAT (ivf.cu) and IVF_PQ (ivf_pq.cu) share: the coarse build (Lloyd k-means and
-// the inverted lists), the probe inversion of a search, the bulk copy that streams list storage and the per-query merge
-// of the probed lists.  The host functions live in ivf.cu; one copy of each.
+// the inverted lists), the probe inversion of a search and the bulk copy that streams list storage.  The host functions
+// live in ivf.cu; one copy of each.  Both merge a query's probed lists with topk.cuh's warp_merge.
 #pragma once
 
 #include <stddef.h>
@@ -81,25 +81,6 @@ __device__ __forceinline__ void bulk_copy(uint32_t dst, const void* src, uint32_
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
                : "memory");
-}
-
-// Called by a whole warp: merges one query's nprobe ascending lists of k candidates (mine[j * k + i]; lane owns lists
-// lane and lane + 32) and calls emit(r, key, id) in every lane for the r-th best, r = 0 .. k - 1.
-template <class Emit>
-__device__ __forceinline__ void ivf_merge_warp(const Cand* __restrict__ mine, int nprobe, int k, Emit emit) {
-  const int lane = threadIdx.x & 31;
-  int h0 = 0, h1 = 0;
-  for (int r = 0; r < k; ++r) {
-    float k0 = FLT_MAX, k1 = FLT_MAX; int i0 = kNoId, i1 = kNoId;
-    if (lane < nprobe && h0 < k) { const Cand c = mine[(long long)lane * k + h0]; k0 = c.key; i0 = c.id; }
-    if (lane + 32 < nprobe && h1 < k) { const Cand c = mine[(long long)(lane + 32) * k + h1]; k1 = c.key; i1 = c.id; }
-    const bool second = better(k1, i1, k0, i0);
-    float key = second ? k1 : k0;
-    int id = second ? i1 : i0, owner = lane;
-    warp_argmin(key, id, owner);
-    if (lane == owner) { if (second) ++h1; else ++h0; }
-    emit(r, key, id);
-  }
 }
 
 }  // namespace recnn

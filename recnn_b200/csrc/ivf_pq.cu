@@ -183,12 +183,7 @@ pq_scan_lists_kernel(const float* __restrict__ queries, int dim, int nprobe, int
     const long long q = warp < nq ? group[g0 + warp] / nprobe : -1;
     const float* qrow = queries + (q < 0 ? 0 : q) * dim;
     float inv = 1.0f;
-    if (metric == RECNN_METRIC_COS && q >= 0) {
-      float qn = 0.f;
-      for (int d = lane; d < dim; d += 32) { const float v = qrow[d]; qn = fmaf(v, v, qn); }
-      qn = warp_sum(qn);
-      inv = 1.0f / fmaxf(sqrtf(qn), 1e-30f);
-    }
+    if (metric == RECNN_METRIC_COS && q >= 0) inv = 1.0f / fmaxf(sqrtf(warp_sq_norm(qrow, dim)), 1e-30f);
     float* sq = s_q + warp * dim;
     for (int d = lane; d < dim; d += 32)
       sq[d] = q < 0 ? 0.f : (l2 ? qrow[d] - cl[d] : (metric == RECNN_METRIC_COS ? qrow[d] * inv : qrow[d]));
@@ -300,19 +295,18 @@ pq_scan_lists_kernel(const float* __restrict__ queries, int dim, int nprobe, int
 }
 
 // the exact key of (query row q, item id) by the instructions of ivf_scan_lists_kernel: an fp32 fma dot product in
-// ascending d, then retrieval's score_key with the item's norm
+// ascending d, then metric_key with the item's norm
 __device__ __forceinline__ float pq_exact_key(const float* __restrict__ q, const float* __restrict__ table, int dim,
                                               const float* __restrict__ norms, int metric, int id) {
   const float* x = table + (long long)id * dim;
   float s = 0.f;
   for (int d = 0; d < dim; ++d) s = fmaf(q[d], __ldg(x + d), s);
-  return finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + id))
-                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + id) : -s);
+  return metric_key(s, norms, id, metric);
 }
 
-// one warp per query: merge its nprobe ascending lists of k' into the k' best (ivf_merge_warp).  Without refine the
-// first k are written with their ADC distances; with refine the k' are re-scored exactly and the best k written,
-// finished as ivf_merge_kernel finishes them.
+// one warp per query: merge its nprobe <= 64 ascending lists of k' into the k' best (warp_merge, two lists per lane).
+// Without refine the first k are written with their ADC distances; with refine the k' are re-scored exactly and the
+// best k reported as the flat search reports them (metric_distance).
 __global__ void __launch_bounds__(128)
 pq_merge_kernel(const Cand* __restrict__ part, int nprobe, int kp, int k, bool refine, long long n_queries, int metric,
                 const float* __restrict__ queries, int dim, const float* __restrict__ table,
@@ -322,7 +316,10 @@ pq_merge_kernel(const Cand* __restrict__ part, int nprobe, int kp, int k, bool r
   const int lane = threadIdx.x & 31;
   if (q >= n_queries) return;
   Cand* best = s_best[threadIdx.x >> 5];
-  ivf_merge_warp(part + q * (long long)nprobe * kp, nprobe, kp, [&](int r, float key, int id) {
+  const Cand* mine = part + q * (long long)nprobe * kp;
+  warp_merge<2>(kp, [&](int l, int pos) {
+    return l < nprobe && pos < kp ? mine[(long long)l * kp + pos] : Cand{FLT_MAX, kNoId};
+  }, [&](int r, float key, int id, int) {
     if (lane == 0) { best[r].key = key; best[r].id = id; }
   });
   __syncwarp();
@@ -336,9 +333,7 @@ pq_merge_kernel(const Cand* __restrict__ part, int nprobe, int kp, int k, bool r
     return;
   }
   const float* qrow = queries + q * dim;
-  float qn = 0.f;
-  for (int d = lane; d < dim; d += 32) { const float v = qrow[d]; qn = fmaf(v, v, qn); }
-  qn = warp_sum(qn);
+  const float qn = warp_sq_norm(qrow, dim);
   float k0 = FLT_MAX, k1 = FLT_MAX;
   int i0 = kNoId, i1 = kNoId;
   if (lane < kp && best[lane].id != kNoId) { i0 = best[lane].id; k0 = pq_exact_key(qrow, table, dim, norms, metric, i0); }
@@ -355,13 +350,8 @@ pq_merge_kernel(const Cand* __restrict__ part, int nprobe, int kp, int k, bool r
       if (second) { k1 = FLT_MAX; i1 = kNoId; } else { k0 = FLT_MAX; i0 = kNoId; }
     }
     if (lane == 0) {
-      float d;
-      if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);
-      else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);
-      else d = -key;
-      if (id == kNoId) d = pad;
       ids_out[q * k + r] = id == kNoId ? -1 : (int64_t)id;
-      dist_out[q * k + r] = d;
+      dist_out[q * k + r] = metric_distance(key, id, qn, metric);
     }
   }
 }

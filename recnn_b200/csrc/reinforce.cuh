@@ -668,8 +668,6 @@ template <int KMAX, bool SETS, class Key>
 __global__ void __launch_bounds__(kTopkThreads)
 policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int id0, int k, ItemSets ex, int stage_cap,
                           const Cand* __restrict__ run, Cand* __restrict__ part, Key key_of) {
-  __shared__ float s_key[32];
-  __shared__ int s_id[32], s_owner[32];
   extern __shared__ int s_set[];
   const int sp = blockIdx.x, splits = gridDim.x;
   const int per = (w + splits - 1) / splits;
@@ -696,19 +694,7 @@ policy_topk_select_kernel(const float* __restrict__ z, long long n, int w, int i
           (!SETS || set.n == 0 || !set_has(set, s_set, id)))
         list_insert(keys, ids, key, id);
     }
-    // merge the CTA's sorted lists: rounds of arg-min over the heads, until k or every list is empty
-    Cand* out = part + (r * splits + sp) * k;
-    int head = 0, i = 0;
-    for (; i < k; ++i) {
-      float hk, wk;
-      int hid, wi, wo;
-      list_at(keys, ids, head, hk, hid);
-      block_argmin(hk, hid, s_key, s_id, s_owner, wk, wi, wo);
-      if (wi == kNoId) break;                               // the same decision in every thread
-      if ((int)threadIdx.x == wo) ++head;
-      if (threadIdx.x == 0) out[i] = Cand{wk, wi};
-    }
-    for (int j = i + threadIdx.x; j < k; j += blockDim.x) out[j] = Cand{FLT_MAX, kNoId};
+    block_merge(keys, ids, k, part + (r * splits + sp) * k);
     __syncthreads();                                        // s_set is refilled for the next row
   }
 }
@@ -722,19 +708,10 @@ policy_topk_merge_kernel(const Cand* __restrict__ run_in, const Cand* __restrict
   if (r >= n) return;
   const Cand* mine = lane == 0 ? run_in + r * k : part + (r * splits + lane - 1) * k;
   const bool has = lane <= splits;
-  int head = 0;
-  for (int i = 0; i < k; ++i) {
-    float key = FLT_MAX;
-    int id = kNoId, owner = lane;
-    if (has && head < k) {
-      const Cand c = mine[head];
-      key = c.key;
-      id = c.id;
-    }
-    warp_argmin(key, id, owner);
-    if (lane == owner) ++head;
-    if (lane == 0) run_out[r * k + i] = Cand{key, id};
-  }
+  warp_merge<1>(k, [&](int, int pos) { return has && pos < k ? mine[pos] : Cand{FLT_MAX, kNoId}; },
+                [&](int i, float key, int id, int) {
+                  if (lane == 0) run_out[r * k + i] = Cand{key, id};
+                });
 }
 
 // ids (-1 for an empty slot) and pi = exp(z - M) / S of the final lists
@@ -790,25 +767,20 @@ policy_topk_shard_finish_kernel(const float* __restrict__ g, long long n, int k,
   float M, S;
   shard_merge_stats(g, stride, W, n, r, M, S);
   const float* planes = shard_plane(g, n, 2, lane < W ? lane : 0, stride);
-  int head = 0;
-  for (int i = 0; i < k; ++i) {
-    float key = FLT_MAX;
-    int id = kNoId, owner = lane;
-    if (lane < W && head < k) {
-      const int v = __float_as_int(planes[(k + head) * n + r]);
-      if (v >= 0) {
-        key = -planes[head * n + r];
-        id = v;
-      }
+  warp_merge<1>(k, [&](int, int pos) {
+    Cand c = {FLT_MAX, kNoId};
+    if (lane < W && pos < k) {
+      const int v = __float_as_int(planes[(k + pos) * n + r]);
+      if (v >= 0) c = Cand{-planes[pos * n + r], v};
     }
-    warp_argmin(key, id, owner);
-    if (lane == owner) ++head;
+    return c;
+  }, [&](int i, float key, int id, int) {
     if (lane == 0) {
       const bool none = id == kNoId;
       ids[r * k + i] = none ? -1 : id;
       values[r * k + i] = none ? 0.f : expf(-key - M) / S;
     }
-  }
+  });
 }
 
 // ---- Sampled slates (serving): the select pass with GumbelKey.  Its lists hold perturbed keys, so a winner's value
@@ -898,27 +870,26 @@ policy_sample_shard_finish_kernel(const float* __restrict__ g, long long n, int 
   float M, S;
   shard_merge_stats(g, stride, W, n, r, M, S);
   const float* planes = shard_plane(g, n, 2, lane < W ? lane : 0, stride);
-  int head = 0;
-  for (int i = 0; i < k; ++i) {
-    float key = FLT_MAX, zc = 0.f;
-    int id = kNoId, owner = lane;
-    if (lane < W && head < k) {
-      const int v = __float_as_int(planes[(2 * k + head) * n + r]);
+  float zc;                                                 // the logit of this lane's head, read with its key
+  warp_merge<1>(k, [&](int, int pos) {
+    Cand c = {FLT_MAX, kNoId};
+    zc = 0.f;
+    if (lane < W && pos < k) {
+      const int v = __float_as_int(planes[(2 * k + pos) * n + r]);
       if (v >= 0) {
-        key = planes[head * n + r];
-        zc = planes[(k + head) * n + r];
-        id = v;
+        c = Cand{planes[pos * n + r], v};
+        zc = planes[(k + pos) * n + r];
       }
     }
-    warp_argmin(key, id, owner);
-    zc = __shfl_sync(0xffffffffu, zc, owner);
-    if (lane == owner) ++head;
+    return c;
+  }, [&](int i, float key, int id, int owner) {
+    const float z = __shfl_sync(0xffffffffu, zc, owner);
     if (lane == 0) {
       const bool none = id == kNoId;
       ids[r * k + i] = none ? -1 : id;
-      values[r * k + i] = none ? 0.f : expf(zc - M) / S;
+      values[r * k + i] = none ? 0.f : expf(z - M) / S;
     }
-  }
+  });
 }
 
 struct TopkWorkspace {

@@ -12,8 +12,8 @@
 //
 // Top-k: every CTA owns one (query, column range); each thread keeps the best k of its strided share in a sorted
 // register list (an element is compared with the list's worst first, so the insertion runs ~k ln(n/k) times);
-// the CTA then merges its 256 sorted lists by k rounds of a block arg-min over the list heads; a second tiny
-// kernel merges the column ranges of a query the same way.  Everything is exact (no approximate search).
+// the CTA then merges its 256 sorted lists (block_merge, topk.cuh); a second tiny kernel merges the column ranges of a
+// query (warp_merge) and reports the distances (metric_distance).  Everything is exact (no approximate search).
 #include <float.h>
 #include <string.h>
 
@@ -37,13 +37,6 @@ item_norms_kernel(const float* __restrict__ table, long long n_items, int dim, i
   if (lane == 0) out[row] = metric == RECNN_METRIC_COS ? 1.0f / fmaxf(sqrtf(s), 1e-30f) : s;
 }
 
-// the key of item j from its score: smaller is better; a NaN or +inf key ranks as FLT_MAX (finite_key), so the item is
-// still returned, after every finite key
-__device__ __forceinline__ float score_key(float s, const float* __restrict__ norms, long long j, int metric) {
-  return finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
-                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s);
-}
-
 // grid (splits, n_queries).  scores [n_queries, ld]; writes k candidates per (query, split), ascending.  Query q is
 // row row0 + q of the call; with SETS its excluded set (ex) is tested only for a candidate that enters the thread's
 // list (without, the kernel is the plain search, nothing staged).
@@ -51,8 +44,6 @@ template <int KMAX, bool SETS>
 __global__ void __launch_bounds__(kTopkThreads)
 topk_partial_kernel(const float* __restrict__ scores, long long ld, long long n_items, const float* __restrict__ norms,
                     int metric, int k, ItemSets ex, long long row0, int stage_cap, Cand* __restrict__ part) {
-  __shared__ float s_key[32];
-  __shared__ int s_id[32], s_owner[32];
   extern __shared__ int s_set[];
   const int q = blockIdx.y, sp = blockIdx.x, splits = gridDim.x;
   const long long per = (n_items + splits - 1) / splits;
@@ -67,57 +58,35 @@ topk_partial_kernel(const float* __restrict__ scores, long long ld, long long n_
   int ids[KMAX];
   list_clear(keys, ids);
   for (long long j = lo + threadIdx.x; j < hi; j += blockDim.x) {
-    const float key = score_key(__ldcs(row + j), norms, j, metric);
+    const float key = metric_key(__ldcs(row + j), norms, j, metric);
     int id = (int)j;
     if (better(key, id, keys[KMAX - 1], ids[KMAX - 1]) && (!SETS || set.n == 0 || !set_has(set, s_set, id)))
       list_insert(keys, ids, key, id);
   }
-  // merge the 256 sorted lists: k rounds of arg-min over the heads
-  int head = 0;
-  Cand* out = part + ((long long)q * splits + sp) * k;
-  for (int r = 0; r < k; ++r) {
-    float hk; int hid;
-    list_at(keys, ids, head, hk, hid);
-    float wk; int wi, wo;
-    block_argmin(hk, hid, s_key, s_id, s_owner, wk, wi, wo);
-    if ((int)threadIdx.x == wo) ++head;
-    if (threadIdx.x == 0) { out[r].key = wk; out[r].id = wi; }
-  }
+  block_merge(keys, ids, k, part + ((long long)q * splits + sp) * k);
 }
 
-// one warp per query: merge `splits` ascending lists of k candidates; finish the metric
+// one warp per query: merge `splits` <= 32 ascending lists of k candidates; finish the metric
 __global__ void __launch_bounds__(128)
 topk_merge_kernel(const Cand* __restrict__ part, int splits, int k, long long n_queries, int metric,
                   const float* __restrict__ queries, int dim, int64_t* __restrict__ ids_out, float* __restrict__ dist_out) {
   const long long q = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (q >= n_queries) return;
-  float qn = 0.f;
-  for (int d = lane; d < dim; d += 32) { const float v = queries[q * dim + d]; qn = fmaf(v, v, qn); }
-  qn = warp_sum(qn);
+  const float qn = warp_sq_norm(queries + q * dim, dim);
   const Cand* mine = part + q * (long long)splits * k;
-  // lane l walks lists l, l+32, ...: keeps one head per owned list in a small loop (splits <= 32 in practice)
-  int head = 0;                                      // lane's position in list `lane` (splits <= 32)
-  for (int r = 0; r < k; ++r) {
-    float key = FLT_MAX; int id = kNoId;
-    if (lane < splits && head < k) { key = mine[(long long)lane * k + head].key; id = mine[(long long)lane * k + head].id; }
-    int owner = lane;
-    warp_argmin(key, id, owner);
-    if (lane == owner) ++head;
+  warp_merge<1>(k, [&](int l, int pos) {
+    return l < splits && pos < k ? mine[(long long)l * k + pos] : Cand{FLT_MAX, kNoId};
+  }, [&](int r, float key, int id, int) {
     if (lane == 0) {
-      float d;
-      if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);                 // squared L2 distance
-      else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);  // cosine similarity
-      else d = -key;                                                           // inner product
-      if (id == kNoId) d = metric == RECNN_METRIC_L2 ? FLT_MAX : -FLT_MAX;       // fewer than k eligible items
       ids_out[q * k + r] = id == kNoId ? -1 : (int64_t)id;
-      dist_out[q * k + r] = d;
+      dist_out[q * k + r] = metric_distance(key, id, qn, metric);
     }
-  }
+  });
 }
 
 // grid (splits, n_queries): rank[row0 + q] += the items of columns [lo, hi) that beat the query's target by
-// score_key (ties: the smaller id), minus the excluded ones (SETS).  The target's key is read from the same scores row,
+// metric_key (ties: the smaller id), minus the excluded ones (SETS).  The target's key is read from the same scores row,
 // so every comparison is between the bits the search ranks.  A target outside [0, n_items) counts nothing.
 template <bool SETS>
 __global__ void __launch_bounds__(kTopkThreads)
@@ -131,13 +100,13 @@ rank_count_kernel(const float* __restrict__ scores, long long ld, long long n_it
   const long long t = target[row0 + q];
   if (t < 0 || t >= n_items) return;
   const float* row = scores + (long long)q * ld;
-  const float kt = score_key(row[t], norms, t, metric);
+  const float kt = metric_key(row[t], norms, t, metric);
   int c = 0;
   for (long long j = lo + threadIdx.x; j < hi; j += blockDim.x)
-    c += j != t && better(score_key(__ldcs(row + j), norms, j, metric), (int)j, kt, (int)t);
+    c += j != t && better(metric_key(__ldcs(row + j), norms, j, metric), (int)j, kt, (int)t);
   if (SETS)
     c -= excluded_beaters(ex, row0 + q, lo, hi, kt, (int)t,
-                          [&](long long x) { return score_key(row[x], norms, x, metric); }, s_range);
+                          [&](long long x) { return metric_key(row[x], norms, x, metric); }, s_range);
   c = __reduce_add_sync(0xffffffffu, c);
   if ((threadIdx.x & 31) == 0 && c != 0)
     atomicAdd(reinterpret_cast<unsigned long long*>(rank + row0 + q), (unsigned long long)(long long)c);

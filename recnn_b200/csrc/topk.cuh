@@ -1,7 +1,11 @@
-// Exact top-k building blocks shared by nearest-item retrieval (retrieval.cu) and the REINFORCE policy's top-k
-// (reinforce.cuh): a candidate is (key, id), smaller key first, ties towards the smaller id (== a stable argsort of the
-// keys).  Each thread keeps the best KMAX of its share in a sorted register list; a CTA merges its lists by rounds of a
-// block arg-min over the list heads.  Every selector builds its keys through finite_key: NaN and +inf rank as FLT_MAX.
+// Exact top-k building blocks shared by every selector: nearest-item retrieval (retrieval.cu, ivf.cu, ivf_pq.cu), the
+// REINFORCE policy's top-k and sampled slates (reinforce.cuh) and Q-scored critic serving (critic_serve.cuh).  A
+// candidate is (key, id), smaller key first, ties towards the smaller id (== a stable argsort of the keys); an empty
+// slot is {FLT_MAX, kNoId}.  Every selector builds its keys through finite_key (NaN and +inf rank as FLT_MAX), and the
+// retrieval ones through metric_key, so that a flat search, an IVF search probing every list and a rank see the same
+// key bits.  Each thread keeps the best KMAX of its share in a sorted register list; a CTA merges its lists with
+// block_merge, and a warp merges sorted lists in memory (the CTAs' outputs) with warp_merge.  The retrieval merges
+// report a key as a distance through metric_distance.
 #pragma once
 
 #include <float.h>
@@ -105,6 +109,79 @@ __device__ __forceinline__ void list_at(const float (&keys)[KMAX], const int (&i
   k = FLT_MAX; id = kNoId;
 #pragma unroll
   for (int i = 0; i < KMAX; ++i) if (i == head) { k = keys[i]; id = ids[i]; }
+}
+
+// Called by every thread of the CTA: merges the threads' sorted register lists into out[0, k), ascending, by rounds of
+// block_argmin over the list heads; thread 0 writes each winner.  Once a round's winner is an empty slot every list is
+// exhausted (a real candidate, NaN-keyed included, has a real id), so the rounds stop there and the rest of out is
+// padded with empty slots: the bytes k rounds would write.
+template <int KMAX>
+__device__ __forceinline__ void block_merge(const float (&keys)[KMAX], const int (&ids)[KMAX], int k, Cand* out) {
+  __shared__ float s_key[32];
+  __shared__ int s_id[32], s_owner[32];
+  int head = 0, i = 0;
+  for (; i < k; ++i) {
+    float hk, wk;
+    int hid, wi, wo;
+    list_at(keys, ids, head, hk, hid);
+    block_argmin(hk, hid, s_key, s_id, s_owner, wk, wi, wo);
+    if (wi == kNoId) break;                               // the same decision in every thread
+    if ((int)threadIdx.x == wo) ++head;
+    if (threadIdx.x == 0) out[i] = Cand{wk, wi};
+  }
+  for (int j = i + threadIdx.x; j < k; j += blockDim.x) out[j] = Cand{FLT_MAX, kNoId};
+}
+
+// Called by a whole warp: the k best of up to 32 * LISTS sorted candidate lists, lane l owning lists l, l + 32, ...
+// read(list, pos) returns entry pos of a list, {FLT_MAX, kNoId} past its end or for a list that does not exist; it is
+// called once per list a lane owns in every round, before the round's arg-min.  emit(i, key, id, owner) runs in every
+// lane for the i-th best, i = 0 .. k - 1, owner being the lane whose list held it.
+template <int LISTS, class Read, class Emit>
+__device__ __forceinline__ void warp_merge(int k, Read read, Emit emit) {
+  const int lane = threadIdx.x & 31;
+  int head[LISTS];
+#pragma unroll
+  for (int l = 0; l < LISTS; ++l) head[l] = 0;
+  for (int i = 0; i < k; ++i) {
+    Cand c = read(lane, head[0]);
+    int from = 0;
+#pragma unroll
+    for (int l = 1; l < LISTS; ++l) {
+      const Cand o = read(lane + 32 * l, head[l]);
+      if (better(o.key, o.id, c.key, c.id)) { c = o; from = l; }
+    }
+    int owner = lane;
+    warp_argmin(c.key, c.id, owner);
+#pragma unroll
+    for (int l = 0; l < LISTS; ++l) if (lane == owner && l == from) ++head[l];
+    emit(i, c.key, c.id, owner);
+  }
+}
+
+// The ranking key of item j with inner product s under a retrieval metric: |t_j|^2 - 2 s (L2, norms[j] = |t_j|^2),
+// -s / |t_j| (COS, norms[j] = 1 / |t_j|), -s (IP: norms is not read and may be NULL).  Every retrieval search and rank
+// keys its items here, so their results agree bit for bit.
+__device__ __forceinline__ float metric_key(float s, const float* __restrict__ norms, long long j, int metric) {
+  return finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
+                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s);
+}
+
+// Called by a whole warp: |row|^2, lane l summing d = l, l + 32, ... by fma, then the butterfly sum; in every lane
+__device__ __forceinline__ float warp_sq_norm(const float* row, int dim) {
+  float s = 0.f;
+  for (int d = threadIdx.x & 31; d < dim; d += 32) { const float v = row[d]; s = fmaf(v, v, s); }
+  return warp_sum(s);
+}
+
+// The distance a search reports for a metric_key key, qn = |query|^2: the squared L2 distance, the inner product or the
+// cosine similarity; an empty slot (fewer than k eligible items) reports FLT_MAX (L2) or -FLT_MAX.
+__device__ __forceinline__ float metric_distance(float key, int id, float qn, int metric) {
+  float d;
+  if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);
+  else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);
+  else d = -key;
+  if (id == kNoId) d = metric == RECNN_METRIC_L2 ? FLT_MAX : -FLT_MAX;
+  return d;
 }
 
 // ---- Item-set exclusion: the ids a row must never return ----------------------------------------------------------
