@@ -80,12 +80,12 @@ __global__ void __launch_bounds__(kRowThreads) softmax_rows_kernel(float* __rest
       if (x > m) {
         s = s * __expf(m - x) + 1.f;      // m == -inf: s == 0, exp(-inf) == 0
         m = x;
-      } else {
+      } else if (x != -INFINITY) {        // a -inf logit adds exp(-inf) = 0, and NaN = exp(-inf - -inf) while m is -inf
         s += __expf(x - m);
       }
     }
     const float M = block_max(m, red);
-    s = (m == -INFINITY) ? 0.f : s * __expf(m - M);
+    s = (m == -INFINITY) ? s : s * __expf(m - M);   // no finite logit: s is 0, or NaN after a NaN logit (kept)
     const float S = block_sum(s, red);
     for (int j = threadIdx.x; j < items; j += blockDim.x) row[j] = expf(row[j] - M) / S;
     __syncthreads();
@@ -213,12 +213,12 @@ logit_stats_kernel(const float* __restrict__ z, long long ld, long long n, int w
       if (x > m) {
         s = s * __expf(m - x) + 1.f;
         m = x;
-      } else {
+      } else if (x != -INFINITY) {
         s += __expf(x - m);
       }
     }
     const float M = block_max(m, red);
-    s = (m == -INFINITY) ? 0.f : s * __expf(m - M);
+    s = (m == -INFINITY) ? s : s * __expf(m - M);
     const float S = block_sum(s, red);
     if (threadIdx.x == 0) {
       if (c0 == 0) {
@@ -226,7 +226,8 @@ logit_stats_kernel(const float* __restrict__ z, long long ld, long long n, int w
         run_sum[r] = S;
       } else {
         const float M0 = run_max[r], Mn = fmaxf(M0, M);
-        run_sum[r] = run_sum[r] * expf(M0 - Mn) + S * expf(M - Mn);
+        // no finite logit yet (M0 == M == -inf): both sums are 0, and exp(-inf - -inf) would make them NaN
+        run_sum[r] = Mn == -INFINITY ? 0.f : run_sum[r] * expf(M0 - Mn) + S * expf(M - Mn);
         run_max[r] = Mn;
       }
       if (action) {
