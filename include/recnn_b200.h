@@ -325,13 +325,38 @@ RECNN_API int recnn_optimizer_step(const recnn_optim* o, const recnn_net* net, i
  * (MilvusConnection.search(search_vecs, topk) -> ids, distances).  Exact search: one
  * [n_queries, dim] x [dim, n_items] contraction on the tensor cores (3xTF32) + an exact top-k.
  * Ordering: best first; L2 reports the squared distance (as faiss / Milvus do), IP the inner product,
- * COS the cosine similarity; ties go to the smaller item id.  k <= 64. */
-enum { RECNN_METRIC_L2 = 0, RECNN_METRIC_IP = 1, RECNN_METRIC_COS = 2 };
-/* out[n_items]: |item|^2 (L2) or 1/|item| (COS); computed once per table ("index build") */
+ * COS the cosine similarity; ties go to the smaller item id.  k <= 64.
+ *
+ * The scipy.spatial.distance metrics of examples/streamlit_demo.py:207-230 that are not inner products (codes 3-7) are
+ * computed on the CUDA cores, one thread per (query q, item t) pair, summing over d ascending; the library builds
+ * without fast math, so each step is one IEEE fp32 operation.  Their distance is their key: smallest first, reported
+ * as computed, NaN and +inf ranked and reported as FLT_MAX (after every finite distance, before a -1 pad, which
+ * reports FLT_MAX too).  Only the flat search and rank take them (the IVF / IVF_PQ calls refuse them).
+ *   L1         (cityblock)   acc += |q_d - t_d|
+ *   LINF       (chebyshev)   acc = max(acc, |q_d - t_d|), NaN-propagating (PTX max.NaN), so a NaN row ranks last
+ *   CANBERRA                 acc += |q_d - t_d| / (|q_d| + |t_d|), a term with a zero denominator 0 (scipy's rule)
+ *   BRAYCURTIS               num += |q_d - t_d|, den += |q_d + t_d|; num == 0 ? 0 : num / den (den == 0 < num: +inf)
+ *   CORR       (correlation) 1 - r clipped to [0, 2] (NaN kept): r = dot / (|q_c| |t_c|), 0 when that product is 0,
+ *                            dot = fma over d of q_c,d t_c,d where x_c,d = x_d - mean(x); a constant row (every x_d
+ *                            equal) has mean x_0 and centred norm 0, so its distance to anything is 1.  mean(x) is
+ *                            (sum of x_d, ascending) / dim, |x_c| = sqrt(fma-sum of x_c,d^2, ascending). */
+enum {
+  RECNN_METRIC_L2 = 0,
+  RECNN_METRIC_IP = 1,
+  RECNN_METRIC_COS = 2,
+  RECNN_METRIC_L1 = 3,          /* cityblock (Manhattan) distance */
+  RECNN_METRIC_LINF = 4,        /* Chebyshev distance */
+  RECNN_METRIC_CANBERRA = 5,    /* Canberra distance */
+  RECNN_METRIC_BRAYCURTIS = 6,  /* Bray-Curtis dissimilarity */
+  RECNN_METRIC_CORR = 7         /* correlation distance, 1 - Pearson r; needs recnn_item_norms */
+};
+/* Computed once per table ("index build"): out[n_items] = |item|^2 (L2) or 1/|item| (COS); for CORR out[2 * n_items]
+ * = the item means, then the items' centred norms |t_c| (see above).  The other metrics take no norms (NULL). */
 RECNN_API int recnn_item_norms(const float* table, int64_t n_items, int32_t dim, int32_t metric, float* out,
                                void* stream);
 RECNN_API int64_t recnn_retrieve_workspace_bytes(int64_t n_queries, int64_t n_items, int32_t k);
-/* ids_out int64[n_queries, k], dist_out fp32[n_queries, k]; norms from recnn_item_norms (NULL for IP);
+/* ids_out int64[n_queries, k], dist_out fp32[n_queries, k]; norms from recnn_item_norms (NULL for IP, L1, LINF,
+ * CANBERRA, BRAYCURTIS); the workspace is the same for every metric;
  * workspace: any address, workspace_bytes >= recnn_retrieve_workspace_bytes (else RECNN_E_WORKSPACE) */
 RECNN_API int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32_t dim, const float* table,
                                   int64_t n_items, const float* norms, int32_t metric, int32_t k,
@@ -347,7 +372,8 @@ RECNN_API int recnn_retrieve_topk(const float* queries, int64_t n_queries, int32
  * global memory, and only for a candidate that would enter a row's list.
  *
  * recnn_retrieve_topk with exclusion: the ids of row q's set are never returned.  A row with fewer than k eligible
- * items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  Every row_set -1: recnn_retrieve_topk's bits.
+ * items ends in id -1, distance -FLT_MAX (IP, COS) or FLT_MAX (the others).  Every row_set -1: recnn_retrieve_topk's
+ * bits.
  * Same workspace. */
 RECNN_API int recnn_retrieve_topk_sets(const float* queries, int64_t n_queries, int32_t dim, const float* table,
                                        int64_t n_items, const float* norms, int32_t metric, int32_t k,

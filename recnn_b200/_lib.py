@@ -19,6 +19,7 @@ PH_ALL = 255
 ALGO_DDPG, ALGO_TD3 = 0, 1
 OPT_EXTERNAL, OPT_SGD, OPT_ADAM, OPT_RANGER, OPT_RADAM = 0, 1, 2, 3, 4
 METRIC_L2, METRIC_IP, METRIC_COS = 0, 1, 2
+METRIC_L1, METRIC_LINF, METRIC_CANBERRA, METRIC_BRAYCURTIS, METRIC_CORR = 3, 4, 5, 6, 7
 REINFORCE_BASIC, REINFORCE_CORRECTED, REINFORCE_TOPK = 0, 1, 2
 
 

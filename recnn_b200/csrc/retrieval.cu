@@ -18,6 +18,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "distance.cuh"
 #include "gemm_simt.cuh"
 #include "tc_gemm.cuh"
 #include "topk.cuh"
@@ -155,7 +156,14 @@ using namespace recnn;
 extern "C" int recnn_item_norms(const float* table, int64_t n_items, int32_t dim, int32_t metric, float* out,
                                 void* stream) {
   RECNN_REQUIRE(table && out && n_items > 0 && dim > 0, "table/out");
-  RECNN_REQUIRE(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_COS, "norms exist for L2 and COS");
+  RECNN_REQUIRE(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_COS || metric == RECNN_METRIC_CORR,
+                "norms exist for L2, COS and CORR");
+  if (metric == RECNN_METRIC_CORR) {
+    corr_stats_kernel<<<(unsigned)ceil_div(n_items, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(table, n_items,
+                                                                                                       dim, out);
+    RECNN_CHECK_LAUNCH("corr_stats_kernel");
+    return RECNN_OK;
+  }
   const int64_t blocks = ceil_div(n_items, 8);
   item_norms_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(table, n_items, dim, metric, out);
   RECNN_CHECK_LAUNCH("item_norms_kernel");
@@ -168,16 +176,23 @@ extern "C" int64_t recnn_retrieve_workspace_bytes(int64_t n_queries, int64_t n_i
 }
 
 // The slab loop of every retrieval call: for each slab of up to w.slab query rows, scores[q, j] = <query q0 + q,
-// item j> into w.scores (the tensor-core GEMM when the operands allow it, else the CUDA-core one: one choice per call),
-// then after(q0, nq) reads the slab.  A search and a rank over the same queries see the same score bits.
+// item j> into w.scores for L2 / IP / COS (the tensor-core GEMM when the operands allow it, else the CUDA-core one: one
+// choice per call), the distance of the pair for the other metrics (distance.cuh), then after(q0, nq) reads the slab.
+// A search and a rank over the same queries see the same score bits.
 template <class After>
 static int retrieve_slabs(const float* queries, int64_t n_queries, int32_t dim, const float* table, int64_t n_items,
-                          const RetrieveWorkspace& w, cudaStream_t st, After after) {
+                          const float* norms, int32_t metric, const RetrieveWorkspace& w, cudaStream_t st,
+                          After after) {
   const bool tc_ok = dim % 4 == 0 && (reinterpret_cast<uintptr_t>(queries) & 15) == 0 &&
                      (reinterpret_cast<uintptr_t>(table) & 15) == 0;
   for (int64_t q0 = 0; q0 < n_queries; q0 += w.slab) {
     const int64_t nq = n_queries - q0 < w.slab ? n_queries - q0 : w.slab;
     const float* Q = queries + q0 * dim;
+    if (metric >= RECNN_METRIC_L1) {
+      RECNN_PROPAGATE(distance_slab(metric, Q, nq, table, n_items, dim, norms, w.scores, w.ld, st));
+      RECNN_PROPAGATE(after(q0, nq));
+      continue;
+    }
     Epilogue e;
     memset(&e, 0, sizeof(e));
     e.out = w.scores;
@@ -203,8 +218,9 @@ static int retrieve_check(const float* queries, int64_t n_queries, int32_t dim, 
                           const float* norms, int32_t metric, const void* workspace) {
   RECNN_REQUIRE(queries && table && workspace, "null pointer");
   RECNN_REQUIRE(n_queries >= 0 && n_items > 0 && dim > 0, "sizes");
-  RECNN_REQUIRE(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_IP || metric == RECNN_METRIC_COS, "metric");
-  RECNN_REQUIRE(metric == RECNN_METRIC_IP || norms != nullptr, "L2 / COS need recnn_item_norms");
+  RECNN_REQUIRE(metric >= RECNN_METRIC_L2 && metric <= RECNN_METRIC_CORR, "metric");
+  RECNN_REQUIRE(!(metric == RECNN_METRIC_L2 || metric == RECNN_METRIC_COS || metric == RECNN_METRIC_CORR) ||
+                norms != nullptr, "L2 / COS / CORR need recnn_item_norms");
   RECNN_REQUIRE(n_items < (1ll << 31), "n_items must fit int32");
   return RECNN_OK;
 }
@@ -230,7 +246,7 @@ static int retrieve(const float* queries, int64_t n_queries, int32_t dim, const 
   const int stage = set_stage_bytes(ex);
   auto kernel = k <= 16 ? (stage ? topk_partial_kernel<16, true> : topk_partial_kernel<16, false>)
                         : (stage ? topk_partial_kernel<64, true> : topk_partial_kernel<64, false>);
-  return retrieve_slabs(queries, n_queries, dim, table, n_items, w, st, [&](int64_t q0, int64_t nq) {
+  return retrieve_slabs(queries, n_queries, dim, table, n_items, norms, metric, w, st, [&](int64_t q0, int64_t nq) {
     const float* Q = queries + q0 * dim;
     const int splits = topk_splits(nq, n_items, 32);
     dim3 grid((unsigned)splits, (unsigned)nq);
@@ -266,7 +282,7 @@ static int retrieve_rank(const float* queries, int64_t n_queries, int32_t dim, c
   rank_init_kernel<<<(unsigned)ceil_div(n_queries, 256), 256, 0, st>>>(tgt, n_queries, n_items, rank, error_flag);
   RECNN_CHECK_LAUNCH("rank_init_kernel");
   auto kernel = ex.ids ? rank_count_kernel<true> : rank_count_kernel<false>;
-  return retrieve_slabs(queries, n_queries, dim, table, n_items, w, st, [&](int64_t q0, int64_t nq) {
+  return retrieve_slabs(queries, n_queries, dim, table, n_items, norms, metric, w, st, [&](int64_t q0, int64_t nq) {
     dim3 grid((unsigned)topk_splits(nq, n_items, 32), (unsigned)nq);
     kernel<<<grid, kTopkThreads, 0, st>>>(w.scores, w.ld, n_items, norms, metric, tgt, ex, q0, rank);
     RECNN_CHECK_LAUNCH("rank_count_kernel");

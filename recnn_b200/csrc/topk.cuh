@@ -159,11 +159,13 @@ __device__ __forceinline__ void warp_merge(int k, Read read, Emit emit) {
 }
 
 // The ranking key of item j with inner product s under a retrieval metric: |t_j|^2 - 2 s (L2, norms[j] = |t_j|^2),
-// -s / |t_j| (COS, norms[j] = 1 / |t_j|), -s (IP: norms is not read and may be NULL).  Every retrieval search and rank
-// keys its items here, so their results agree bit for bit.
+// -s / |t_j| (COS, norms[j] = 1 / |t_j|), -s (IP: norms is not read and may be NULL); for the metrics from L1 on, s is
+// already the distance (distance.cuh) and is its own key.  Every retrieval search and rank keys its items here, so
+// their results agree bit for bit.
 __device__ __forceinline__ float metric_key(float s, const float* __restrict__ norms, long long j, int metric) {
   return finite_key(metric == RECNN_METRIC_L2 ? fmaf(-2.0f, s, __ldg(norms + j))
-                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j) : -s);
+                    : metric == RECNN_METRIC_COS ? -s * __ldg(norms + j)
+                    : metric == RECNN_METRIC_IP ? -s : s);
 }
 
 // Called by a whole warp: |row|^2, lane l summing d = l, l + 32, ... by fma, then the butterfly sum; in every lane
@@ -173,14 +175,16 @@ __device__ __forceinline__ float warp_sq_norm(const float* row, int dim) {
   return warp_sum(s);
 }
 
-// The distance a search reports for a metric_key key, qn = |query|^2: the squared L2 distance, the inner product or the
-// cosine similarity; an empty slot (fewer than k eligible items) reports FLT_MAX (L2) or -FLT_MAX.
+// The distance a search reports for a metric_key key, qn = |query|^2: the squared L2 distance, the inner product, the
+// cosine similarity, or the key itself for the metrics from L1 on; an empty slot (fewer than k eligible items) reports
+// -FLT_MAX (IP, COS) or FLT_MAX (the others).
 __device__ __forceinline__ float metric_distance(float key, int id, float qn, int metric) {
   float d;
   if (metric == RECNN_METRIC_L2) d = fmaxf(key + qn, 0.f);
   else if (metric == RECNN_METRIC_COS) d = -key / fmaxf(sqrtf(qn), 1e-30f);
-  else d = -key;
-  if (id == kNoId) d = metric == RECNN_METRIC_L2 ? FLT_MAX : -FLT_MAX;
+  else if (metric == RECNN_METRIC_IP) d = -key;
+  else d = key;
+  if (id == kNoId) d = metric == RECNN_METRIC_IP || metric == RECNN_METRIC_COS ? -FLT_MAX : FLT_MAX;
   return d;
 }
 

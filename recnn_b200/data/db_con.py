@@ -23,6 +23,13 @@ stays exact, so recall can be measured against it or against a flat index.
 ``build_ivf(nlist, m=M)`` builds IVF_PQ instead: the same lists, each item
 stored as M one-byte codes of its residual, scanned through lookup tables and
 optionally re-ranked exactly from the table (``search_param={"refine": r}``).
+
+``ItemIndex`` also takes the eight ``scipy.spatial.distance`` names the reference
+demo ranks by (examples/streamlit_demo.py:207-230, 319-345), so that its
+``rank(action, distance.<name>, k)`` is ``ItemIndex(table, name).search(action, k)``:
+"euclidean" and "cosine" run on L2 and COS, "cityblock", "chebyshev",
+"canberra", "braycurtis" and "correlation" on CUDA-core distance kernels
+(recnn_b200.h documents their fp32 arithmetic), "minkowski" on one of them by p.
 """
 from __future__ import annotations
 
@@ -34,6 +41,27 @@ import torch
 from .. import _lib
 
 _METRICS = {"L2": _lib.METRIC_L2, "IP": _lib.METRIC_IP, "COS": _lib.METRIC_COS}
+# scipy.spatial.distance names -> the metric that ranks them; "euclidean" reports sqrt of L2's squared distance and
+# "cosine" 1 - COS's similarity, the others report the kernel's distance as it is
+_SCIPY = {"euclidean": _lib.METRIC_L2, "cosine": _lib.METRIC_COS, "cityblock": _lib.METRIC_L1,
+          "chebyshev": _lib.METRIC_LINF, "canberra": _lib.METRIC_CANBERRA, "braycurtis": _lib.METRIC_BRAYCURTIS,
+          "correlation": _lib.METRIC_CORR}
+_MINKOWSKI = {1.0: "cityblock", 2.0: "euclidean", float("inf"): "chebyshev"}
+_FLT_MAX = float(torch.finfo(torch.float32).max)
+
+
+def _metric_name(metric, p):
+    """the name in _METRICS or _SCIPY that metric (and minkowski's p) stands for"""
+    if metric == "minkowski":
+        p = 2.0 if p is None else float(p)
+        if p not in _MINKOWSKI:
+            raise ValueError("minkowski is served for p = 1, 2 and inf only (got p = %r)" % (p,))
+        return _MINKOWSKI[p]
+    if metric not in _METRICS and metric not in _SCIPY:
+        raise ValueError("metric must be one of %s" % sorted(list(_METRICS) + list(_SCIPY) + ["minkowski"]))
+    if p is not None:
+        raise ValueError("p is minkowski's order; metric %s takes none" % metric)
+    return metric
 
 
 class SearchResult:
@@ -94,32 +122,57 @@ class ItemIndex:
     """Exact top-k search over an item-embedding matrix resident on one GPU.
 
     metric: "L2" (squared Euclidean distance, smallest first -- faiss IndexFlatL2 / Milvus L2),
-            "IP" (inner product, largest first), "COS" (cosine similarity, largest first).
+            "IP" (inner product, largest first), "COS" (cosine similarity, largest first), or a
+            scipy.spatial.distance name, smallest first, distances as scipy reports them up to fp32 rounding:
+            "euclidean", "cosine" (1 - similarity, clipped to [0, 2]), "cityblock", "chebyshev", "canberra",
+            "braycurtis", "correlation", or "minkowski" with ``p`` 1, 2 (the default, as in scipy) or inf, which
+            is cityblock, euclidean or chebyshev.  Where scipy gives NaN, Bray-Curtis of two zero rows is 0 and
+            correlation with a constant row is 1; a distance that is NaN or +inf (a NaN row, an overflow, Bray-Curtis
+            of t = -q != 0) ranks and reports as FLT_MAX.
 
     ``build_ivf`` turns ``search`` into an IVF_FLAT search (see there); the index is a snapshot of the table at build
-    time, which RecNN's workflows keep fixed.
+    time, which RecNN's workflows keep fixed.  The k-means lists are L2 objects: an index over cityblock, chebyshev,
+    canberra, braycurtis or correlation has none.
     """
 
-    def __init__(self, embeddings, metric="L2"):
-        if metric not in _METRICS:
-            raise ValueError("metric must be one of %s" % sorted(_METRICS))
+    def __init__(self, embeddings, metric="L2", p=None):
+        name = _metric_name(metric, p)
         if not torch.is_tensor(embeddings):
             embeddings = torch.as_tensor(embeddings)
         if embeddings.device.type != "cuda":
             raise _lib.RecnnError("ItemIndex needs the embedding table on a CUDA device (got %s); there is no CPU path"
                                   % embeddings.device)
         self.table = embeddings.detach().to(torch.float32).contiguous()
-        self.metric_name, self.metric = metric, _METRICS[metric]
+        self.metric_name, self.metric = metric, _METRICS.get(name, _SCIPY.get(name))
+        self._scipy = name if name in _SCIPY else None
         self.device = self.table.device
         self.n_items, self.dim = int(self.table.shape[0]), int(self.table.shape[1])
         self.norms = None
-        if self.metric != _lib.METRIC_IP:
-            self.norms = torch.empty(self.n_items, dtype=torch.float32, device=self.device)
+        if self.metric in (_lib.METRIC_L2, _lib.METRIC_COS, _lib.METRIC_CORR):
+            # CORR: the item means, then the centred norms
+            n = 2 * self.n_items if self.metric == _lib.METRIC_CORR else self.n_items
+            self.norms = torch.empty(n, dtype=torch.float32, device=self.device)
             with torch.cuda.device(self.device):
                 _lib.check(_lib.lib().recnn_item_norms(self.table.data_ptr(), self.n_items, self.dim, self.metric,
                                                        self.norms.data_ptr(), _lib.stream_ptr(self.device)))
         self._ws = None
         self._ivf = None
+
+    def _result(self, ids, dist):
+        """SearchResult, the distances converted for "euclidean" and "cosine"; a -1 pad reports FLT_MAX under every
+        scipy name"""
+        if self._scipy is not None:
+            if self._scipy == "euclidean":
+                dist = torch.sqrt(dist)
+            elif self._scipy == "cosine":
+                dist = torch.clamp(1.0 - dist, 0.0, 2.0)
+            dist = torch.where(ids < 0, torch.full_like(dist, _FLT_MAX), dist)
+        return SearchResult(ids, dist)
+
+    def _ivf_metric_check(self):
+        if self.metric not in _METRICS.values():
+            raise ValueError("an IVF index needs metric L2, IP or COS (or euclidean / cosine); its k-means lists do not "
+                             "describe %s" % self.metric_name)
 
     # ------------------------------------------------------------------------------------------------ IVF index
     @property
@@ -166,6 +219,7 @@ class ItemIndex:
         Lloyd rounds (the coarse build's) on the residuals of the first min(len(sample), 65536) sample points, from the
         codewords ``ivf_pq_sample(len(sample), seed)`` picks; each code is the nearest codeword (fp32, ties to the
         smaller code).  See ``search`` for how the codes are scored."""
+        self._ivf_metric_check()
         nlist, n_iter, mppc = int(nlist), int(n_iter), int(max_points_per_centroid)
         if not 1 <= nlist <= self.n_items:
             raise ValueError("nlist must be in [1, n_items = %d] (got %d)" % (self.n_items, nlist))
@@ -264,6 +318,7 @@ class ItemIndex:
             params = dict(state["params"])
         except (KeyError, TypeError) as e:
             raise ValueError("not an ivf_state() dict: %s" % e)
+        self._ivf_metric_check()
         m = params.get("m")
         if m is not None:
             if not isinstance(m, int):
@@ -353,9 +408,9 @@ class ItemIndex:
         """search_vecs: [n, dim] (tensor / array on any device).  Returns SearchResult on the index's device.
         ``exclude``: an ``ItemSets`` of item ids never returned (e.g. ``DeviceFrameFeed.seen_items()``), with
         ``exclude_rows`` int64 [n] naming each query's set (-1: none; default query r -> set r).  A query with fewer
-        than topk eligible items ends in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS).  An item whose key is NaN
-        or +inf (a NaN row, an overflowing |t|^2 or score) ranks as key FLT_MAX: after every finite key, ties by id, and
-        before any -1.  An excluded id outside [0, n_items) raises IndexError, a malformed table ValueError.
+        than topk eligible items ends in id -1, distance -FLT_MAX (IP, COS) or FLT_MAX (L2 and every scipy name).  An
+        item whose key is NaN or +inf (a NaN row, an overflowing |t|^2, score or distance) ranks as key FLT_MAX: after
+        every finite key, ties by id, and before any -1.  An excluded id outside [0, n_items) raises IndexError, a malformed table ValueError.
 
         Without an IVF index the search is exact and ``search_param`` is ignored.  After ``build_ivf`` / ``load_ivf``
         it is the IVF_FLAT search: ``search_param={"nprobe": p}`` (default 16, at most min(nlist, 64); any other key
@@ -405,7 +460,7 @@ class ItemIndex:
             if sets is None:
                 _lib.check(L.recnn_retrieve_topk(*args, ids.data_ptr(), dist.data_ptr(), self._ws.data_ptr(),
                                                  self._ws.numel(), _lib.stream_ptr(self.device)))
-                return SearchResult(ids, dist)
+                return self._result(ids, dist)
             sets = sets.to(self.device)
             rows = None if rows is None else rows.to(self.device).contiguous()
             flag = torch.empty(1, dtype=torch.int32, device=self.device)
@@ -415,7 +470,7 @@ class ItemIndex:
                                                   self._ws.data_ptr(), self._ws.numel(),
                                                   _lib.stream_ptr(self.device)))
         self._raise_set_bits(int(flag.item()), len(sets))
-        return SearchResult(ids, dist)
+        return self._result(ids, dist)
 
     def _raise_set_bits(self, bits, n_sets):
         if bits & 1:
@@ -454,7 +509,7 @@ class ItemIndex:
                 _lib.check(L.recnn_ivf_pq_search(ctypes.byref(args), _lib.stream_ptr(dev)))
         if flag is not None:
             self._raise_set_bits(int(flag.item()), len(sets))
-        return SearchResult(ids, dist)
+        return self._result(ids, dist)
 
     def rank(self, search_vecs, target, exclude=None, exclude_rows=None):
         """int64 [n]: for offline evaluation, the number of items ``search`` on the same queries would return before
