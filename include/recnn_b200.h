@@ -578,6 +578,87 @@ RECNN_API int64_t recnn_ivf_pq_search_workspace_bytes(int64_t n_queries, int32_t
                                                       int32_t refine);
 RECNN_API int recnn_ivf_pq_search(const recnn_ivf_pq_search_args* args, void* stream);
 
+/* ---- serving: a proximity-graph index (CAGRA-style, Milvus's GPU_CAGRA) ----------------------------------------
+ * Built on the device from k-NN lists of the table and searched one CTA per query against the resident table; the
+ * index holds only the graph and the entry points.
+ *
+ * recnn_graph_index: table fp32 [n_items, dim] row-major, 1 <= dim <= 512, the rows the graph was built over;
+ *   norms fp32 [n_items] (recnn_item_norms of the table; NULL for IP); metric L2, IP or COS; graph int32
+ *   [n_items, degree], degree in {16, 32, 64}, degree < n_items < 2^31: every row degree distinct ids of other items;
+ *   entry int32 [n_entry] distinct item ids, 1 <= n_entry <= min(512, n_items).  The search does not check the
+ *   contents of graph and entry. */
+typedef struct recnn_graph_index {
+  int64_t n_items;
+  int32_t dim, metric, degree, n_entry;
+  const float* table;
+  const float* norms;
+  int32_t* graph;
+  const int32_t* entry;
+} recnn_graph_index;
+RECNN_API int64_t recnn_sizeof_graph_index(void);
+
+/* recnn_graph_build: index->graph from knn int64 [n_items, knn_degree] (degree <= knn_degree <= 64 < n_items,
+ * n_items * degree < 2^31): row u
+ * is N(u) = [v_0 .. v_{D-1}], u's D best items by (key, id), without u.  Only index.n_items, index.degree and
+ * index.graph are read.
+ *   prune    c_j = #{i < j : v_j is in N(v_i) at a position p < j}; P(u) = the first d positions in (c_j, j) order
+ *   reverse  each kept edge u -> v at rank r of P(u) makes u a reverse candidate of v with rank r, ordered by (r, u)
+ *   merge    v's out-list is the first d/2 of P(v), then its reverse candidates, then the rest of P(v), each skipping
+ *            ids already present, until d are held: d distinct ids and no self-loop
+ * Integer work only (a stable radix sort for the reverse edges), so the same knn gives the same bits.
+ * *error_flag <- bits: 1 = a knn id outside [0, n_items); 2 = a row holding u itself or a repeated id (the graph is
+ * then not usable).  workspace_bytes >= recnn_graph_build_workspace_bytes (else RECNN_E_WORKSPACE, before any device
+ * work). */
+typedef struct recnn_graph_build_args {
+  recnn_graph_index index;    /* sizes in, graph out */
+  const int64_t* knn;         /* [n_items, knn_degree] */
+  int32_t knn_degree, reserved;
+  int32_t* error_flag;
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_graph_build_args;
+RECNN_API int64_t recnn_sizeof_graph_build_args(void);
+RECNN_API int64_t recnn_offsetof_graph_build_args(int field);
+RECNN_API int64_t recnn_graph_build_workspace_bytes(int64_t n_items, int32_t degree);
+RECNN_API int recnn_graph_build(const recnn_graph_build_args* args, void* stream);
+
+/* recnn_graph_search: a beam search per query over the graph.  A buffer of itopk = T (key, id, explored) entries
+ * (a multiple of 32 in [32, 256], T >= k), starting empty; iteration 0 takes the first min(W * degree, n_entry) entry
+ * points as candidates, each later iteration the out-lists of the W = search_width (1 <= W <= 8, W * degree <= 512)
+ * best unexplored entries, which become explored.  A candidate already in the buffer, or repeated in the iteration,
+ * is dropped; the others are keyed as recnn_retrieve_topk keys (L2 |x|^2 - 2 q.x, IP -q.x, COS -q.x / |x|), the dot
+ * product an fp32 fma sum over t = l, l + 32, ... per lane l in ascending t, then the warp's butterfly sum, so a
+ * key's bits depend only on the query, the item and dim; the buffer becomes the best T of buffer and candidates by
+ * (key, id).  The search stops when no entry is unexplored, or after max_iterations iterations past iteration 0
+ * (0: no cap).  The result is the k best entries of the final buffer that the row's set does not exclude (excluded
+ * items are still traversed); fewer than k end in id -1, distance FLT_MAX (L2) or -FLT_MAX (IP, COS); distances as
+ * recnn_retrieve_topk reports them.  A query's result does not depend on the other queries of the call.
+ * iterations_out int32 [n_queries] (optional): the iterations each query ran past iteration 0.  Exclusion: set_offsets
+ * NULL for none, else the set table of recnn_retrieve_topk_sets with its error bits in *error_flag.
+ * workspace_bytes >= recnn_graph_search_workspace_bytes (else RECNN_E_WORKSPACE, before any device work): the final
+ * buffers. */
+typedef struct recnn_graph_search_args {
+  recnn_graph_index index;    /* read only */
+  const float* queries;       /* [n_queries, dim] */
+  int64_t n_queries;
+  int32_t k, itopk, search_width, max_iterations;
+  const int64_t* set_ids;
+  int64_t n_set_ids;
+  const int64_t* set_offsets;
+  int64_t n_sets;
+  const int64_t* row_set;
+  int64_t* ids_out;           /* [n_queries, k] */
+  float* dist_out;            /* [n_queries, k] */
+  int32_t* iterations_out;
+  int32_t* error_flag;
+  void* workspace;
+  int64_t workspace_bytes;
+} recnn_graph_search_args;
+RECNN_API int64_t recnn_sizeof_graph_search_args(void);
+RECNN_API int64_t recnn_offsetof_graph_search_args(int field);
+RECNN_API int64_t recnn_graph_search_workspace_bytes(int64_t n_queries, int32_t itopk);
+RECNN_API int recnn_graph_search(const recnn_graph_search_args* args, void* stream);
+
 /* ---- offline evaluation: distances between the items of each served slate ---------------------------
  * The reference's diversity test: examples/streamlit_demo.py:355-445 ("Test Diversity") draws heatmaps of
  * recnn/utils/plot.py:9-35 pairwise_distances_fig, i.e. scipy cdist(..., "cosine") and cdist(..., "euclidean") over

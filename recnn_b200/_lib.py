@@ -181,6 +181,44 @@ def ivf_pq_index(n_items, dim, metric, nlist, m, centroids, centroid_norms, list
                       ptr(list_ids), ptr(codebooks), ptr(codes))
 
 
+class GraphIndex(C.Structure):
+    _fields_ = [
+        ("n_items", C.c_int64), ("dim", C.c_int32), ("metric", C.c_int32), ("degree", C.c_int32),
+        ("n_entry", C.c_int32), ("table", C.c_void_p), ("norms", C.c_void_p), ("graph", C.c_void_p),
+        ("entry", C.c_void_p),
+    ]
+
+
+class GraphBuildArgs(C.Structure):
+    _fields_ = [
+        ("index", GraphIndex), ("knn", C.c_void_p), ("knn_degree", C.c_int32), ("reserved", C.c_int32),
+        ("error_flag", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
+class GraphSearchArgs(C.Structure):
+    _fields_ = [
+        ("index", GraphIndex), ("queries", C.c_void_p), ("n_queries", C.c_int64), ("k", C.c_int32),
+        ("itopk", C.c_int32), ("search_width", C.c_int32), ("max_iterations", C.c_int32), ("set_ids", C.c_void_p),
+        ("n_set_ids", C.c_int64), ("set_offsets", C.c_void_p), ("n_sets", C.c_int64), ("row_set", C.c_void_p),
+        ("ids_out", C.c_void_p), ("dist_out", C.c_void_p), ("iterations_out", C.c_void_p), ("error_flag", C.c_void_p),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64),
+    ]
+
+
+# the fields recnn_offsetof_graph_*_args(i) reports, in order
+GRAPH_BUILD_PROBE_FIELDS = ["index", "knn", "knn_degree", "error_flag", "workspace", "workspace_bytes"]
+GRAPH_SEARCH_PROBE_FIELDS = ["index", "queries", "n_queries", "k", "itopk", "search_width", "max_iterations",
+                             "set_ids", "n_set_ids", "set_offsets", "n_sets", "row_set", "ids_out", "dist_out",
+                             "iterations_out", "error_flag", "workspace", "workspace_bytes"]
+
+
+def graph_index(n_items, dim, metric, degree, table, norms, graph, entry):
+    """a GraphIndex over device tensors (None -> NULL); n_entry is entry's length"""
+    return GraphIndex(n_items, dim, metric, degree, 0 if entry is None else int(entry.numel()), ptr(table),
+                      ptr(norms), ptr(graph), ptr(entry))
+
+
 _BETA_PROBE_FIELDS = ["dims", "n_rows", "net", "optim", "state", "action", "probs_out", "loss", "error",
                       "workspace_bytes", "n_rows_global"]
 
@@ -262,6 +300,15 @@ SIGNATURES = {
     "recnn_offsetof_ivf_pq_search_args": (C.c_int64, [C.c_int]),
     "recnn_ivf_pq_search_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "recnn_ivf_pq_search": (C.c_int, [C.POINTER(IvfPqSearchArgs), C.c_void_p]),
+    "recnn_sizeof_graph_index": (C.c_int64, []),
+    "recnn_sizeof_graph_build_args": (C.c_int64, []),
+    "recnn_offsetof_graph_build_args": (C.c_int64, [C.c_int]),
+    "recnn_graph_build_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
+    "recnn_graph_build": (C.c_int, [C.POINTER(GraphBuildArgs), C.c_void_p]),
+    "recnn_sizeof_graph_search_args": (C.c_int64, []),
+    "recnn_offsetof_graph_search_args": (C.c_int64, [C.c_int]),
+    "recnn_graph_search_workspace_bytes": (C.c_int64, [C.c_int64, C.c_int32]),
+    "recnn_graph_search": (C.c_int, [C.POINTER(GraphSearchArgs), C.c_void_p]),
     "recnn_slate_distances": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "recnn_slate_diversify": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,

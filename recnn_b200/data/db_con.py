@@ -24,6 +24,13 @@ stays exact, so recall can be measured against it or against a flat index.
 stored as M one-byte codes of its residual, scanned through lookup tables and
 optionally re-ranked exactly from the table (``search_param={"refine": r}``).
 
+``ItemIndex.build_graph()`` adds a proximity-graph index instead (CAGRA-style,
+Milvus's GPU_CAGRA): a pruned k-NN graph of the items, built on the device,
+after which ``search(..., search_param={"itopk_size": T, "search_width": W,
+"max_iterations": M})`` runs a beam search with one CTA per query
+(recnn_graph_build / recnn_graph_search).  An index holds at most one of the
+IVF and graph indexes.
+
 ``ItemIndex`` also takes the eight ``scipy.spatial.distance`` names the reference
 demo ranks by (examples/streamlit_demo.py:207-230, 319-345), so that its
 ``rank(action, distance.<name>, k)`` is ``ItemIndex(table, name).search(action, k)``:
@@ -110,6 +117,20 @@ def ivf_pq_sample(n_sample, seed=0):
     return torch.randperm(n_train, generator=g)[:PQ_CODEWORDS].to(torch.int64)
 
 
+GRAPH_DEGREES = (16, 32, 64)
+GRAPH_MAX_KNN = 64         # the k-NN lists come from a search, whose k is at most 64
+GRAPH_MAX_DIM = 512        # a lane of the search keeps at most 16 elements of a row in flight
+GRAPH_N_ENTRY = 512        # entry points stored with a graph
+GRAPH_KNN_SLAB = 16384     # table rows per k-NN search call
+
+
+def graph_entry_points(n_items, seed=0):
+    """int64 CPU tensor: the first min(512, n_items) ids of torch.randperm(n_items) drawn from
+    torch.Generator().manual_seed(seed), the entry points of a graph search (it starts from the first W * degree)"""
+    g = torch.Generator().manual_seed(int(seed))
+    return torch.randperm(n_items, generator=g)[:GRAPH_N_ENTRY].to(torch.int64)
+
+
 class IVFLists(NamedTuple):
     """The inverted lists of an ItemIndex: list l holds list_ids[list_offsets[l]:list_offsets[l + 1]], ascending, around
     centroids[l].  The tensors are the index's own device storage: read them, do not write them."""
@@ -157,6 +178,7 @@ class ItemIndex:
                                                        self.norms.data_ptr(), _lib.stream_ptr(self.device)))
         self._ws = None
         self._ivf = None
+        self._graph = None
 
     def _result(self, ids, dist):
         """SearchResult, the distances converted for "euclidean" and "cosine"; a -1 pad reports FLT_MAX under every
@@ -257,6 +279,7 @@ class ItemIndex:
         if m is not None:
             ivf["params"]["m"] = m
         self._ivf_finish(ivf)
+        self._graph = None
         return self
 
     def _ivf_buffers(self, nlist, m=None):
@@ -383,6 +406,7 @@ class ItemIndex:
                 del ws
         ivf["params"] = params
         self._ivf_finish(ivf)
+        self._graph = None
         return self
 
     def _nprobe(self, search_param):
@@ -424,9 +448,19 @@ class ItemIndex:
         "refine": r}``: r = 0 (default) returns the ADC top-k with ADC distances; r >= 1 re-scores the best r * topk
         ADC candidates exactly against ``table`` (r * topk <= 64) and returns their exact top-k with exact distances,
         computed as IVF_FLAT computes them: when r * topk covers every eligible item of the probed lists, the result is
-        IVF_FLAT's at the same nprobe, bit for bit."""
+        IVF_FLAT's at the same nprobe, bit for bit.
+
+        On a graph index (``build_graph`` / ``load_graph``) the search is a beam search over the graph, one CTA per
+        query: ``search_param={"itopk_size": T, "search_width": W, "max_iterations": M}`` (Milvus GPU_CAGRA's names;
+        defaults 64, 1, 0; T a multiple of 32 in [32, 256] and >= topk, 1 <= W <= 8 with W * graph_degree <= 512,
+        M >= 0, 0 meaning until converged; any other key raises ValueError).  A buffer of the T best items found so
+        far starts from the first W * graph_degree entry points; each iteration expands the out-lists of the W best
+        unexplored entries.  Keys are computed as the flat search computes them (its bits on small-integer tables), and
+        a query's result does not depend on the other queries of the call.  Excluded items are traversed but never
+        returned: the result is the topk best eligible items of the final buffer, padded as above."""
         from .item_sets import ItemSets, row_map
         nprobe = self._nprobe(search_param) if self._ivf is not None else None
+        gparam = self._graph_param(search_param) if self._graph is not None else None
         q = torch.as_tensor(search_vecs)
         if q.dim() == 1:
             q = q.unsqueeze(0)
@@ -436,6 +470,8 @@ class ItemIndex:
         if not 1 <= topk <= min(64, self.n_items):
             raise ValueError("topk must be in [1, min(64, n_items)]")
         refine = self._refine(search_param, topk) if nprobe is not None and "codes" in self._ivf else None
+        if gparam is not None and topk > gparam[0]:
+            raise ValueError("topk must be <= itopk_size (got topk %d, itopk_size %d)" % (topk, gparam[0]))
         n = int(q.shape[0])
         sets = rows = None
         if exclude is not None:
@@ -452,6 +488,8 @@ class ItemIndex:
         L = _lib.lib()
         if nprobe is not None:
             return self._ivf_search(q, n, topk, nprobe, sets, rows, refine)
+        if gparam is not None:
+            return self._graph_search(q, n, topk, gparam, sets, rows)
         need = L.recnn_retrieve_workspace_bytes(n, self.n_items, topk)
         if self._ws is None or self._ws.numel() < need:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
@@ -510,6 +548,217 @@ class ItemIndex:
         if flag is not None:
             self._raise_set_bits(int(flag.item()), len(sets))
         return self._result(ids, dist)
+
+    # ---------------------------------------------------------------------------------------------- graph index
+    @property
+    def graph(self):
+        """None, or int32 [n_items, graph_degree]: the out-neighbours of every item in the graph built by build_graph /
+        load_graph.  A view of the index's own device storage: read it, do not write it."""
+        return None if self._graph is None else self._graph["graph"]
+
+    @property
+    def graph_entry(self):
+        """None, or int32 [min(512, n_items)]: the entry points of the graph search"""
+        return None if self._graph is None else self._graph["entry"]
+
+    def _graph_check(self, d, D):
+        self._ivf_metric_check()
+        if d not in GRAPH_DEGREES:
+            raise ValueError("graph_degree must be one of %s (got %d)" % (GRAPH_DEGREES, d))
+        if not d <= D <= GRAPH_MAX_KNN:
+            raise ValueError("intermediate_degree must be in [graph_degree = %d, %d]: the k-NN lists come from a search "
+                             "whose k is at most %d (got %d)" % (d, GRAPH_MAX_KNN, GRAPH_MAX_KNN, D))
+        if self.n_items <= D:
+            raise ValueError("a graph index needs n_items > intermediate_degree (got %d items, degree %d)"
+                             % (self.n_items, D))
+        if self.dim > GRAPH_MAX_DIM:
+            raise ValueError("a graph index supports dim <= %d (got %d)" % (GRAPH_MAX_DIM, self.dim))
+
+    def knn_lists(self, degree, knn_nlist=None, knn_nprobe=None):
+        """int64 [n_items, degree] on the index's device: row u holds u's ``degree`` best items by (key, id) under the
+        index's metric, u itself excluded through an ItemSets of one id per row.  Exact (the flat search, in slabs of
+        16,384 rows) by default; with ``knn_nlist`` from an IVF_FLAT index of that many lists, built for the purpose
+        and freed after, probed at ``knn_nprobe`` (default min(16, knn_nlist)); a row whose probed lists hold fewer
+        than ``degree`` eligible items is searched again exactly."""
+        from .item_sets import ItemSets
+        n, dev = self.n_items, self.device
+        flat = ItemIndex(self.table, self.metric_name)
+        selves = ItemSets(torch.arange(n, device=dev), torch.arange(n + 1, device=dev))
+        approx, param = flat, None
+        if knn_nlist is not None:
+            approx = ItemIndex(self.table, self.metric_name).build_ivf(int(knn_nlist))
+            param = {"nprobe": int(knn_nprobe) if knn_nprobe is not None else min(16, int(knn_nlist))}
+        elif knn_nprobe is not None:
+            raise ValueError("knn_nprobe needs knn_nlist")
+        out = torch.empty(n, degree, dtype=torch.int64, device=dev)
+        for r0 in range(0, n, GRAPH_KNN_SLAB):
+            rows = torch.arange(r0, min(n, r0 + GRAPH_KNN_SLAB), device=dev)
+            out[r0:r0 + len(rows)] = approx.search(self.table[rows], degree, search_param=param, exclude=selves,
+                                                   exclude_rows=rows).ids
+        del approx
+        if knn_nlist is not None:
+            short = (out < 0).any(1).nonzero().flatten()
+            for s0 in range(0, len(short), GRAPH_KNN_SLAB):
+                rows = short[s0:s0 + GRAPH_KNN_SLAB]
+                out[rows] = flat.search(self.table[rows], degree, exclude=selves, exclude_rows=rows).ids
+        return out
+
+    def build_graph(self, graph_degree=32, intermediate_degree=64, knn_nlist=None, knn_nprobe=None, seed=0):
+        """Build a proximity-graph index over the table on the device (CAGRA's construction) and return self; it
+        replaces an IVF index.  Metric L2, IP or COS (or euclidean / cosine), graph_degree d in {16, 32, 64},
+        d <= intermediate_degree D <= 64 < n_items, dim <= 512.
+
+        1. k-NN lists: N(u) = u's D best items (``knn_lists``: exact, or through a temporary IVF_FLAT index with
+           ``knn_nlist`` / ``knn_nprobe``).
+        2. Pruning: c_j = the number of i < j such that v_j is in N(v_i) at a position p < j; P(u) keeps the d
+           positions first in (c_j, j) order.
+        3. Reverse edges: each kept edge u -> v at rank r makes u a reverse candidate of v, ordered by (r, u).
+        4. Merge: v's out-list is the first d/2 of P(v), then its reverse candidates, then the rest of P(v), skipping
+           repeats, until it holds d ids: every item gets d distinct out-neighbours and no self-loop.
+        5. Entry points: ``graph_entry_points(n_items, seed)``.
+
+        Steps 2-4 run on the device (recnn_graph_build) on integer data only, so the graph is a function of the k-NN
+        ids, bit for bit.  The index holds n_items * d int32 ids (128 MB at 1M items, d = 32) and reads the table
+        itself: it is a snapshot of the table at build time."""
+        d, D = int(graph_degree), int(intermediate_degree)
+        self._graph_check(d, D)
+        knn = self.knn_lists(D, knn_nlist, knn_nprobe)
+        gr = self._graph_buffers(d, graph_entry_points(self.n_items, seed))
+        L, dev = _lib.lib(), self.device
+        flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            ws = torch.empty(L.recnn_graph_build_workspace_bytes(self.n_items, d), dtype=torch.uint8, device=dev)
+            args = _lib.GraphBuildArgs(self._graph_descriptor(gr), knn.data_ptr(), D, 0, flag.data_ptr(),
+                                       ws.data_ptr(), ws.numel())
+            _lib.check(L.recnn_graph_build(ctypes.byref(args), _lib.stream_ptr(dev)))
+        del ws, knn
+        if int(flag.item()) != 0:
+            raise _lib.RecnnError("the k-NN lists of the graph build were malformed (error bits %d)" % int(flag.item()))
+        gr["params"] = dict(graph_degree=d, intermediate_degree=D, knn_nlist=knn_nlist, knn_nprobe=knn_nprobe,
+                            seed=int(seed))
+        self._graph, self._ivf = gr, None
+        return self
+
+    def _graph_buffers(self, d, entry):
+        dev = self.device
+        return dict(graph=torch.empty(self.n_items, d, dtype=torch.int32, device=dev),
+                    entry=entry.to(device=dev, dtype=torch.int32).contiguous(), degree=d)
+
+    def _graph_descriptor(self, gr):
+        """the recnn_graph_index of the buffers in gr"""
+        return _lib.graph_index(self.n_items, self.dim, self.metric, gr["degree"], self.table, self.norms,
+                                gr["graph"], gr["entry"])
+
+    def graph_state(self):
+        """The graph index as host tensors and plain values, for torch.save: graph int32 [n_items, d], entry int32,
+        the build parameters, the metric and the table's shape.  None without a graph."""
+        if self._graph is None:
+            return None
+        return dict(graph=self._graph["graph"].cpu(), entry=self._graph["entry"].cpu(),
+                    params=dict(self._graph["params"]), metric=self.metric_name, n_items=self.n_items, dim=self.dim)
+
+    def load_graph(self, state):
+        """Restore a graph saved by graph_state over this index's table (the one it was built on) and return self; it
+        replaces an IVF index.  The metric and shapes must match, every id must be in [0, n_items), and no graph row
+        may hold its own item or a repeated id (checked on the device): ValueError otherwise."""
+        try:
+            graph, entry = state["graph"], state["entry"]
+            metric, n_items, dim = state["metric"], int(state["n_items"]), int(state["dim"])
+            params = dict(state["params"])
+        except (KeyError, TypeError) as e:
+            raise ValueError("not a graph_state() dict: %s" % e)
+        self._ivf_metric_check()
+        if metric != self.metric_name:
+            raise ValueError("the graph was built for metric %s, this ItemIndex is %s" % (metric, self.metric_name))
+        if (n_items, dim) != (self.n_items, self.dim):
+            raise ValueError("the graph was built over a [%d, %d] table, this one is [%d, %d]"
+                             % (n_items, dim, self.n_items, self.dim))
+        if self.dim > GRAPH_MAX_DIM:
+            raise ValueError("a graph index supports dim <= %d (got %d)" % (GRAPH_MAX_DIM, self.dim))
+        if not (torch.is_tensor(graph) and torch.is_tensor(entry)):
+            raise ValueError("graph and entry must be tensors")
+        n_entry = min(GRAPH_N_ENTRY, n_items)
+        if (graph.dim() != 2 or graph.shape[0] != n_items or int(graph.shape[1]) not in GRAPH_DEGREES
+                or int(graph.shape[1]) >= n_items or graph.dtype != torch.int32
+                or tuple(entry.shape) != (n_entry,) or entry.dtype != torch.int32):
+            raise ValueError("malformed graph state: graph int32 [%d, d] with d in %s, entry int32 [%d]"
+                             % (n_items, GRAPH_DEGREES, n_entry))
+        dev = self.device
+        g, e = graph.to(dev).contiguous(), entry.to(dev).contiguous()
+        ok = bool(((g >= 0) & (g < n_items)).all()) and bool(((e >= 0) & (e < n_items)).all())
+        if ok:
+            srt = torch.sort(g, dim=1).values
+            self_loop = (g == torch.arange(n_items, device=dev, dtype=torch.int32)[:, None]).any()
+            ok = not bool(self_loop) and not bool((srt[:, 1:] == srt[:, :-1]).any())
+        if ok:
+            se = torch.sort(e).values
+            ok = not bool((se[1:] == se[:-1]).any())
+        if not ok:
+            raise ValueError("malformed graph state: every id must be in [0, %d), no graph row may hold its own item "
+                             "or a repeated id, and the entry points must be distinct" % n_items)
+        gr = self._graph_buffers(int(graph.shape[1]), e)
+        gr["graph"].copy_(g)
+        gr["params"] = params
+        self._graph, self._ivf = gr, None
+        return self
+
+    def _graph_param(self, search_param):
+        p = dict(search_param or {})
+        unknown = sorted(set(p) - {"itopk_size", "search_width", "max_iterations"})
+        if unknown:
+            raise ValueError("unknown search_param keys %s (a graph index takes only itopk_size, search_width and "
+                             "max_iterations)" % unknown)
+        T, W, M = int(p.get("itopk_size", 64)), int(p.get("search_width", 1)), int(p.get("max_iterations", 0))
+        d = self._graph["degree"]
+        if not (32 <= T <= 256 and T % 32 == 0):
+            raise ValueError("itopk_size must be a multiple of 32 in [32, 256] (got %d)" % T)
+        if not (1 <= W <= 8 and W * d <= 512):
+            raise ValueError("search_width must be in [1, 8] with search_width * graph_degree <= 512 (got %d, degree "
+                             "%d)" % (W, d))
+        if M < 0:
+            raise ValueError("max_iterations must be >= 0 (got %d)" % M)
+        return T, W, M
+
+    def _graph_search(self, q, n, topk, gparam, sets, rows, iterations=None):
+        L, gr, dev = _lib.lib(), self._graph, self.device
+        T, W, M = gparam
+        ids = torch.empty(n, topk, dtype=torch.int64, device=dev)
+        dist = torch.empty(n, topk, dtype=torch.float32, device=dev)
+        need = L.recnn_graph_search_workspace_bytes(n, T)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        set_args, flag = (None, 0, None, 0, None), None
+        if sets is not None:
+            sets = sets.to(dev)
+            rows = None if rows is None else rows.to(dev).contiguous()
+            flag = torch.empty(1, dtype=torch.int32, device=dev)
+            set_args = (sets.ids.data_ptr() if sets.ids.numel() else None, sets.ids.numel(), sets.offsets.data_ptr(),
+                        len(sets), _lib.ptr(rows))
+        with torch.cuda.device(dev):
+            args = _lib.GraphSearchArgs(self._graph_descriptor(gr), q.data_ptr(), n, topk, T, W, M, *set_args,
+                                        ids.data_ptr(), dist.data_ptr(), _lib.ptr(iterations), _lib.ptr(flag),
+                                        self._ws.data_ptr(), self._ws.numel())
+            _lib.check(L.recnn_graph_search(ctypes.byref(args), _lib.stream_ptr(dev)))
+        if flag is not None:
+            self._raise_set_bits(int(flag.item()), len(sets))
+        return self._result(ids, dist)
+
+    def graph_iterations(self, search_vecs, search_param=None):
+        """int32 [n]: the iterations past the entry step that ``search`` runs for each query at these parameters (the
+        same for every topk), e.g. to see how long a search takes to converge"""
+        if self._graph is None:
+            raise ValueError("graph_iterations needs a graph index (build_graph / load_graph)")
+        T, W, M = self._graph_param(search_param)
+        q = torch.as_tensor(search_vecs)
+        if q.dim() == 1:
+            q = q.unsqueeze(0)
+        if q.dim() != 2 or q.shape[1] != self.dim:
+            raise ValueError("search_vecs must be [n, %d]" % self.dim)
+        q = q.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        it = torch.zeros(q.shape[0], dtype=torch.int32, device=self.device)
+        if q.shape[0]:
+            self._graph_search(q, int(q.shape[0]), 1, (T, W, M), None, None, iterations=it)
+        return it
 
     def rank(self, search_vecs, target, exclude=None, exclude_rows=None):
         """int64 [n]: for offline evaluation, the number of items ``search`` on the same queries would return before
@@ -576,8 +825,10 @@ class MilvusConnection(ItemIndex):
     "IVF_FLAT" with ``param["nlist"]`` builds the IVF index at construction (Milvus create_index(IVF_FLAT, {"nlist"})),
     so that ``search(..., search_param={"nprobe": p})`` means what it means to Milvus; "IVF_PQ" with ``param["nlist"]``,
     ``param["m"]`` and optionally ``param["nbits"]`` (8, the only width) builds the IVF_PQ index (Milvus
-    create_index(IVF_PQ, {"nlist", "m", "nbits"})); without it, or with "FLAT", the search is exact.  No Milvus server
-    is involved."""
+    create_index(IVF_PQ, {"nlist", "m", "nbits"})); "GPU_CAGRA" with optional ``param["intermediate_graph_degree"]``
+    (default 64) and ``param["graph_degree"]`` (default 32, both at most 64) builds the graph index (build_graph), searched
+    with search_param {"itopk_size", "search_width", "max_iterations"}; without it, or with "FLAT", the search is exact.
+    No Milvus server is involved."""
 
     def __init__(self, env, name="movies_L2", port="19530", param=None):
         metric = "L2"
@@ -585,18 +836,26 @@ class MilvusConnection(ItemIndex):
             mt = str(param["metric_type"]).upper()
             metric = "IP" if mt.endswith("IP") else "L2"
         index_type = str(param.get("index_type", "FLAT")).upper() if param else "FLAT"
-        if index_type not in ("FLAT", "IVF_FLAT", "IVF_PQ"):
-            raise ValueError("index_type must be FLAT, IVF_FLAT or IVF_PQ (got %s)" % index_type)
-        if index_type != "FLAT" and "nlist" not in param:
+        if index_type not in ("FLAT", "IVF_FLAT", "IVF_PQ", "GPU_CAGRA"):
+            raise ValueError("index_type must be FLAT, IVF_FLAT, IVF_PQ or GPU_CAGRA (got %s)" % index_type)
+        if index_type in ("IVF_FLAT", "IVF_PQ") and "nlist" not in param:
             raise ValueError("index_type %s needs param['nlist']" % index_type)
         if index_type == "IVF_PQ":
             if "m" not in param:
                 raise ValueError("index_type IVF_PQ needs param['m']")
             if int(param.get("nbits", 8)) != 8:
                 raise ValueError("IVF_PQ supports nbits = 8 only (got %s)" % param["nbits"])
+        if index_type == "GPU_CAGRA":
+            D, d = int(param.get("intermediate_graph_degree", 64)), int(param.get("graph_degree", 32))
+            if D > GRAPH_MAX_KNN or d > GRAPH_MAX_KNN:
+                raise ValueError("GPU_CAGRA supports intermediate_graph_degree and graph_degree up to %d (got %d, %d): "
+                                 "the k-NN lists are built by the search, whose k is at most %d"
+                                 % (GRAPH_MAX_KNN, D, d, GRAPH_MAX_KNN))
         emb = env.base.embeddings if hasattr(env, "base") else env
         super().__init__(emb, metric)
-        if index_type == "IVF_FLAT":
+        if index_type == "GPU_CAGRA":
+            self.build_graph(graph_degree=d, intermediate_degree=D)
+        elif index_type == "IVF_FLAT":
             self.build_ivf(int(param["nlist"]))
         elif index_type == "IVF_PQ":
             self.build_ivf(int(param["nlist"]), m=int(param["m"]))
