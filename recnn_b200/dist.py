@@ -7,15 +7,14 @@ step, actor on policy steps) plus the loss scalars -- with an all-reduce before
 the (identical) optimizer step.  Local loss terms are already scaled by
 1/N_global on the device, so SUM over ranks gives the single-device gradient.
 
-One process per GPU (torchrun).  torch.distributed supplies rendezvous, the weight broadcast and a
-NCCL fallback; the per-step gradient exchange itself runs inside the step's CUDA graph as kernels that
-read the peers' staging buffers over NVLink (``PeerComm`` -> ``recnn_comm_*`` in include/recnn_b200.h).
+One process per GPU (torchrun).  torch.distributed supplies rendezvous and the weight broadcast; the
+per-step gradient exchange itself runs inside the step's CUDA graph as kernels that read the peers'
+staging buffers over NVLink (``PeerComm`` -> ``recnn_comm_*`` in include/recnn_b200.h), so the GPUs of
+the node need peer access to each other.
 """
 from __future__ import annotations
 
 import ctypes
-import os
-import warnings
 
 import torch
 import torch.distributed as dist
@@ -41,7 +40,7 @@ class PeerComm:
             everyone = [None] * self.world
             dist.all_gather_object(everyone, bytes(mine.raw), group=group)
             status = L.recnn_comm_connect(self.handle, b"".join(everyone))
-            # all ranks must agree, otherwise some would wait in a kernel for peers that use NCCL
+            # all ranks must agree: a rank that went on would wait in a kernel for peers that raise here
             ok = [None] * self.world
             dist.all_gather_object(ok, int(status), group=group)
             if any(ok):
@@ -90,7 +89,8 @@ def broadcast_nets(nets: dict, group=None, src: int = 0):
 
 def enable_data_parallel(agent_or_nets, group=None, sync_weights=True, beta=None):
     """Turn on gradient all-reduce for an Algo (or a nets dict).  Must be called on every
-    rank after the nets are on their CUDA device.
+    rank after the nets are on their CUDA device.  The all-reduce runs over a peer communicator
+    (PeerComm), so the GPUs need peer access to each other; without it every rank raises RecnnError.
 
     With a DiscreteActor policy (REINFORCE) the agent trains row-parallel instead (RowParallel below): the nets -- and
     ``beta``, the Top-K behaviour policy -- are made identical to rank 0's, one peer communicator is built and
@@ -112,14 +112,11 @@ def enable_data_parallel(agent_or_nets, group=None, sync_weights=True, beta=None
     policy = nets["policy_net"]
     comm = None
     arena = param_arena(policy)
-    if world > 1 and arena.is_cuda and os.environ.get("RECNN_B200_COMM", "peer") != "nccl":
-        try:
-            comm = PeerComm(group, arena.device, max(param_arena(m).numel() for m in nets.values()))
-        except _lib.RecnnError as exc:     # e.g. no peer access between the GPUs: NCCL between the phases instead
-            warnings.warn("recnn_b200: %s; falling back to NCCL all-reduces between the step's phases" % exc)
+    if world > 1 and arena.is_cuda:
+        comm = PeerComm(group, arena.device, max(param_arena(m).numel() for m in nets.values()))
     policy.__dict__["_recnn_dp"] = (group, world, comm)
     for eng in policy.__dict__.get("_recnn_engines", {}).values():
-        eng.group, eng.world, eng.comm = group, world, comm
+        eng.world, eng.comm = world, comm
         eng.graphs.clear()
         eng._fast.clear()
     return agent_or_nets

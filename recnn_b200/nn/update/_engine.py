@@ -4,8 +4,9 @@ Responsibilities (all plumbing; the arithmetic is in recnn_b200/csrc):
   * validate / (re)build the flat parameter, gradient and optimizer arenas;
   * stage the batch into fixed device buffers (one async copy per tensor) so the
     step is replayable as a CUDA graph;
-  * pick the phase split: one call (built-in optimizers, one GPU), or three
-    calls with gradient all-reduces / external ``optimizer.step()`` in between;
+  * pick the phase split: one call (built-in optimizers; with several GPUs the
+    peer communicator's all-reduces are kernels of that call), or phase by phase
+    with the communicator's all-reduces / external ``optimizer.step()`` in between;
   * read the 3-4 loss scalars back (the only synchronisation of a step -- the
     reference API returns Python floats, recnn/nn/update/ddpg.py:102).
 """
@@ -60,11 +61,9 @@ class StepEngine:
         self.n_rows = -1
         self.form = None
         self.graphs = {}
-        self.seg_graphs = {}
         self._fast = {}
         self.graph_sig = None
         self.eager_runs = {}
-        self.group = None            # torch.distributed process group for data parallel
         self.world = 1
         self.comm = None             # recnn_b200.dist.PeerComm: in-kernel all-reduce over NVLink peer memory
         self.plan = None             # recnn_b200.dist.RowParallel of a data-parallel REINFORCE critic (value_only)
@@ -82,12 +81,11 @@ class StepEngine:
 
     # ------------------------------------------------------------------ staging
     def _invalidate(self):
-        """Drop everything that baked device addresses in: captured graphs (whole-step and per-segment),
-        the fast-path table of (tokens -> graph / cached StepArgs) and the first-sight bookkeeping.  Called
+        """Drop everything that baked device addresses in: captured graphs, the fast-path table of
+        (tokens -> graph) and the first-sight bookkeeping.  Called
         whenever a staging buffer or the workspace is (re)allocated, the batch shape changes, or data
         parallelism is (re)configured -- a stale graph would run against freed memory."""
         self.graphs.clear()
-        self.seg_graphs.clear()
         self._fast.clear()
         self.eager_runs.clear()
 
@@ -283,36 +281,14 @@ class StepEngine:
         self.last_call_kernels = L.recnn_b200_launch_count() - before
         self.kernels += self.last_call_kernels
 
-    def _body(self, a, nets, do_policy):
-        """The whole step with built-in optimizers: one C call on one GPU.  (The multi-GPU branch below
-        is kept for direct launches only: capturing the NCCL all-reduces into the step graph deadlocked
-        on the 2-GPU box, so data parallel runs go through the split-phase path in _step.)"""
-        P = _lib
-        if self.world == 1 or a.comm:      # with a peer communicator the gradient all-reduces are kernels of the step
-            self._launch(a, P.PH_ALL)
-            return self.last_call_kernels
-        td3 = self.algo == P.ALGO_TD3
-        kernels = 0
-        self._launch(a, P.PH_GATHER | P.PH_VALUE_GRAD)
-        kernels += self.last_call_kernels
-        for i in range(2 if td3 else 1):
-            self._allreduce(grad_arena(nets["value_net" + (str(i + 1) if td3 else "")]))
-        self._launch(a, P.PH_VALUE_OPT | P.PH_POLICY_LOSS | P.PH_POLICY_GRAD)
-        kernels += self.last_call_kernels
-        if do_policy:
-            self._allreduce(grad_arena(nets["policy_net"]))
-        self._allreduce(self.losses[:3])
-        self._launch(a, P.PH_POLICY_OPT | P.PH_SOFT_UPDATE | P.PH_FINISH)
-        kernels += self.last_call_kernels
-        return kernels
-
-    def _run_fused(self, a, nets, do_policy):
-        """Direct launches the first time a variant is seen, then one CUDA graph (kernels, side-stream
-        forks/joins, the loss read-back and -- with several GPUs -- the NCCL all-reduces) per variant."""
+    def _run_fused(self, a):
+        """The whole step with built-in optimizers, one C call (with a communicator its all-reduces are kernels of
+        the step): direct launches the first time a variant is seen, then one CUDA graph (kernels, side-stream
+        forks/joins and the loss read-back) per variant."""
         a.phases = _lib.PH_ALL
         key = self._signature(a)
         if not _USE_GRAPHS:
-            self._body(a, nets, do_policy)
+            self._launch(a, _lib.PH_ALL)
             return None
         g = self.graphs.get(key)
         if g is not None:
@@ -324,7 +300,7 @@ class StepEngine:
             self.eager_runs.clear()       # a new variant; do not let the bookkeeping grow with the run
         self.eager_runs[key] = runs + 1
         if runs < 1:                      # first time: plain launch (also warms lazy module loading)
-            self._body(a, nets, do_policy)
+            self._launch(a, _lib.PH_ALL)
             return None
         if len(self.graphs) > 16:
             self._invalidate()
@@ -332,7 +308,8 @@ class StepEngine:
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                n_kernels = self._body(a, nets, do_policy)
+                self._launch(a, _lib.PH_ALL)
+            n_kernels = self.last_call_kernels
             self.graphs[key] = (g, n_kernels)
             g.replay()
             self.kernels += n_kernels
@@ -340,51 +317,8 @@ class StepEngine:
         except Exception as exc:      # capture unsupported in this context: stay on direct launches
             warnings.warn("recnn_b200: CUDA graph capture failed (%s); using direct launches" % exc)
             globals()["_USE_GRAPHS"] = False
-            self._body(a, nets, do_policy)
+            self._launch(a, _lib.PH_ALL)
             return None
-
-    def _run_segments(self, a, nets, do_policy, vkey):
-        """Data parallel: the step is cut where gradients are complete.  Each cut piece is its own CUDA
-        graph (kernels only); the NCCL all-reduces run between the replays on the same stream."""
-        P = _lib
-        td3 = self.algo == P.ALGO_TD3
-        segs = (P.PH_GATHER | P.PH_VALUE_GRAD, P.PH_VALUE_OPT | P.PH_POLICY_LOSS | P.PH_POLICY_GRAD,
-                P.PH_POLICY_OPT | P.PH_SOFT_UPDATE | P.PH_FINISH)
-        a.phases = 0
-        key = self._signature(a)
-        ent = self.seg_graphs.get(key)
-        runs = self.eager_runs.get(key, 0)
-        self.eager_runs[key] = runs + 1
-        if ent is None and _USE_GRAPHS and runs >= 1:
-            try:
-                torch.cuda.synchronize(self.device)
-                ent = []
-                for ph in segs:
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        self._launch(a, ph)
-                    ent.append((g, self.last_call_kernels))
-                self.seg_graphs[key] = ent
-            except Exception as exc:
-                warnings.warn("recnn_b200: CUDA graph capture failed (%s); using direct launches" % exc)
-                globals()["_USE_GRAPHS"] = False
-                ent = None
-
-        def run(i):
-            if ent is not None:
-                ent[i][0].replay()
-                self.kernels += ent[i][1]
-            else:
-                self._launch(a, segs[i])
-
-        run(0)
-        for i in range(2 if td3 else 1):
-            self._allreduce(grad_arena(nets["value_net" + (str(i + 1) if td3 else "")]))
-        run(1)
-        if do_policy:
-            self._allreduce(grad_arena(nets["policy_net"]))
-        self._allreduce(self.losses[:3])
-        run(2)
 
     def _read_losses(self):
         """After the stream synchronisation of a step: the loss scalars, or the step's error."""
@@ -403,14 +337,12 @@ class StepEngine:
             return self._step(batch, params, nets, optimizer, learn, step, debug, policy_every_key)
 
     def _allreduce(self, t):
-        if self.plan is not None:
-            self.plan.all_reduce(t)
-            return
-        import torch.distributed as dist
-        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        """The engine's one exchange: through the RowParallel plan of a data-parallel REINFORCE critic, else through
+        the step's communicator."""
+        (self.plan if self.plan is not None else self.comm).all_reduce(t)
 
     def _tokens(self, nets, optimizer, params, st):
-        """Cheap fingerprint of everything a cached StepArgs / CUDA graph depends on: storage addresses of the nets
+        """Cheap fingerprint of everything a captured CUDA graph depends on: storage addresses of the nets
         (first and last parameter, gradient), optimizer hyper-parameters and state arenas, the algorithm's scalars
         and the staged batch buffers.  This runs on every step between the batch copies and the graph launch, i.e.
         while the GPU idles, so it avoids nn.Module attribute lookups (the Parameter objects are cached per net) and
@@ -458,11 +390,8 @@ class StepEngine:
             ent = self._fast.get(vkey)
             tok = self._tokens(nets, optimizer, params, st)
             if ent is not None and ent[0] == tok:
-                if self.world == 1 or self.comm is not None:
-                    ent[1].replay()
-                    self.kernels += ent[2]
-                else:
-                    self._run_segments(ent[1], nets, do_policy, None)      # cached StepArgs
+                ent[1].replay()
+                self.kernels += ent[2]
                 torch.cuda.current_stream(self.device).synchronize()
                 return self._read_losses()
         a, pol_opt, val_opts = self._build_args(st, nets, optimizer, params, learn, do_policy)
@@ -474,16 +403,11 @@ class StepEngine:
             want_debug = {"next_action": torch.empty(n, A, device=self.device),
                           "gen_action": torch.empty(n, A, device=self.device)}
         fused = builtin and learn and want_debug is None
-        if fused and self.comm is not None:
-            a.comm = self.comm.ptr
-        if fused and self.world > 1 and self.comm is None:
-            self._run_segments(a, nets, do_policy, None)
-            if _USE_GRAPHS:
-                self._fast[(do_policy, st["form"], st["n"])] = (self._tokens(nets, optimizer, params, st), a, 0)
-            torch.cuda.current_stream(self.device).synchronize()
-            return self._read_losses()
+        exchange = self.comm is not None
         if fused:
-            g = self._run_fused(a, nets, do_policy)
+            if exchange:
+                a.comm = self.comm.ptr
+            g = self._run_fused(a)
             if g is not None:
                 # arenas may have been (re)built by _build_args: fingerprint after the fact
                 self._fast[(do_policy, st["form"], st["n"])] = (self._tokens(nets, optimizer, params, st), g[0], g[1])
@@ -494,7 +418,7 @@ class StepEngine:
             value_nets = [nets["value_net" + (str(i + 1) if td3 else "")] for i in range(2 if td3 else 1)]
             self._launch(a, P.PH_GATHER | P.PH_VALUE_GRAD, want_debug)
             if learn:
-                if self.world > 1:
+                if exchange:
                     for vn in value_nets:
                         self._allreduce(grad_arena(vn))
                 # Each optimizer is stepped exactly once, by whoever owns it: the C side runs the fused
@@ -508,7 +432,7 @@ class StepEngine:
             self._launch(a, P.PH_POLICY_LOSS, want_debug)
             if do_policy:
                 self._launch(a, P.PH_POLICY_GRAD, want_debug)
-                if self.world > 1:
+                if exchange:
                     self._allreduce(grad_arena(nets["policy_net"]))
                 # clip coefficient (+ the fused optimizer when the policy optimizer is built in; for an
                 # external one the C side only scales the gradient in place)
@@ -517,7 +441,7 @@ class StepEngine:
                     grad_arena(nets["policy_net"])
                     pol_opt.step()
                 self._launch(a, P.PH_SOFT_UPDATE, want_debug)
-            if self.world > 1:
+            if exchange:
                 self._allreduce(self.losses[:3])
             self._launch(a, P.PH_FINISH, want_debug)     # ++rng_step, losses -> pinned host
         torch.cuda.current_stream(self.device).synchronize()
@@ -574,7 +498,10 @@ def get_engine(algo, nets, device) -> StepEngine:
         eng = StepEngine(algo, nets, dev)
         dp = policy.__dict__.get("_recnn_dp")
         if dp is not None:
-            eng.group, eng.world, eng.comm = dp
+            _, eng.world, eng.comm = dp
+            if eng.world > 1 and eng.comm is None:
+                raise _lib.RecnnError("enable_data_parallel was called while the nets were not on their CUDA device, "
+                                      "so no peer communicator exists: call it again on every rank")
         rows = policy.__dict__.get("_recnn_rows")
         if rows is not None:
             eng.plan, eng.world = rows, rows.world

@@ -12,7 +12,9 @@ wherever the communicator path and the single-GPU path compute the same thing th
     .grad, optimizer state, step counters and value losses are bit-identical at every step;
   * DDPG and TD3 agree bit for bit on step 0 (a policy step) up to the actor's clip coefficient, whose L1 norm is
     summed in a different order; from step 1 DDPG's critic sees that actor through the soft-updated target policy,
-    so both runs are held to the float64 oracle instead.
+    so both runs are held to the float64 oracle instead;
+  * with external torch optimizers the step runs phase by phase and calls the collective between the phases: every
+    exchange is made, and the two runs are bit-identical throughout.
 
 What world 1 does not reach -- slicing across owners, rank-order sums of W > 1 contributions, the double buffering
 when one rank is an epoch ahead, the n_rows_global mismatch flag -- is left to the multi-GPU parametrisations of
@@ -48,10 +50,12 @@ SIMT_ROW = "h320"
 # ----------------------------------------------------------------------------- the communicator
 class World1Comm:
     """A one-rank peer communicator made through the C ABI (no torch.distributed): create, take the local handle,
-    connect with it (a single local handle maps nothing)."""
+    connect with it (a single local handle maps nothing).  ``reduced``: the sizes of the all_reduce calls made through
+    it from Python, in order (the step's own all-reduce kernels are not calls of this object)."""
 
     def __init__(self, capacity_floats):
         L = _lib.lib()
+        self.reduced = []
         self.handle = ctypes.c_void_p()
         _lib.check(L.recnn_comm_create(0, 1, int(capacity_floats), ctypes.byref(self.handle)))
         self.capacity = -(-int(capacity_floats) // 4) * 4       # the library rounds the staging capacity up to 4
@@ -71,6 +75,7 @@ class World1Comm:
         assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
         _lib.check(_lib.lib().recnn_comm_allreduce(self.handle, t.data_ptr(), t.numel(),
                                                    torch.cuda.current_stream(t.device).cuda_stream))
+        self.reduced.append(t.numel())
         return t
 
     def close(self):
@@ -346,24 +351,61 @@ def run_pair(case, algo, opt, open_comm, **kw):
     return a, b, ulp, l1_rel
 
 
+def run_split_pair(case, algo, opt, open_comm, **kw):
+    """The same case plain and through a world-1 communicator, with external torch optimizers (``opt``: "sgd" or
+    "adam").  The step then runs phase by phase, and with a communicator attached it all-reduces between the phases
+    what the one-call step all-reduces inside it: each critic's gradient every step, the actor's gradient on policy
+    steps, then the three loss words.  At world 1 those all-reduces are the identity and the phases launch the same
+    kernels as the plain run's, so the two runs agree bit for bit."""
+    reduced = []
+
+    def count(step, nets, opts, loss):
+        comm = engine_of(nets).comm
+        reduced.append(list(comm.reduced))
+        comm.reduced.clear()
+
+    a = run_cuda_case(case, algo, opt, form="frames", external=True, **kw)
+    b = run_cuda_case(case, algo, opt, form="frames", external=True, comm=open_comm, on_step=count, **kw)
+    assert engine_of(a["_nets"]).comm is None and engine_of(b["_nets"]).comm is not None
+    nets = b["_nets"]
+    critics = [param_arena(nets[name]).numel() for name in critic_names(algo)]
+    actor = param_arena(nets["policy_net"]).numel()
+    assert len(reduced) == C.CASES[case]["steps"]
+    for s, got in enumerate(reduced):
+        assert got == critics + ([actor] if s % POLICY_EVERY == 0 else []) + [3], (s, got)
+    assert engine_of(a["_nets"]).kernels == engine_of(b["_nets"]).kernels
+    for k in a:
+        if k.startswith(("final.", "loss.", "after", "grad_")):
+            assert np.array_equal(np.atleast_1d(a[k]).view(np.uint8), np.atleast_1d(b[k]).view(np.uint8)), k
+    return a, b
+
+
 def _pads(res):
     return {"pads": pad_report(res["_nets"], res["_opts"])}
 
 
-@pytest.mark.parametrize("opt", ["sgd", "sgd_momentum", "adam", "ranger"])
+@pytest.mark.parametrize("opt", ["sgd", "sgd_momentum", "adam", "ranger", "torch_sgd", "torch_adam"])
 @pytest.mark.parametrize("algo", ["ddpg", "td3"])
 @pytest.mark.parametrize("case", ["tiny", "canon"])
 def test_step_through_world1_comm(case, algo, opt, open_comm):
     """tiny / canon, 12 steps (policy steps 0 and 10; Ranger's rectification switch and Lookahead at step 6 and
     Lookahead again at 12): bit-identical to the single-GPU step where it must be, and the communicator run against
-    the golden fixtures (SGD, Adam: weights, losses and gradients) or the live oracle (SGD with momentum, Ranger)."""
-    gold = load_golden("%s_%s_%s.npz" % (algo, case, opt)) if opt in ("sgd", "adam") else None
+    the golden fixtures (SGD, Adam: weights, losses and gradients) or the live oracle (SGD with momentum, Ranger).
+    torch_sgd / torch_adam: the same SGD / Adam as torch optimizers, through the phase-by-phase step
+    (run_split_pair)."""
+    external = opt.startswith("torch_")
+    kind = opt[len("torch_"):] if external else opt
+    gold = load_golden("%s_%s_%s.npz" % (algo, case, kind)) if kind in ("sgd", "adam") else None
     inp, dropped = None, 0
     if opt == "sgd_momentum":
         # the seeds are screened for clean ReLU gates along the SGD / Adam / Ranger trajectories only: drop the
         # ambiguous ones of this trajectory from the replayed masks
         inp, dropped, _ = neutralise_ambiguous_gates(C.CASES[case], algo, opt)
-    _, b, ulp, l1_rel = run_pair(case, algo, opt, open_comm, golden=gold, inp=inp)
+    if external:
+        _, b = run_split_pair(case, algo, kind, open_comm, golden=gold)
+        ulp = l1_rel = 0.0
+    else:
+        _, b, ulp, l1_rel = run_pair(case, algo, opt, open_comm, golden=gold, inp=inp)
     assert_pads_zero(_pads(b))
     if gold is not None:
         rep = compare_with_golden(b, gold)

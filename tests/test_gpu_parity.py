@@ -368,18 +368,17 @@ def test_cpu_device_is_rejected_loudly():
 
 
 # ----------------------------------------------------------------------------- data parallel (2 GPUs)
-def _dp_worker(rank, world, port, algo, transport, q):
+def _dp_worker(rank, world, port, algo, external, q):
     import os
     import torch.distributed as dist
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
-    os.environ["RECNN_B200_COMM"] = transport
     torch.cuda.set_device(rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     try:
         gold = load_golden("%s_canon_adam.npz" % algo)
         got = run_cuda_case("canon", algo, "adam", golden=gold, form="frames", device="cuda:%d" % rank,
-                            shard=(rank, world))
+                            shard=(rank, world), external=external)
         nets = got.pop("_nets")
         got.pop("_opts")
         comm = nets["policy_net"].__dict__["_recnn_dp"][2]
@@ -407,12 +406,13 @@ def _dp_worker(rank, world, port, algo, transport, q):
 
 
 @pytest.mark.parametrize("world", [2, 4, 8])
-@pytest.mark.parametrize("transport", ["peer", "nccl"])
+@pytest.mark.parametrize("external", [False, True], ids=["peer", "peer_torch_optim"])
 @pytest.mark.parametrize("algo", ["ddpg", "td3"])
-def test_data_parallel_equals_reference(algo, transport, world):
-    """Rows sharded over `world` ranks + gradient all-reduce == the single-process reference (golden),
-    and the replicas stay bit-identical.  transport: the in-graph NVLink peer-memory all-reduce
-    (recnn_comm_*: two-shot, fused with the optimizer and the loss sums) or NCCL calls between the phases.
+def test_data_parallel_equals_reference(algo, external, world):
+    """Rows sharded over `world` ranks + gradient all-reduce over the NVLink peer communicator (recnn_comm_*:
+    two-shot) == the single-process reference (golden), and the replicas stay bit-identical.  Built-in
+    optimizers run the all-reduces inside the one-call step, fused with the optimizer and the loss sums;
+    external torch optimizers (``external``) run the step phase by phase with the all-reduces between the phases.
     The canonical case has 32 rows: 16 / 8 / 4 rows per rank."""
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
@@ -421,7 +421,7 @@ def test_data_parallel_equals_reference(algo, transport, world):
     s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    procs = [ctx.Process(target=_dp_worker, args=(r, world, port, algo, transport, q)) for r in range(world)]
+    procs = [ctx.Process(target=_dp_worker, args=(r, world, port, algo, external, q)) for r in range(world)]
     for p in procs:
         p.start()
     res = dict(q.get(timeout=300) for _ in range(world))
@@ -430,7 +430,7 @@ def test_data_parallel_equals_reference(algo, transport, world):
         assert p.exitcode == 0
     gold = load_golden("%s_canon_adam.npz" % algo)
     for rank in range(world):
-        assert bool(res[rank].pop("_peer_comm")) == (transport == "peer"), "wrong all-reduce transport was used"
+        assert bool(res[rank].pop("_peer_comm")), "no peer communicator was used"
         compare_with_golden(res[rank], gold, check_grads=False)
     for rank in range(1, world):
         for k in res[0]:
